@@ -275,6 +275,14 @@ bank_pipe_kernel(const __grid_constant__ PipeParams P, const BankArgs a) {
     const bool want_e = alive && a.energies != nullptr;
     float *eout0 = a.energies ? a.energies + (size_t)ch0 * a.e_stride : nullptr;
     const int fdelta = P.fdelta;
+    // dB weighting of the bands this lane emits at a flush, loaded once instead of at every flush
+    constexpr int NWT = (BANK_MAX_OCT * BPO + HW - 1) / HW;
+    float wreg[NWT];
+#pragma unroll
+    for (int t = 0; t < NWT; t++) {
+        const int i = hl + HW * t;
+        wreg[t] = (a.db && a.weight && i < nbands) ? __ldg(a.weight + i) : 0.f;
+    }
 
     // ---- lane roles (phase A)
     const bool worker = hl < 2 * NR;
@@ -536,51 +544,76 @@ bank_pipe_kernel(const __grid_constant__ PipeParams P, const BankArgs a) {
         constexpr bool CHECK = decltype(check_tag)::value;
         const int kb = k - BSK;        // the stage-0 chunk whose band outputs were written in step k
         const bool valid0 = !CHECK || (k >= 0 && (unsigned)kb < (unsigned)n_chunks);
-        // ---- block ends (warp-uniform conditions: they depend on the step only)
+        // ---- block ends (warp-uniform conditions: they depend on the step only).  The BPO bands of a
+        // stage are reduced side by side, level by level, so that their shuffle latencies overlap
+        // instead of adding up; each band's sum is formed in the same order as a band on its own.
         if (valid0 && (((kb + 1) & nbmask) == 0)) {    // stage 0: weighted sum of its CH accumulators
             const int blk = ((kb + 1) >> lognb) - 1;
+            T val[BPO];
 #pragma unroll
             for (int b = 0; b < BPO; b++) {
-                T val = v_fma(-om0[0], acc0[b][0], acc0[b][0]);
+                val[b] = v_fma(-om0[0], acc0[b][0], acc0[b][0]);
 #pragma unroll
-                for (int q = 1; q < NSL; q++) val = v_add(val, v_fma(-om0[q], acc0[b][q], acc0[b][q]));
+                for (int q = 1; q < NSL; q++) val[b] = v_add(val[b], v_fma(-om0[q], acc0[b][q], acc0[b][q]));
+            }
 #pragma unroll
-                for (int dlt = HW / 2; dlt >= 1; dlt >>= 1) val = v_add(val, v_shfl_xor(val, dlt));
+            for (int dlt = HW / 2; dlt >= 1; dlt >>= 1) {
+#pragma unroll
+                for (int b = 0; b < BPO; b++) val[b] = v_add(val[b], v_shfl_xor(val[b], dlt));
+            }
+#pragma unroll
+            for (int b = 0; b < BPO; b++) {
 #pragma unroll
                 for (int q = 0; q < NSL; q++) {
                     v_set(acc0[b][q], 0.f, 0.f);
-                    if (hl + HW * q == CH - 1) acc0[b][q] = val;
+                    if (hl + HW * q == CH - 1) acc0[b][q] = val[b];
                 }
-                if (hl == 0)
-                    sEN[(blk & (EN_RING - 1)) * 32 + (n_oct - 1) * BPO + b] = v_mul(P.alpha[0] * P.gband[b] * P.gband[b], val);
+            }
+            if (hl == 0) {
+#pragma unroll
+                for (int b = 0; b < BPO; b++)
+                    sEN[(blk & (EN_RING - 1)) * 32 + (n_oct - 1) * BPO + b] =
+                        v_mul(P.alpha[0] * P.gband[b] * P.gband[b], val[b]);
             }
         }
 #pragma unroll
         for (int j = 1; j <= LOGCH; j++) {             // chunked lower-rate stages
             const int cm = kb - DEC_DEPTH * j;
-            const bool ev = j <= n_oct - 1 && (unsigned)cm < (unsigned)n_chunks && (((cm + 1) & nbmask) == 0);
+            // the steps of the unchecked loop have every stage's chunk index in range
+            const bool ev = j <= n_oct - 1 && (!CHECK || (unsigned)cm < (unsigned)n_chunks) &&
+                            (((cm + 1) & nbmask) == 0);
             if (!ev) continue;
             const int blk = ((cm + 1) >> lognb) - 1;
             const int len = CH >> j, lo = CH - 2 * len;          // slots [lo, lo + len)
             const int kb0 = (n_oct - 1 - j) * BPO;
+            const float alj = sAl[j];
+            T val[BPO];
             if (len >= HW) {
                 // the stage fills whole registers q in [lo/HW, (lo+len)/HW): every lane takes part
 #pragma unroll
                 for (int b = 0; b < BPO; b++) {
-                    T val;
-                    v_set(val, 0.f, 0.f);
+                    v_set(val[b], 0.f, 0.f);
 #pragma unroll
                     for (int q = lo / HW; q < (lo + len) / HW; q++)
-                        val = v_add(val, v_fma(-omm[q], accm[b][q], accm[b][q]));
+                        val[b] = v_add(val[b], v_fma(-omm[q], accm[b][q], accm[b][q]));
+                }
 #pragma unroll
-                    for (int dlt = HW / 2; dlt >= 1; dlt >>= 1) val = v_add(val, v_shfl_xor(val, dlt));
+                for (int dlt = HW / 2; dlt >= 1; dlt >>= 1) {
+#pragma unroll
+                    for (int b = 0; b < BPO; b++) val[b] = v_add(val[b], v_shfl_xor(val[b], dlt));
+                }
+#pragma unroll
+                for (int b = 0; b < BPO; b++) {
 #pragma unroll
                     for (int q = lo / HW; q < (lo + len) / HW; q++) {
                         v_set(accm[b][q], 0.f, 0.f);
-                        if (hl + HW * q == lo + len - 1) accm[b][q] = val;
+                        if (hl + HW * q == lo + len - 1) accm[b][q] = val[b];
                     }
-                    if (hl == 0)
-                        sEN[(blk & (EN_RING - 1)) * 32 + kb0 + b] = v_mul(sAl[j] * P.gband[b] * P.gband[b], val);
+                }
+                if (hl == 0) {
+#pragma unroll
+                    for (int b = 0; b < BPO; b++)
+                        sEN[(blk & (EN_RING - 1)) * 32 + kb0 + b] = v_mul(alj * P.gband[b] * P.gband[b], val[b]);
                 }
             } else {
                 // the stage sits in lanes [lo % HW, lo % HW + len) of the last register
@@ -589,18 +622,26 @@ bank_pipe_kernel(const __grid_constant__ PipeParams P, const BankArgs a) {
                 const bool mine = hl >= l0 && hl < l0 + len;
 #pragma unroll
                 for (int b = 0; b < BPO; b++) {
-                    T val;
-                    v_set(val, 0.f, 0.f);
-                    if (mine) val = v_fma(-omm[q], accm[b][q], accm[b][q]);
+                    v_set(val[b], 0.f, 0.f);
+                    if (mine) val[b] = v_fma(-omm[q], accm[b][q], accm[b][q]);
+                }
 #pragma unroll
-                    for (int dlt = 1; dlt < HW / 2; dlt <<= 1) {
-                        if (dlt < len) val = v_add(val, v_shfl_xor(val, dlt));
+                for (int dlt = 1; dlt < HW / 2; dlt <<= 1) {
+                    if (dlt < len) {
+#pragma unroll
+                        for (int b = 0; b < BPO; b++) val[b] = v_add(val[b], v_shfl_xor(val[b], dlt));
                     }
-                    if (mine) {
+                }
+                if (mine) {
+#pragma unroll
+                    for (int b = 0; b < BPO; b++) {
                         v_set(accm[b][q], 0.f, 0.f);
-                        if (hl == l0 + len - 1) accm[b][q] = val;
-                        if (hl == l0)
-                            sEN[(blk & (EN_RING - 1)) * 32 + kb0 + b] = v_mul(sAl[j] * P.gband[b] * P.gband[b], val);
+                        if (hl == l0 + len - 1) accm[b][q] = val[b];
+                    }
+                    if (hl == l0) {
+#pragma unroll
+                        for (int b = 0; b < BPO; b++)
+                            sEN[(blk & (EN_RING - 1)) * 32 + kb0 + b] = v_mul(alj * P.gband[b] * P.gband[b], val[b]);
                     }
                 }
             }
@@ -612,17 +653,21 @@ bank_pipe_kernel(const __grid_constant__ PipeParams P, const BankArgs a) {
                 __syncwarp();
                 if (want_e) {
                     const int blk = (kf >> lognb) - 1;
-                    for (int i = hl; i < nbands; i += HW) {
-                        const T v = sEN[(blk & (EN_RING - 1)) * 32 + i];
-                        float e0 = v_x(v), e1 = v_y(v);
-                        if (a.db) {     // friture/octavespectrum.py:119-121: 10*log10(sp + 1e-30) + w
-                            const float w = a.weight ? __ldg(a.weight + i) : 0.f;
-                            e0 = fmaf(3.01029995663981195f, lg2_fast(e0 + 1e-30f), w);
-                            e1 = fmaf(3.01029995663981195f, lg2_fast(e1 + 1e-30f), w);
+#pragma unroll
+                    for (int t = 0; t < NWT; t++) {
+                        const int i = hl + HW * t;
+                        if (i < nbands) {
+                            const T v = sEN[(blk & (EN_RING - 1)) * 32 + i];
+                            float e0 = v_x(v), e1 = v_y(v);
+                            if (a.db) {     // friture/octavespectrum.py:119-121: 10*log10(sp + 1e-30) + w
+                                const float w = wreg[t];
+                                e0 = fmaf(3.01029995663981195f, lg2_fast(e0 + 1e-30f), w);
+                                e1 = fmaf(3.01029995663981195f, lg2_fast(e1 + 1e-30f), w);
+                            }
+                            float *o = eout0 + (size_t)blk * nbands + i;
+                            o[0] = e0;
+                            if (PACK == 2 && has2) o[a.e_stride] = e1;
                         }
-                        float *o = eout0 + (size_t)blk * nbands + i;
-                        o[0] = e0;
-                        if (PACK == 2 && has2) o[a.e_stride] = e1;
                     }
                 }
             }
