@@ -78,6 +78,8 @@ SIGNATURES = {
     "frt_firbank_plan": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "frt_firbank_reset": (c_int, [c_void_p]),
     "frt_firbank_process": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_void_p, c_int64, c_void_p]),
+    "frt_firbank_set_smoothing": (c_int, [c_void_p, c_void_p, c_void_p]),
+    "frt_firbank_levels": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p, c_int, c_void_p]),
     "frt_gcc_plan": (c_int, [c_void_p, c_int]),
     "frt_gcc_phat": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_void_p, c_void_p, c_int,
                              c_void_p, c_void_p, c_void_p]),

@@ -7,9 +7,19 @@
 //     stage j:  y_i = (x_j * h_i)[0:N_j]  (i = bpo-1 .. 0),   x_{j+1} = (x_j * h_dec)[0:N_j:2]
 // This is the parity mode for callers that want the live path's exact output (it differs from
 // the IIR designs it approximates by ~5e-4 on band energy); the throughput path is the IIR bank
-// of bank.cu / bank_pipe.cu.  One CTA per channel, the taps and the stage signal in shared memory,
-// double-precision accumulation (512-term sums with heavy cancellation in the stop bands).
+// of bank.cu / bank_pipe.cu.  One CTA per channel, the taps, the stage signal and every stage's
+// input history in shared memory, double-precision accumulation (512-term sums with heavy
+// cancellation in the stop bands).
+//
+// One kernel serves two entry points:
+//   frt_firbank_process  one block, the ragged band outputs y (the literal `.filter()` contract);
+//   frt_firbank_levels   n_blocks blocks in one launch, no y: per block and band the octave widget's
+//                        smoothed level (friture/octavespectrum.py:101-121), accumulated in float64
+//                        from the squared double accumulators.
+// Each output is one double fma chain over k = 0..L-1, whatever the entry point or the blocking, so
+// y is the same on both paths and any cut of a stream into launches gives the same bits.
 #include <cmath>
+#include <vector>
 
 #include "frt_internal.cuh"
 
@@ -17,74 +27,228 @@ namespace {
 
 constexpr int FIR_MAX_OCT = 10;
 constexpr int FIR_THREADS = 256;
+constexpr int FIR_WARPS = FIR_THREADS / 32;
 constexpr int FIR_MAX_BLOCK = 4096;
+constexpr int FIR_R = 4;    // consecutive outputs per thread (larger banks): each broadcast tap feeds FIR_R chains
+constexpr int FIR_F = 4;    // filters per thread: each input sample feeds FIR_F chains
+constexpr int FIR_DECAY_STRIDE = FIR_MAX_BLOCK + 1;   // decay table row: (1-alpha_j)^m, m = 0..4096
 
 struct FirArgs {
     const float *x;
     long long x_stride;
-    int n_samples;           // per channel in this call
+    int block;               // samples per channel and block
+    int n_blocks;
     int L;                   // taps
     int bpo, n_oct;
     const double *taps;      // [bpo + 1][L]: bands 0..bpo-1, then the decimator
     float *hist;             // [C][n_oct][L-1] last inputs of every stage
-    float *y;                // ragged band outputs: channel c at y + c*y_stride, bands k = 0..nbands-1
-    long long y_stride;      //   concatenated, band k = (n_oct-1-j)*bpo + i holding n_samples >> j samples
+    float *y;                // NULL, or (n_blocks == 1) the ragged band outputs: channel c at
+    long long y_stride;      //   y + c*y_stride, band k = (n_oct-1-j)*bpo + i holding block >> j samples
+    // band levels (levels != NULL)
+    const double *alpha;     // [n_oct]
+    const double *decay;     // [n_oct][FIR_DECAY_STRIDE]
+    const float *weight_db;  // [nbands] or NULL
+    double *sp;              // [C][nbands] carried smoothed energies
+    float *levels;           // [C][n_blocks][nbands]
+    int db;
 };
 
-__global__ void __launch_bounds__(FIR_THREADS) fir_bank_kernel(const FirArgs a) {
-    extern __shared__ double smem_d[];
-    const int L = a.L, Lm1 = a.L - 1, nf = a.bpo + 1;
-    double *s_taps = smem_d;                                        // [nf][L]
-    float *s_x = reinterpret_cast<float *>(s_taps + (size_t)nf * L);   // [Lm1 + n_samples]
-    float *s_next = s_x + Lm1 + a.n_samples;                        // [Lm1 + n_samples/2]
-    const int c = blockIdx.x, tid = threadIdx.x;
-    for (int i = tid; i < nf * L; i += FIR_THREADS) s_taps[i] = a.taps[i];
-    float *hist = a.hist + (size_t)c * a.n_oct * Lm1;
-    for (int i = tid; i < Lm1; i += FIR_THREADS) s_x[i] = hist[i];
-    const float *xc = a.x + (size_t)c * a.x_stride;
-    for (int i = tid; i < a.n_samples; i += FIR_THREADS) s_x[Lm1 + i] = xc[i];
-    __syncthreads();
-    float *yc = a.y + (size_t)c * a.y_stride;
-    int N = a.n_samples;
-    for (int j = 0; j < a.n_oct; j++) {
-        // offset of band (j, i = 0) in the ragged layout: stages j' > j first (they are shorter)
-        long long off = 0;
-        for (int jj = a.n_oct - 1; jj > j; jj--) off += (long long)a.bpo * (a.n_samples >> jj);
-        const bool last = (j + 1 == a.n_oct);
-        if (!last)
-            for (int i = tid; i < Lm1; i += FIR_THREADS) s_next[i] = hist[(size_t)(j + 1) * Lm1 + i];
-        for (int n = tid; n < N; n += FIR_THREADS) {
-            const float *xp = s_x + Lm1 + n;          // xp[-k] = x_j[n - k]
-            for (int f0 = 0; f0 < nf; f0 += 4) {
-                double acc0 = 0.0, acc1 = 0.0, acc2 = 0.0, acc3 = 0.0;
-                const double *t0 = s_taps + (size_t)f0 * L;
-                const int nv = nf - f0;
-                for (int k = 0; k < L; k++) {
-                    const double xv = (double)xp[-k];
-                    acc0 = fma(t0[k], xv, acc0);
-                    if (nv > 1) acc1 = fma(t0[L + k], xv, acc1);
-                    if (nv > 2) acc2 = fma(t0[2 * L + k], xv, acc2);
-                    if (nv > 3) acc3 = fma(t0[3 * L + k], xv, acc3);
-                }
-                const double accs[4] = {acc0, acc1, acc2, acc3};
+__host__ __device__ inline int round4(int n) { return (n + 3) & ~3; }
+
+// Shared-memory layout, in bytes from the (16-byte aligned) dynamic base.  The stage buffers put
+// x_j[0] at float index P = round4(L) so that the float4 input loads of the convolution are aligned;
+// x_j[-(L-1)..-1] (the history) sits just below it.
+struct FirSmem {
+    int P;
+    size_t taps, red, sp, hist, xa, xb, total;
+    __host__ __device__ FirSmem(int L, int bpo, int n_oct, int block) {
+        const int nf = bpo + 1, nbands = bpo * n_oct;
+        P = round4(L);
+        taps = 0;
+        red = taps + sizeof(double) * (size_t)((nf * L + 1) & ~1);
+        sp = red + sizeof(double) * FIR_WARPS * FIR_F;
+        hist = sp + sizeof(double) * (size_t)((nbands + 1) & ~1);
+        xa = hist + sizeof(float) * (size_t)round4(n_oct * (L - 1));
+        xb = xa + sizeof(float) * (size_t)(P + round4(block) + FIR_R);
+        total = xb + sizeof(float) * (size_t)(P + round4(block / 2) + FIR_R);
+    }
+};
+
+// R consecutive outputs n0.. of FIR_F filters (nv of them valid) of one stage:
+// acc[r][q] = sum_k t[q*L + k] * xs[n0 + r - k], one fma chain per output in k order.
+// R = 4 reuses each broadcast tap for four outputs (n0 % 4 == 0, aligned float4 input loads);
+// R = 1 keeps four times as many threads busy, for banks of at most two filter groups.
+template <int R>
+__device__ __forceinline__ void fir_tile(const double *__restrict__ t, int L, int nv,
+                                         const float *__restrict__ xs, int n0,
+                                         double (&acc)[R][FIR_F]) {
 #pragma unroll
-                for (int q = 0; q < 4; q++) {
-                    const int f = f0 + q;
-                    if (f < a.bpo) yc[off + (long long)f * N + n] = (float)accs[q];
-                    else if (f == a.bpo && !last && !(n & 1)) s_next[Lm1 + (n >> 1)] = (float)accs[q];
-                }
+    for (int r = 0; r < R; r++)
+#pragma unroll
+        for (int q = 0; q < FIR_F; q++) acc[r][q] = 0.0;
+    if constexpr (R == 1) {
+        for (int k = 0; k < L; k++) {
+            const double xv = (double)xs[n0 - k];
+#pragma unroll
+            for (int q = 0; q < FIR_F; q++)
+                if (q < nv) acc[0][q] = fma(t[q * L + k], xv, acc[0][q]);
+        }
+        return;
+    }
+    // w[4 + d] = x[n0 - k0 + d], d = -4..3: the window of the current group of four taps
+    double w[8];
+    {
+        const float4 v = *reinterpret_cast<const float4 *>(xs + n0);
+        w[4] = v.x; w[5] = v.y; w[6] = v.z; w[7] = v.w;
+    }
+    const int L4 = L & ~3;
+    for (int k0 = 0; k0 < L4; k0 += 4) {
+        const float4 v = *reinterpret_cast<const float4 *>(xs + n0 - k0 - 4);
+        w[0] = v.x; w[1] = v.y; w[2] = v.z; w[3] = v.w;
+#pragma unroll
+        for (int kk = 0; kk < 4; kk++) {
+            const int k = k0 + kk;
+            double tq[FIR_F];
+#pragma unroll
+            for (int q = 0; q < FIR_F; q++) tq[q] = (q < nv) ? t[q * L + k] : 0.0;
+#pragma unroll
+            for (int r = 0; r < R; r++) {
+                const double xv = w[4 + r - kk];
+#pragma unroll
+                for (int q = 0; q < FIR_F; q++)
+                    if (q < nv) acc[r][q] = fma(tq[q], xv, acc[r][q]);
             }
         }
-        __syncthreads();
-        // this stage's new history = its last L-1 inputs
-        for (int i = tid; i < Lm1; i += FIR_THREADS) hist[(size_t)j * Lm1 + i] = s_x[N + i];
-        __syncthreads();
-        if (last) break;
-        float *t = s_x;
-        s_x = s_next;
-        s_next = t;
-        N >>= 1;
+#pragma unroll
+        for (int d = 0; d < 4; d++) w[4 + d] = w[d];
     }
+    for (int k = L4; k < L; k++) {
+        double tq[FIR_F];
+#pragma unroll
+        for (int q = 0; q < FIR_F; q++) tq[q] = (q < nv) ? t[q * L + k] : 0.0;
+#pragma unroll
+        for (int r = 0; r < R; r++) {
+            const double xv = (double)xs[n0 + r - k];
+#pragma unroll
+            for (int q = 0; q < FIR_F; q++)
+                if (q < nv) acc[r][q] = fma(tq[q], xv, acc[r][q]);
+        }
+    }
+}
+
+template <int R>
+__global__ void __launch_bounds__(FIR_THREADS, R == 1 ? 4 : 2) fir_bank_kernel(const FirArgs a) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    const int L = a.L, Lm1 = a.L - 1, nf = a.bpo + 1, nbands = a.bpo * a.n_oct;
+    const FirSmem lay(L, a.bpo, a.n_oct, a.block);
+    const int P = lay.P;
+    double *s_taps = reinterpret_cast<double *>(smem_raw + lay.taps);   // [nf][L]
+    double *s_red = reinterpret_cast<double *>(smem_raw + lay.red);     // [FIR_WARPS][FIR_F]
+    double *s_sp = reinterpret_cast<double *>(smem_raw + lay.sp);       // [nbands]
+    float *s_hist = reinterpret_cast<float *>(smem_raw + lay.hist);     // [n_oct][Lm1]
+    float *s_xa = reinterpret_cast<float *>(smem_raw + lay.xa);         // stages 0, 2, 4, ...
+    float *s_xb = reinterpret_cast<float *>(smem_raw + lay.xb);         // stages 1, 3, 5, ...
+    const int c = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const bool levels = a.levels != nullptr;
+
+    for (int i = tid; i < nf * L; i += FIR_THREADS) s_taps[i] = a.taps[i];
+    float *hist = a.hist + (size_t)c * a.n_oct * Lm1;
+    for (int i = tid; i < a.n_oct * Lm1; i += FIR_THREADS) s_hist[i] = hist[i];
+    if (levels)
+        for (int i = tid; i < nbands; i += FIR_THREADS) s_sp[i] = a.sp[(size_t)c * nbands + i];
+    // the padding the float4 loads may touch (never used by an output) starts out finite
+    for (int i = tid; i < (int)((lay.total - lay.xa) / sizeof(float)); i += FIR_THREADS) s_xa[i] = 0.f;
+    __syncthreads();
+
+    // filters are processed FIR_F at a time: group g = filters g*FIR_F.., served by wpg warps
+    const int n_groups = (nf + FIR_F - 1) / FIR_F;
+    const int wpg = FIR_WARPS / n_groups >= 1 ? FIR_WARPS / n_groups : 1;
+    const int g = warp / wpg;
+    const int tig = tid - g * wpg * 32, tpg = wpg * 32;
+    const int nv = min(FIR_F, nf - g * FIR_F);
+
+    for (int b = 0; b < a.n_blocks; b++) {
+        float *sx = s_xa, *sn = s_xb;
+        int N = a.block;
+        long long off = 0;     // ragged y: stages j' > j first (they are shorter)
+        for (int jj = a.n_oct - 1; jj > 0; jj--) off += (long long)a.bpo * (a.block >> jj);
+        for (int j = 0; j < a.n_oct; j++) {
+            const bool last = (j + 1 == a.n_oct);
+            float *xs = sx + P;                     // xs[m] = x_j[m], m = -(L-1) .. N-1
+            for (int i = tid; i < Lm1; i += FIR_THREADS) xs[i - Lm1] = s_hist[(size_t)j * Lm1 + i];
+            if (j == 0) {
+                const float *xc = a.x + (size_t)c * a.x_stride + (size_t)b * a.block;
+                for (int i = tid; i < N; i += FIR_THREADS) xs[i] = xc[i];
+            }
+            __syncthreads();
+            if (g < n_groups) {
+                const double *t = s_taps + (size_t)g * FIR_F * L;
+                const double *dec = a.decay + (size_t)j * FIR_DECAY_STRIDE;
+                double part[FIR_F] = {0.0, 0.0, 0.0, 0.0};
+                const int n_chunks = (N + R - 1) / R;
+                for (int ch = tig; ch < n_chunks; ch += tpg) {
+                    const int n0 = ch * R;
+                    double acc[R][FIR_F];
+                    fir_tile<R>(t, L, nv, xs, n0, acc);
+#pragma unroll
+                    for (int r = 0; r < R; r++) {
+                        const int n = n0 + r;
+                        if (n >= N) break;
+                        const double wn = levels ? __ldg(dec + (N - 1 - n)) : 0.0;
+#pragma unroll
+                        for (int q = 0; q < FIR_F; q++) {
+                            const int f = g * FIR_F + q;
+                            if (f < a.bpo) {
+                                if (a.y) a.y[(size_t)c * a.y_stride + off + (long long)f * N + n] = (float)acc[r][q];
+                                if (levels) part[q] = fma(wn, acc[r][q] * acc[r][q], part[q]);
+                            } else if (f == a.bpo && !last && !(n & 1)) {
+                                sn[P + (n >> 1)] = (float)acc[r][q];
+                            }
+                        }
+                    }
+                }
+                if (levels) {
+#pragma unroll
+                    for (int q = 0; q < FIR_F; q++)
+#pragma unroll
+                        for (int o = 16; o > 0; o >>= 1) part[q] += __shfl_xor_sync(0xffffffffu, part[q], o);
+                    if (lane == 0)
+#pragma unroll
+                        for (int q = 0; q < FIR_F; q++) s_red[warp * FIR_F + q] = part[q];
+                }
+            }
+            __syncthreads();
+            if (levels && tid < a.bpo) {
+                // sp <- alpha * sum_n (1-alpha)^(N-1-n) y[n]^2 + sp * (1-alpha)^N
+                // (exp_smoothed_value, friture/signal/exp_smoothing.py:40-56, with N <= its kernel)
+                const int gg = tid / FIR_F, q = tid % FIR_F;
+                double s = 0.0;
+                for (int w = 0; w < wpg; w++) s += s_red[(gg * wpg + w) * FIR_F + q];
+                const int k = (a.n_oct - 1 - j) * a.bpo + tid;
+                s_sp[k] = a.alpha[j] * s + s_sp[k] * a.decay[(size_t)j * FIR_DECAY_STRIDE + N];
+            }
+            // this stage's new history = its last L-1 inputs
+            for (int i = tid; i < Lm1; i += FIR_THREADS) s_hist[(size_t)j * Lm1 + i] = xs[N - Lm1 + i];
+            __syncthreads();
+            if (last) break;
+            float *tmp = sx;
+            sx = sn;
+            sn = tmp;
+            N >>= 1;
+            off -= (long long)a.bpo * N;
+        }
+        if (levels) {
+            float *lv = a.levels + ((size_t)c * a.n_blocks + b) * nbands;
+            for (int k = tid; k < nbands; k += FIR_THREADS) {
+                const double e = s_sp[k];
+                lv[k] = a.db ? (float)(10.0 * log10(e + 1e-30) + (a.weight_db ? (double)a.weight_db[k] : 0.0))
+                             : (float)e;
+            }
+        }
+    }
+    for (int i = tid; i < a.n_oct * Lm1; i += FIR_THREADS) hist[i] = s_hist[i];
+    if (levels)
+        for (int i = tid; i < nbands; i += FIR_THREADS) a.sp[(size_t)c * nbands + i] = s_sp[i];
 }
 
 }   // namespace
@@ -93,14 +257,28 @@ struct FirPlan {
     int n_channels = 0, bpo = 0, n_oct = 0, L = 0;
     double *taps = nullptr;
     float *hist = nullptr;
+    double *sp = nullptr;          // [C][nbands]
+    double *alpha = nullptr;       // [n_oct]
+    double *decay = nullptr;       // [n_oct][FIR_DECAY_STRIDE]
+    float *weight_db = nullptr;    // [nbands]
+    bool smoothing = false;        // frt_firbank_set_smoothing has been called
+    bool weighted = false;
 };
+
+static void fir_plan_free(FirPlan *pl) {
+    if (pl->taps) cudaFree(pl->taps);
+    if (pl->hist) cudaFree(pl->hist);
+    if (pl->sp) cudaFree(pl->sp);
+    if (pl->alpha) cudaFree(pl->alpha);
+    if (pl->decay) cudaFree(pl->decay);
+    if (pl->weight_db) cudaFree(pl->weight_db);
+    delete pl;
+}
 
 void frt_fir_release(frt_ctx *h) {
     FirPlan *pl = reinterpret_cast<FirPlan *>(h->fir);
     if (!pl) return;
-    if (pl->taps) cudaFree(pl->taps);
-    if (pl->hist) cudaFree(pl->hist);
-    delete pl;
+    fir_plan_free(pl);
     h->fir = nullptr;
 }
 
@@ -122,19 +300,23 @@ extern "C" int frt_firbank_plan(frt_handle h, int n_channels, int bands_per_octa
     pl->L = n_taps;
     const size_t nt = (size_t)(bands_per_octave + 1) * n_taps;
     const size_t nh = (size_t)n_channels * n_octaves * (n_taps - 1);
+    const size_t nb = (size_t)bands_per_octave * n_octaves;
     cudaError_t e = cudaMalloc(&pl->taps, sizeof(double) * nt);
     if (e == cudaSuccess) e = cudaMalloc(&pl->hist, sizeof(float) * nh);
+    if (e == cudaSuccess) e = cudaMalloc(&pl->sp, sizeof(double) * n_channels * nb);
+    if (e == cudaSuccess) e = cudaMalloc(&pl->alpha, sizeof(double) * n_octaves);
+    if (e == cudaSuccess) e = cudaMalloc(&pl->decay, sizeof(double) * n_octaves * FIR_DECAY_STRIDE);
+    if (e == cudaSuccess) e = cudaMalloc(&pl->weight_db, sizeof(float) * nb);
     if (e == cudaSuccess)
         e = cudaMemcpy(pl->taps, fir_band, sizeof(double) * (size_t)bands_per_octave * n_taps, cudaMemcpyHostToDevice);
     if (e == cudaSuccess)
         e = cudaMemcpy(pl->taps + (size_t)bands_per_octave * n_taps, fir_dec, sizeof(double) * n_taps,
                        cudaMemcpyHostToDevice);
     if (e == cudaSuccess) e = cudaMemset(pl->hist, 0, sizeof(float) * nh);
+    if (e == cudaSuccess) e = cudaMemset(pl->sp, 0, sizeof(double) * n_channels * nb);
     if (e == cudaSuccess) e = cudaDeviceSynchronize();
     if (e != cudaSuccess) {
-        if (pl->taps) cudaFree(pl->taps);
-        if (pl->hist) cudaFree(pl->hist);
-        delete pl;
+        fir_plan_free(pl);
         return frt_fail(h, FRT_ECUDA, "frt_firbank_plan: %s", cudaGetErrorString(e));
     }
     h->fir = pl;
@@ -147,7 +329,48 @@ extern "C" int frt_firbank_reset(frt_handle h) {
     if (!pl) return frt_fail(h, FRT_ESTATE, "frt_firbank_reset: no plan");
     DeviceGuard g(h->device);
     FRT_CUDA(h, cudaMemset(pl->hist, 0, sizeof(float) * (size_t)pl->n_channels * pl->n_oct * (pl->L - 1)));
+    FRT_CUDA(h, cudaMemset(pl->sp, 0, sizeof(double) * (size_t)pl->n_channels * pl->n_oct * pl->bpo));
     FRT_CUDA(h, cudaDeviceSynchronize());
+    return FRT_OK;
+}
+
+extern "C" int frt_firbank_set_smoothing(frt_handle h, const double *alphas, const float *weight_db) {
+    if (!h) return FRT_EINVAL;
+    FirPlan *pl = reinterpret_cast<FirPlan *>(h->fir);
+    if (!pl) return frt_fail(h, FRT_ESTATE, "frt_firbank_set_smoothing: call frt_firbank_plan first");
+    DeviceGuard g(h->device);
+    FRT_CHECK_ARG(h, alphas, "NULL alphas");
+    for (int j = 0; j < pl->n_oct; j++)
+        FRT_CHECK_ARG(h, alphas[j] > 0.0 && alphas[j] <= 1.0, "alphas must be in (0, 1]");
+    std::vector<double> decay((size_t)pl->n_oct * FIR_DECAY_STRIDE);
+    for (int j = 0; j < pl->n_oct; j++)
+        for (int m = 0; m < FIR_DECAY_STRIDE; m++)
+            decay[(size_t)j * FIR_DECAY_STRIDE + m] = std::pow(1.0 - alphas[j], (double)m);
+    FRT_CUDA(h, cudaMemcpy(pl->alpha, alphas, sizeof(double) * pl->n_oct, cudaMemcpyHostToDevice));
+    FRT_CUDA(h, cudaMemcpy(pl->decay, decay.data(), sizeof(double) * decay.size(), cudaMemcpyHostToDevice));
+    if (weight_db)
+        FRT_CUDA(h, cudaMemcpy(pl->weight_db, weight_db, sizeof(float) * (size_t)pl->n_oct * pl->bpo,
+                               cudaMemcpyHostToDevice));
+    pl->weighted = weight_db != nullptr;
+    pl->smoothing = true;
+    return FRT_OK;
+}
+
+static int fir_launch(frt_handle h, FirPlan *pl, FirArgs &a, void *stream) {
+    a.L = pl->L;
+    a.bpo = pl->bpo;
+    a.n_oct = pl->n_oct;
+    a.taps = pl->taps;
+    a.hist = pl->hist;
+    const size_t smem = FirSmem(pl->L, pl->bpo, pl->n_oct, a.block).total;
+    // a bank of one or two filter groups (bpo <= 7) leaves most threads idle at four outputs per
+    // thread: on an H100 (400 W) at 1024 channels, 512-sample blocks, 3 and 6 bands per octave ran 40 % and
+    // 20 % slower than one output per thread; 12 and 24 bands per octave ran 1.6x and 1.7x faster
+    auto kernel = pl->bpo + 1 <= 2 * FIR_F ? fir_bank_kernel<1> : fir_bank_kernel<FIR_R>;
+    FRT_CUDA(h, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kernel<<<pl->n_channels, FIR_THREADS, smem, (cudaStream_t)stream>>>(a);
+    h->launches++;
+    FRT_CUDA(h, cudaGetLastError());
     return FRT_OK;
 }
 
@@ -167,22 +390,45 @@ extern "C" int frt_firbank_process(frt_handle h, const float *x_dev, int64_t x_s
     long long need = 0;
     for (int j = 0; j < pl->n_oct; j++) need += (long long)pl->bpo * (n_samples >> j);
     FRT_CHECK_ARG(h, y_stride >= need, "y_stride smaller than the ragged output size");
-    FirArgs a;
+    FirArgs a = {};
     a.x = x_dev;
     a.x_stride = x_stride;
-    a.n_samples = n_samples;
-    a.L = pl->L;
-    a.bpo = pl->bpo;
-    a.n_oct = pl->n_oct;
-    a.taps = pl->taps;
-    a.hist = pl->hist;
+    a.block = n_samples;
+    a.n_blocks = 1;
     a.y = y_dev;
     a.y_stride = y_stride;
-    const size_t smem = sizeof(double) * (size_t)(pl->bpo + 1) * pl->L +
-                        sizeof(float) * (2 * (size_t)(pl->L - 1) + n_samples + n_samples / 2 + 8);
-    FRT_CUDA(h, cudaFuncSetAttribute(fir_bank_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    fir_bank_kernel<<<pl->n_channels, FIR_THREADS, smem, (cudaStream_t)stream>>>(a);
-    h->launches++;
-    FRT_CUDA(h, cudaGetLastError());
-    return FRT_OK;
+    return fir_launch(h, pl, a, stream);
+}
+
+extern "C" int frt_firbank_levels(frt_handle h, const float *x_dev, int64_t x_stride, int block, int n_blocks,
+                                  float *levels_dev, int db, void *stream) {
+    if (!h) return FRT_EINVAL;
+    FirPlan *pl = reinterpret_cast<FirPlan *>(h->fir);
+    if (!pl) return frt_fail(h, FRT_ESTATE, "frt_firbank_levels: call frt_firbank_plan first");
+    if (!pl->smoothing) return frt_fail(h, FRT_ESTATE, "frt_firbank_levels: call frt_firbank_set_smoothing first");
+    DeviceGuard g(h->device);
+    FRT_CHECK_ARG(h, block > 0, "block must be > 0");
+    FRT_CHECK_ARG(h, n_blocks >= 0, "negative n_blocks");
+    if (n_blocks == 0) return FRT_OK;
+    FRT_CHECK_ARG(h, block <= FIR_MAX_BLOCK, "block must be <= 4096");
+    FRT_CHECK_ARG(h, block % (1 << (pl->n_oct - 1)) == 0,
+                  "block must be a multiple of 2^(n_octaves-1) (every stage keeps its even samples)");
+    // exp_smoothed_value drops the carried value when a block is longer than its 8192/dec-tap
+    // kernel (friture/signal/exp_smoothing.py:43-47); block <= 4096 keeps every stage clear of it
+    for (int j = 0; j < pl->n_oct; j++)
+        FRT_CHECK_ARG(h, (block >> j) <= (8192 >> j), "block longer than the smoothing kernel");
+    FRT_CHECK_ARG(h, x_dev && levels_dev, "NULL buffer");
+    FRT_CHECK_ARG(h, x_stride >= (int64_t)block * n_blocks, "x_stride smaller than block*n_blocks");
+    FirArgs a = {};
+    a.x = x_dev;
+    a.x_stride = x_stride;
+    a.block = block;
+    a.n_blocks = n_blocks;
+    a.alpha = pl->alpha;
+    a.decay = pl->decay;
+    a.weight_db = pl->weighted ? pl->weight_db : nullptr;
+    a.sp = pl->sp;
+    a.levels = levels_dev;
+    a.db = db;
+    return fir_launch(h, pl, a, stream);
 }

@@ -141,12 +141,27 @@ int frt_bank_set_state(frt_handle h, const float *z_host, const float *ema_host)
  * convolution, which the kernel computes directly (double accumulation), carrying the last
  * n_taps-1 inputs of every stage.  Parity mode; the IIR bank above is the throughput path.
  *   fir_band [bands_per_octave][n_taps], fir_dec [n_taps]  (float64 taps)
- *   process: n_samples <= 4096 and a multiple of 2^(n_octaves-1); y_dev ragged as in frt_bank_process */
+ *   process: n_samples <= 4096 and a multiple of 2^(n_octaves-1); y_dev ragged as in frt_bank_process
+ * plan and reset zero the filter history and the smoothed levels of frt_firbank_levels.          */
 int frt_firbank_plan(frt_handle h, int n_channels, int bands_per_octave, int n_octaves, int n_taps,
                      const double *fir_band, const double *fir_dec);
 int frt_firbank_reset(frt_handle h);
 int frt_firbank_process(frt_handle h, const float *x_dev, int64_t x_stride, int n_samples,
                         float *y_dev, int64_t y_stride, void *stream);
+/* Smoothing of the live-path band levels (OctaveSpectrum_Widget.setresponsetime / setweighting,
+ * friture/octavespectrum.py:136-156): alphas[n_octaves] per stage j (rate fs/2^j), weight_db
+ * [nbands] dB offsets added to the dB levels, or NULL for none.  Keeps the filter history and the
+ * smoothed levels, as the widget keeps its display buffers.                                     */
+int frt_firbank_set_smoothing(frt_handle h, const double *alphas, const float *weight_db);
+/* The octave widget's levels on the live-path bank (friture/octavespectrum.py:91-121): n_blocks
+ * consecutive blocks of `block` samples per channel (x[c*x_stride + b*block + n]) in one launch,
+ * no band outputs.  After every block, band k = (n_octaves-1-j)*bpo + i (N = block >> j samples):
+ *     sp_k <- alpha_j * sum_n (1-alpha_j)^(N-1-n) y_k[n]^2 + sp_k * (1-alpha_j)^N     (float64)
+ *   levels_dev  [C][n_blocks][nbands]: sp, or 10*log10(sp + 1e-30) + weight_db when db != 0
+ * block <= 4096 and a multiple of 2^(n_octaves-1); FRT_ESTATE until frt_firbank_set_smoothing.
+ * Any cut of a stream into calls gives the same bits.                                           */
+int frt_firbank_levels(frt_handle h, const float *x_dev, int64_t x_stride, int block, int n_blocks,
+                       float *levels_dev, int db, void *stream);
 
 /* ---------------------------------------------------------------- combined per-hop analysis
  * What Spectrogram_Widget.handle_new_data (friture/spectrogram.py:131-169) and
