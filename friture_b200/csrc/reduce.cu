@@ -13,16 +13,16 @@ __device__ __forceinline__ float lg2_fast(float v) {
     return r;
 }
 
-__device__ __forceinline__ void argmax_merge(float &best, int &besti, float ob, int oi) {
+__device__ __forceinline__ void argmax_merge(double &best, int &besti, double ob, int oi) {
     if (ob > best || (ob == best && oi < besti)) {
         best = ob;
         besti = oi;
     }
 }
 
-__device__ int block_argmax(float best, int besti, float *s_val, int *s_idx) {
+__device__ int block_argmax(double best, int besti, double *s_val, int *s_idx) {
     for (int o = 16; o > 0; o >>= 1) {
-        const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+        const double ob = __shfl_xor_sync(0xffffffffu, best, o);
         const int oi = __shfl_xor_sync(0xffffffffu, besti, o);
         argmax_merge(best, besti, ob, oi);
     }
@@ -38,7 +38,7 @@ __device__ int block_argmax(float best, int besti, float *s_val, int *s_idx) {
         best = l < nw ? s_val[l] : -INFINITY;
         besti = l < nw ? s_idx[l] : 0x7fffffff;
         for (int o = 16; o > 0; o >>= 1) {
-            const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+            const double ob = __shfl_xor_sync(0xffffffffu, best, o);
             const int oi = __shfl_xor_sync(0xffffffffu, besti, o);
             argmax_merge(best, besti, ob, oi);
         }
@@ -54,21 +54,26 @@ spectrum_reduce_kernel(const float *__restrict__ power, long long stride_c, long
                        const float *__restrict__ weight, float *__restrict__ db,
                        int *__restrict__ fmax_idx, int *__restrict__ pitch_idx) {
     extern __shared__ float s_sp[];   // [nbins] smoothed power of this channel
-    __shared__ float s_val[32];
+    __shared__ double s_val[32];
     __shared__ int s_idx[33];
     const int c = blockIdx.x;
     const float *p = power + (size_t)c * stride_c;
     float *d = disp + (size_t)c * nbins;
-    const float om = 1.0f - alpha;
+    const double a = alpha;
     float best = -INFINITY;
     int besti = 0x7fffffff;
     for (int k = threadIdx.x; k < nbins; k += blockDim.x) {
-        float s = d[k];
-        for (int f = 0; f < n_frames; f++)   // s <- alpha x + (1-alpha) s  (exp_smoothing.py:59-107)
-            s = fmaf(alpha, __ldg(p + (size_t)f * stride_f + k), om * s);
-        d[k] = s;
-        s_sp[k] = s;
-        float v = 3.01029995663981195f * lg2_fast(s + 1e-30f);   // spectrum.py:95-101
+        // s <- alpha x + (1-alpha) s  (exp_smoothing.py:59-107), as s + alpha (x - s) in double
+        // across the tick's frames.  In float32, (1-alpha) rounded biases the fixed point by about
+        // eps/alpha, and rounding every frame walks s off by about eps/sqrt(alpha): 1e-4 and 4e-6
+        // of the peak at N = 32, T = 5 s (alpha = 3.5e-5).  Here s is rounded once per tick.
+        double s = d[k];
+        for (int f = 0; f < n_frames; f++)
+            s = fma(a, (double)__ldg(p + (size_t)f * stride_f + k) - s, s);
+        const float sf = (float)s;
+        d[k] = sf;
+        s_sp[k] = sf;
+        float v = 3.01029995663981195f * lg2_fast(sf + 1e-30f);   // spectrum.py:95-101
         if (weight) v += __ldg(weight + k);
         db[(size_t)c * nbins + k] = v;
         if (v > best) {
@@ -77,18 +82,19 @@ spectrum_reduce_kernel(const float *__restrict__ power, long long stride_c, long
         }
     }
     const int imax = block_argmax(best, besti, s_val, s_idx);      // spectrum.py:175
-    // harmonic product spectrum, 3 harmonics (spectrum.py:103-123)
+    // harmonic product spectrum, 3 harmonics (spectrum.py:103-123), in double: a float32 product
+    // of three quiet bins (power 1e-16) underflows to 0 and the arg-max falls to index 0
     const int h = nbins / 3;
-    best = -INFINITY;
+    double bestp = -INFINITY;
     besti = 0x7fffffff;
     for (int k = threadIdx.x; k < h; k += blockDim.x) {
-        const float r = s_sp[k] * s_sp[2 * k] * s_sp[3 * k];
-        if (r > best) {
-            best = r;
+        const double r = (double)s_sp[k] * s_sp[2 * k] * s_sp[3 * k];
+        if (r > bestp) {
+            bestp = r;
             besti = k;
         }
     }
-    const int ipitch = block_argmax(best, besti, s_val, s_idx);    // spectrum.py:180
+    const int ipitch = block_argmax(bestp, besti, s_val, s_idx);   // spectrum.py:180
     if (threadIdx.x == 0) {
         fmax_idx[c] = imax;
         pitch_idx[c] = ipitch;
