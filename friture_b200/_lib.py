@@ -65,7 +65,6 @@ SIGNATURES = {
     "frt_bank_reset": (c_int, [c_void_p]),
     "frt_bank_set_weighting": (c_int, [c_void_p, c_void_p]),
     "frt_bank_schedule": (c_int, [c_int, c_int, c_int64, c_void_p, c_void_p]),
-    "frt_bank_schedule2": (c_int, [c_int, c_int, c_int, c_int64, c_void_p, c_void_p]),
     "frt_bank_process": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p,
                                  c_int64, c_int, c_void_p]),
     "frt_bank_process_strided": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p, c_int64,

@@ -655,20 +655,15 @@ extern "C" int frt_bank_set_weighting(frt_handle h, const float *weight_db_host)
     return FRT_OK;
 }
 
-extern "C" int frt_bank_schedule2(int n_octaves, int log2_chunk, int sections_per_lane, int64_t n_samples,
-                                  int *stage_start, int *n_steps) {
-    if (n_octaves < 1 || n_octaves > MAX_OCT || (log2_chunk != 5 && log2_chunk != 6) || !stage_start ||
-        n_samples < 0 || (sections_per_lane != 1 && sections_per_lane != 2))
-        return FRT_EINVAL;
-    int T[BANK_MAX_OCT + 1];
-    frt_pipe_schedule(n_octaves, log2_chunk, sections_per_lane, n_samples, T, n_steps);
-    for (int j = 0; j < MAX_OCT; j++) stage_start[j] = T[j];
-    return FRT_OK;
-}
-
 extern "C" int frt_bank_schedule(int n_octaves, int log2_chunk, int64_t n_samples, int *stage_start,
                                  int *n_steps) {
-    return frt_bank_schedule2(n_octaves, log2_chunk, 2, n_samples, stage_start, n_steps);
+    if (n_octaves < 1 || n_octaves > MAX_OCT || (log2_chunk != 5 && log2_chunk != 6) || !stage_start ||
+        n_samples < 0)
+        return FRT_EINVAL;
+    int T[BANK_MAX_OCT + 1];
+    frt_pipe_schedule(n_octaves, log2_chunk, n_samples, T, n_steps);
+    for (int j = 0; j < MAX_OCT; j++) stage_start[j] = T[j];
+    return FRT_OK;
 }
 
 extern "C" int frt_bank_state_size(frt_handle h, int64_t *z_floats, int64_t *ema_floats) {
@@ -724,11 +719,10 @@ template <int L0, bool WANT_Y>
 static cudaError_t launch_bank_y(const BankPlan *pl, const BankArgs &a, cudaStream_t st) {
     // few channels: three warps per channel (latency-bound regime); many channels: one warp
     // per channel already saturates the schedulers with less synchronisation
-    static const char *force = getenv("FRT_BANK_WARPS");
     // the three-warp kernel runs all log2(L0) scan-mode stages unconditionally: it needs more
     // octaves than that (always true for the 9- and 10-octave banks of the reference)
     const bool can_three = pl->params.n_oct > Log2<L0>::v;
-    const bool three = can_three && (force ? (force[0] == '3') : (a.n_channels < 1536 && L0 <= 16));
+    const bool three = can_three && a.n_channels < 1536 && L0 <= 16;
     if (three) return launch_bank3<L0, WANT_Y>(pl, a, st);
     const BankParams &P = pl->params;
     const int warps = 2;
@@ -820,7 +814,8 @@ static int bank_process_impl(frt_handle h, const float *x_dev, int64_t x_stride,
     // and is the fast path for the fused energies of 1- and 1/3-octave banks; the chunk-scan
     // kernels below serve the ragged band outputs (`.filter()`), 6/12/24 bands per octave and
     // block lengths that are not a power of two.  FRT_BANK_KERNEL=scan|pipe, FRT_BANK_PACK=1|2 and
-    // FRT_BANK_LOGCH=5|6 override the choice (tuning knobs).
+    // FRT_BANK_LOGCH=5|6 override the choice, so that tests reach every pipelined variant (two
+    // channels per lane, 32-sample steps) at small channel counts.
     const char *force_k = getenv("FRT_BANK_KERNEL");
     const char *force_p = getenv("FRT_BANK_PACK");
     const char *force_c = getenv("FRT_BANK_LOGCH");
@@ -834,17 +829,12 @@ static int bank_process_impl(frt_handle h, const float *x_dev, int64_t x_stride,
         // launches.
         int pack = pl->n_channels > 3072 ? 2 : 1;
         int logch = (block >= 512 && pl->n_channels <= 3072) ? 6 : 5;
-        int spl = 2;
-        const char *force_s = getenv("FRT_BANK_SPL");
         if (force_p) pack = force_p[0] == '2' ? 2 : 1;
         if (force_c) logch = force_c[0] == '6' ? 6 : 5;
-        if (force_s) spl = force_s[0] == '1' ? 1 : 2;
-        // fall back to shorter steps, then to the half-warp layout, when the block is too short for the
-        // variant's pipeline depth (frt_pipe_supported)
-        while (logch > 5 && !frt_pipe_supported(pl, block, logch, spl)) logch--;
-        if (!frt_pipe_supported(pl, block, logch, spl)) spl = 2;
-        while (logch > 5 && !frt_pipe_supported(pl, block, logch, spl)) logch--;
-        e = frt_pipe_launch(pl, a, logch, pack, spl, st);
+        // fall back to shorter steps when the block is too short for the variant's pipeline depth
+        // (frt_pipe_supported)
+        while (logch > 5 && !frt_pipe_supported(pl, block, logch)) logch--;
+        e = frt_pipe_launch(pl, a, logch, pack, st);
     } else if (tile == 1024) e = launch_bank<32>(pl, a, st);
     else if (tile == 512) e = launch_bank<16>(pl, a, st);
     else e = launch_bank<8>(pl, a, st);

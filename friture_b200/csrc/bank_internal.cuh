@@ -33,8 +33,8 @@ constexpr int PIPE_RX = 8;          // input ring depth (chunks)
 constexpr int PIPE_PF = 4;          // prefetch distance (chunks)
 
 struct PipeParams {
-    float c[PIPE_MAX_SEC], na1[PIPE_MAX_SEC], na2[PIPE_MAX_SEC];   // per section
-    float b1[PIPE_MAX_SEC], b2[PIPE_MAX_SEC];                       // c - a1, 1 - a2 (state-space input gains)
+    float na1[PIPE_MAX_SEC], na2[PIPE_MAX_SEC];   // per section: -a1, -a2
+    float b1[PIPE_MAX_SEC];                       // c - a1
     float gband[4];
     float gdec;
     float alpha[BANK_MAX_OCT + 1];
@@ -71,7 +71,7 @@ struct BankArgs {
 
 struct BankPlan {
     BankParams params;
-    PipeParams pipe[4];    // [2*(logch-5) + (2-spl)]: 32 / 64-sample steps x two / one section per lane
+    PipeParams pipe[2];    // [logch - 5]: 32 / 64-sample steps
     bool pipe_ok = false;  // the lane-pipelined kernel supports this bank
     int n_channels = 0;
     float *zstate = nullptr;
@@ -83,8 +83,7 @@ struct BankPlan {
 
 // bank_pipe.cu
 void frt_pipe_prepare(BankPlan *pl);
-void frt_pipe_schedule(int n_oct, int logch, int spl, long long t_total, int *T /*[BANK_MAX_OCT+1]*/,
-                       int *n_steps);
-int frt_pipe_flush_delta(int n_oct, int logch, int spl, const int *T);
-bool frt_pipe_supported(const BankPlan *pl, int block, int logch, int spl);
-cudaError_t frt_pipe_launch(const BankPlan *pl, BankArgs a, int logch, int pack, int spl, cudaStream_t st);
+void frt_pipe_schedule(int n_oct, int logch, long long t_total, int *T /*[BANK_MAX_OCT+1]*/, int *n_steps);
+int frt_pipe_flush_delta(int n_oct, int logch, const int *T);
+bool frt_pipe_supported(const BankPlan *pl, int block, int logch);
+cudaError_t frt_pipe_launch(const BankPlan *pl, BankArgs a, int logch, int pack, cudaStream_t st);

@@ -45,21 +45,14 @@
 
 namespace {
 
-// Two lane layouts, SPL = sections per lane:
-//   SPL = 2  one half-warp per channel (pair), roles as described above, decimator chain 3 lanes deep;
-//   SPL = 1  one WARP per channel (pair): NR = 2 bpo + 6 roles per group, role r = section r, a band is a
-//            chain of two lanes (its output trails the stage input by one step), the decimator a chain
-//            of six.  Half the arithmetic per lane and step -- but not faster: the step time of a warp is set by
-//            latencies spread over the whole step (shared-memory round trips at the segment
-//            switches, the single dependent chain of a lane, branches), not by the count of section
-//            samples per lane.  Kept as a tested variant (FRT_BANK_SPL=1); the dispatch uses SPL = 2.
-template <int SPL> struct Geo {
-    static constexpr int HW = SPL == 2 ? 16 : 32;      // lanes per channel slot
-    static constexpr int NSLOT = 32 / HW;               // channel slots per warp
-    static constexpr int DD = SPL == 2 ? 3 : 6;         // decimator chain depth in lanes = steps a stage trails its parent
-    static constexpr int BSK = SPL == 2 ? 0 : 1;        // steps the band outputs trail the stage input
-    static constexpr int RS = 2 * SPL;                  // state values per role
-};
+// One section per lane (a warp per channel, half the arithmetic per lane and step) was measured and
+// is not faster: the step time of a warp is set by latencies spread over the whole step
+// (shared-memory round trips at the segment switches, the single dependent chain of a lane,
+// branches), not by the count of section samples per lane.
+constexpr int HW = 16;              // lanes per channel slot
+constexpr int NSLOT = 32 / HW;      // channel slots per warp
+constexpr int DEC_DEPTH = 3;        // decimator chain depth in lanes = steps a stage trails its parent
+constexpr int RS = 4;               // state values per role: z1A z2A z1B z2B
 
 template <int PACK> struct VT;
 template <> struct VT<1> { using t = float; };
@@ -136,7 +129,7 @@ __device__ __forceinline__ float lg2_fast(float v) {
 // blocks of band energies staged in shared memory before the flush: a block's vector leaves fdelta
 // steps after its last stage-0 chunk, meanwhile stage 0 keeps staging newer blocks
 // (frt_pipe_supported checks that the ring is deep enough for the block length)
-template <int SPL> struct EnRing { static constexpr int N = SPL == 2 ? 8 : 16; };
+constexpr int EN_RING = 8;
 
 // The two lane groups of a half-warp must run ONE instruction stream with per-lane predicates.
 // Conditions on the (loop-invariant) group index invite the compiler to unswitch the whole
@@ -149,35 +142,15 @@ __device__ __forceinline__ bool opq(bool p) {
 }
 
 // normalised biquad step (bank_internal.cuh): y = x + z1; z1 = c x - a1 y + z2; z2 = x - a2 y.
-// FRT_PIPE_SSFORM=1 selects the state-space form with y substituted,
-//     z1' = -a1 z1 + (B1 x + z2),  z2' = -a2 z1 + B2 x,   B1 = c - a1,  B2 = 1 - a2,
-// which shortens the loop-carried path (z1 -> z1' is one FFMA) at the price of a fifth operation.
-// The step is not bound by this chain alone; default: 4-operation form.
-#ifndef FRT_PIPE_SSFORM
-#define FRT_PIPE_SSFORM 0
-#endif
-// FRT_PIPE_FUSE=1: the smoothing-accumulator updates of step k-1 are issued inside the section loops
-// of step k.
-#ifndef FRT_PIPE_FUSE
-#define FRT_PIPE_FUSE 1
-#endif
-// FRT_PIPE_EVMASK=1: one bit test per step instead of a compare-and-branch per stage for the rare
-// block-end / flush work (see `evmask` in the kernel).
-#ifndef FRT_PIPE_EVMASK
-#define FRT_PIPE_EVMASK 1
-#endif
+// The state-space form with y substituted shortens the loop-carried path (z1 -> z1' is one FFMA) at
+// the price of a fifth operation; it was measured and is not faster, the step is not bound by this
+// chain alone.
 template <class T>
-__device__ __forceinline__ T biquad(T x, T &z1, T &z2, float b1, float b2, float na1, float na2) {
+__device__ __forceinline__ T biquad(T x, T &z1, T &z2, float b1, float na1, float na2) {
     const T y = v_add(x, z1);
-#if FRT_PIPE_SSFORM
-    const T w = v_fma(b1, x, z2);
-    z2 = v_fma(na2, z1, v_mul(b2, x));
-    z1 = v_fma(na1, z1, w);
-#else
     const T t = v_fma(b1 - na1, x, z2);      // c = b1 + a1
     z1 = v_fma(na1, y, t);
     z2 = v_fma(na2, y, x);
-#endif
     return y;
 }
 
@@ -201,20 +174,16 @@ __host__ __device__ constexpr bool seg_starts_at(int slot, int ch) {
 // resident one-warp CTAs per SM the register allocation must allow (65536 / (32 * n) registers per
 // thread): the small-step variant serves many channels and wants warps, the large-step variants
 // serve few channels (one warp per scheduler at best) and want registers
-#ifndef PIPE_MINB5
-#define PIPE_MINB5 16
-#endif
-__host__ __device__ constexpr int pipe_min_blocks(int logch, int pack, int spl) {
-    return spl == 1 ? 8 : (logch == 5 && pack == 1) ? PIPE_MINB5 : (logch == 6 && pack == 1) ? 12 : 8;
+__host__ __device__ constexpr int pipe_min_blocks(int logch, int pack) {
+    return (logch == 5 && pack == 1) ? 16 : (logch == 6 && pack == 1) ? 12 : 8;
 }
 
-template <int LOGCH, int PACK, int BPO, int SPL>
+template <int LOGCH, int PACK, int BPO>
 struct PipeLayout {
     static constexpr int CH = 1 << LOGCH;
-    static constexpr int NR = (BPO + 3) * (2 / SPL);
-    static constexpr int RS = 2 * SPL;
-    static constexpr int NWR = SPL == 2 ? 12 : 2 * NR;        // writer lanes
-    static constexpr int WPAD = SPL == 2 ? 4 : (8 - NWR % 8) % 8;
+    static constexpr int NR = BPO + 3;
+    static constexpr int NWR = 12;                            // writer lanes: two groups of NR <= 6
+    static constexpr int WPAD = 4;                            // 16-byte pads after the writer regions
     static constexpr int TB = 4 * PACK;                       // bytes per T
     static constexpr int PAD = 16 / TB;                       // 16 bytes
     static constexpr int XSLOT = 2 * CH + 8 * PAD;            // ring slot: 128 B of skew + 2 vectors
@@ -223,11 +192,11 @@ struct PipeLayout {
     static constexpr int X = 0;                               // [RX][XSLOT]
     static constexpr int W = X + PIPE_RX * XSLOT;             // [NWR writer lanes][2 bufs][CH] + 16 B each
     static constexpr int WSTR = 2 * CH + PAD;
-    static constexpr int S = W + NWR * WSTR + WPAD * PAD;     // [MAX_OCT][NR][RS]: z1A z2A (z1B z2B)
+    static constexpr int S = W + NWR * WSTR + WPAD * PAD;     // [MAX_OCT][NR][RS]: z1A z2A z1B z2B
     static constexpr int ER = S + BANK_MAX_OCT * NR * RS;     // [MAX_OCT][4]: ruler-stage energies
     static constexpr int MB = ER + BANK_MAX_OCT * 4;          // [MAX_OCT + 2][2] mailboxes
     static constexpr int EN = MB + (BANK_MAX_OCT + 2) * 2;    // [EN_RING][32] staged band energies
-    static constexpr int RAW = EN + EnRing<SPL>::N * 32;
+    static constexpr int RAW = EN + EN_RING * 32;
     // round up to 64 (mod 128) bytes
     static constexpr int RAWB = RAW * TB;
     static constexpr int TOTALB = ((RAWB + 63) / 128) * 128 + 64;
@@ -235,14 +204,12 @@ struct PipeLayout {
     static_assert((NWR * WSTR + WPAD * PAD) % (8 * PAD) == 0, "state rows start on a 128-byte boundary");
 };
 
-template <int LOGCH, int PACK, int BPO, int SPL>
-__global__ void __launch_bounds__(32, pipe_min_blocks(LOGCH, PACK, SPL))
+template <int LOGCH, int PACK, int BPO>
+__global__ void __launch_bounds__(32, pipe_min_blocks(LOGCH, PACK))
 bank_pipe_kernel(const __grid_constant__ PipeParams P, const BankArgs a) {
     using T = typename VT<PACK>::t;
-    using LY = PipeLayout<LOGCH, PACK, BPO, SPL>;
-    constexpr int HW = Geo<SPL>::HW, NSLOT = Geo<SPL>::NSLOT, DEC_DEPTH = Geo<SPL>::DD, BSK = Geo<SPL>::BSK,
-                  RS = Geo<SPL>::RS;
-    constexpr int CH = 1 << LOGCH, JR = LOGCH + 1, NR = LY::NR, NSEC = SPL * NR, EN_RING = EnRing<SPL>::N;
+    using LY = PipeLayout<LOGCH, PACK, BPO>;
+    constexpr int CH = 1 << LOGCH, JR = LOGCH + 1, NR = LY::NR, NSEC = 2 * NR;
     constexpr int NSL = CH / HW;              // sample slots per lane of the channel slot (phase B)
     constexpr int NG = CH / 4;                // 4-sample groups per step
     constexpr int GB = (PACK == 1 ? 32 : 16) / 4;   // groups whose inputs are loaded ahead
@@ -288,18 +255,15 @@ bank_pipe_kernel(const __grid_constant__ PipeParams P, const BankArgs a) {
     const bool worker = hl < 2 * NR;
     const int G = (worker && hl >= NR) ? 1 : 0;
     const int r = worker ? hl - G * NR : 0;
-    const bool isband = r < BPO * (2 / SPL);
-    const int band = SPL == 2 ? r : (r >> 1);
-    const bool isout = isband && (SPL == 2 || (r & 1));      // this lane's output is the band signal
-    // skew = position in the lane chain (band: 2 lanes when SPL = 1; decimator: DEC_DEPTH lanes)
-    const int d = isband ? (SPL == 2 ? 0 : (r & 1)) : r - BPO * (2 / SPL);
+    const bool isband = r < BPO;                             // role r < BPO: band r
+    // skew = position in the lane chain (bands: one lane; decimator: DEC_DEPTH lanes)
+    const int d = isband ? 0 : r - BPO;
     const bool isdec2 = worker && (r == NR - 1);
     const bool ishead = (d == 0);                            // reads the stage input
     const int maxstage = isband ? n_oct - 1 : n_oct - 2;     // the last stage's decimator is unused (filter.py:113)
-    const float b1A = P.b1[SPL * r], b2A = P.b2[SPL * r], n1A = P.na1[SPL * r], n2A = P.na2[SPL * r];
-    const float b1B = P.b1[SPL * r + SPL - 1], b2B = P.b2[SPL * r + SPL - 1], n1B = P.na1[SPL * r + SPL - 1],
-                n2B = P.na2[SPL * r + SPL - 1];
-    const float gb_lane = isband ? P.gband[band] : 0.f;
+    const float b1A = P.b1[2 * r], n1A = P.na1[2 * r], n2A = P.na2[2 * r];
+    const float b1B = P.b1[2 * r + 1], n1B = P.na1[2 * r + 1], n2B = P.na2[2 * r + 1];
+    const float gb_lane = isband ? P.gband[r] : 0.f;
     const float gdec = P.gdec;
 
     // ---- prologue: tables, state
@@ -311,7 +275,7 @@ bank_pipe_kernel(const __grid_constant__ PipeParams P, const BankArgs a) {
     float *gz1 = a.zstate + (size_t)ch1 * n_oct * NSEC * 2;
     float *ge0 = a.ema + (size_t)ch0 * nbands;
     float *ge1 = a.ema + (size_t)ch1 * nbands;
-    for (int i = hl; i < BANK_MAX_OCT * NSEC * 2; i += HW) {    // sS[j][r][RS] == global z[j][SPL r ..][2]
+    for (int i = hl; i < BANK_MAX_OCT * NSEC * 2; i += HW) {    // sS[j][r][RS] == global z[j][2 r ..][2]
         T z;
         v_set(z, 0.f, 0.f);
         if (i < n_oct * NSEC * 2) v_set(z, gz0[i], gz1[i]);
@@ -389,26 +353,26 @@ bank_pipe_kernel(const __grid_constant__ PipeParams P, const BankArgs a) {
     // this step only reads as well.
     auto phaseA = [&](int k, auto check_tag) {
         constexpr bool CHECK = decltype(check_tag)::value;
-        const int kp = k - 1, kbp = kp - BSK;      // kbp: the stage-0 chunk whose band outputs step kp wrote
-        const bool bv0 = !CHECK || (kp >= 0 && (unsigned)kbp < (unsigned)n_chunks);
+        const int kp = k - 1;                      // step kp wrote the band outputs of stage-0 chunk kp
+        const bool bv0 = !CHECK || (kp >= 0 && (unsigned)kp < (unsigned)n_chunks);
         bool bvm[NSL];
 #pragma unroll
         for (int q = 0; q < NSL; q++) {
             bvm[q] = mok[q];
-            if (CHECK) bvm[q] = bvm[q] && kp >= 0 && (unsigned)(kbp - DEC_DEPTH * mst[q]) < (unsigned)n_chunks;
+            if (CHECK) bvm[q] = bvm[q] && kp >= 0 && (unsigned)(kp - DEC_DEPTH * mst[q]) < (unsigned)n_chunks;
         }
         const T *ybuf = sW + (kp & 1) * CH;
         constexpr int NUPD = 2 * BPO * NSL;        // accumulator updates per step
         auto bupd = [&](int i) {                   // i is a compile-time constant after unrolling
-            constexpr int OL = SPL == 2 ? 1 : 2;   // band b's output lane: OL*b + OL-1
             const int which = i & 1, q = (i >> 1) % NSL, b = (i >> 1) / NSL;
             const int p = hl + HW * q;
-            // raw units of the normalised sections; the squared chain gain is applied on emission
+            // raw units of the normalised sections; the squared chain gain is applied on emission.
+            // Band b's output is lane b's region (group 0) or lane NR + b's (group 1).
             if (which == 0) {
-                const T yv = ybuf[(OL * b + OL - 1) * LY::WSTR + p];
+                const T yv = ybuf[b * LY::WSTR + p];
                 if (bv0) acc0[b][q] = v_add(v_fma(-P.aq0, acc0[b][q], acc0[b][q]), v_sq(yv));
             } else {
-                const T yv = ybuf[(NR + OL * b + OL - 1) * LY::WSTR + p];
+                const T yv = ybuf[(NR + b) * LY::WSTR + p];
                 if (bvm[q]) accm[b][q] = v_add(v_fma(-aqm[q], accm[b][q], accm[b][q]), v_sq(yv));
             }
         };
@@ -486,15 +450,12 @@ bank_pipe_kernel(const __grid_constant__ PipeParams P, const BankArgs a) {
                             pvc = pvR;
                         }
                     }
-                    const T ya = biquad(v[q][i], cur[0], cur[1], b1A, b2A, n1A, n2A);
-                    if (SPL == 2) y[i] = biquad(ya, cur[RS - 2], cur[RS - 1], b1B, b2B, n1B, n2B);
-                    else y[i] = ya;
+                    const T ya = biquad(v[q][i], cur[0], cur[1], b1A, n1A, n2A);
+                    y[i] = biquad(ya, cur[2], cur[3], b1B, n1B, n2B);
                 }
                 const int gq = b0 + q;
-#if FRT_PIPE_FUSE
 #pragma unroll
                 for (int i = gq * NUPD / NG; i < (gq + 1) * NUPD / NG; i++) bupd(i);
-#endif
                 if (gq < NG - 1) {
                     if (!isdec2) st4(outp + 4 * gq, y);
                     else st2(xn + 2 * gq, v_mul(gdec, y[0]), v_mul(gdec, y[2]));
@@ -509,26 +470,22 @@ bank_pipe_kernel(const __grid_constant__ PipeParams P, const BankArgs a) {
                         if (gl && pvB && !(cidxB & 1)) sMB[JR * 2 + ((cidxB >> 1) & 1)] = v_mul(gdec, y[2]);
                         if (gl && pvR && !(m & 1)) sMB[(jrc + 1) * 2 + ((m >> 1) & 1)] = v_mul(gdec, y[3]);
                     }
-                    if (gl && isout) {
+                    if (gl && isband) {
                         // exp_smoothed_value of the low-rate stages: e <- (1-alpha) e + y^2 (e/alpha form)
                         const float alj = sAl[jrc];
-                        T e = sER[jrc * 4 + band];
+                        T e = sER[jrc * 4 + r];
                         e = v_add(v_fma(-alj, e, e), v_sq(y[3]));      // raw units
                         if (pvR) {
-                            sER[jrc * 4 + band] = e;
+                            sER[jrc * 4 + r] = e;
                             const int bl = logblock - jrc;           // block >> jrc = 2^bl samples
                             if (((m + 1) & ((1 << bl) - 1)) == 0)
-                                sEN[((((m + 1) >> bl) - 1) & (EN_RING - 1)) * 32 + (n_oct - 1 - jrc) * BPO + band] =
+                                sEN[((((m + 1) >> bl) - 1) & (EN_RING - 1)) * 32 + (n_oct - 1 - jrc) * BPO + r] =
                                     v_mul(alj * gb_lane * gb_lane, e);
                         }
                     }
                 }
             }
         }
-#if !FRT_PIPE_FUSE
-#pragma unroll
-        for (int i = 0; i < NUPD; i++) bupd(i);
-#endif
         const bool ge = opq(G != 0);
         if (ge && pvc) {
 #pragma unroll
@@ -542,13 +499,13 @@ bank_pipe_kernel(const __grid_constant__ PipeParams P, const BankArgs a) {
     // section loops of step k+1, which carried its accumulator updates): block ends, flush
     auto phaseB = [&](int k, auto check_tag) {
         constexpr bool CHECK = decltype(check_tag)::value;
-        const int kb = k - BSK;        // the stage-0 chunk whose band outputs were written in step k
-        const bool valid0 = !CHECK || (k >= 0 && (unsigned)kb < (unsigned)n_chunks);
+        // step k wrote the band outputs of stage-0 chunk k
+        const bool valid0 = !CHECK || (k >= 0 && (unsigned)k < (unsigned)n_chunks);
         // ---- block ends (warp-uniform conditions: they depend on the step only).  The BPO bands of a
         // stage are reduced side by side, level by level, so that their shuffle latencies overlap
         // instead of adding up; each band's sum is formed in the same order as a band on its own.
-        if (valid0 && (((kb + 1) & nbmask) == 0)) {    // stage 0: weighted sum of its CH accumulators
-            const int blk = ((kb + 1) >> lognb) - 1;
+        if (valid0 && (((k + 1) & nbmask) == 0)) {    // stage 0: weighted sum of its CH accumulators
+            const int blk = ((k + 1) >> lognb) - 1;
             T val[BPO];
 #pragma unroll
             for (int b = 0; b < BPO; b++) {
@@ -578,7 +535,7 @@ bank_pipe_kernel(const __grid_constant__ PipeParams P, const BankArgs a) {
         }
 #pragma unroll
         for (int j = 1; j <= LOGCH; j++) {             // chunked lower-rate stages
-            const int cm = kb - DEC_DEPTH * j;
+            const int cm = k - DEC_DEPTH * j;
             // the steps of the unchecked loop have every stage's chunk index in range
             const bool ev = j <= n_oct - 1 && (!CHECK || (unsigned)cm < (unsigned)n_chunks) &&
                             (((cm + 1) & nbmask) == 0);
@@ -681,16 +638,16 @@ bank_pipe_kernel(const __grid_constant__ PipeParams P, const BankArgs a) {
     // (stage j's blocks end DEC_DEPTH*j steps after stage 0's, the flush fdelta steps after): one
     // bit test per step decides whether phase B has anything to do at all, instead of one compare
     // and branch per stage (each costs a lone warp ~20 cycles of branch latency).  The mask only
-    // filters; phase B evaluates its own conditions.
+    // filters; phase B evaluates its own conditions.  Blocks of more than 64 steps do not fit the
+    // mask and run phase B at every step.
     const int NBS = nbmask + 1;
+    const bool ev_always = NBS > 64;
     unsigned long long evmask = ~0ull;
-    if (FRT_PIPE_EVMASK && NBS <= 64) {
-        evmask = 0;
-        evmask |= 1ull << (BSK & nbmask);
-        for (int j = 1; j <= LOGCH && j <= n_oct - 1; j++) evmask |= 1ull << ((BSK + DEC_DEPTH * j) & nbmask);
+    if (!ev_always) {
+        evmask = 1ull;
+        for (int j = 1; j <= LOGCH && j <= n_oct - 1; j++) evmask |= 1ull << ((DEC_DEPTH * j) & nbmask);
         evmask |= 1ull << (fdelta & nbmask);
     }
-    const bool ev_always = !(FRT_PIPE_EVMASK && NBS <= 64);
     auto iteration = [&](int k, auto check_tag) {
         constexpr bool CHECK = decltype(check_tag)::value;
         phaseA(k, check_tag);
@@ -745,28 +702,23 @@ bank_pipe_kernel(const __grid_constant__ PipeParams P, const BankArgs a) {
     }
 }
 
-template <int LOGCH, int PACK, int BPO, int SPL>
+template <int LOGCH, int PACK, int BPO>
 cudaError_t launch_pipe(const PipeParams &P, const BankArgs &a, cudaStream_t st) {
-    using LY = PipeLayout<LOGCH, PACK, BPO, SPL>;
-    const size_t smem = (size_t)LY::TB * Geo<SPL>::NSLOT * LY::TOTAL + 2 * 12 * 4;
-    auto kern = bank_pipe_kernel<LOGCH, PACK, BPO, SPL>;
+    using LY = PipeLayout<LOGCH, PACK, BPO>;
+    const size_t smem = (size_t)LY::TB * NSLOT * LY::TOTAL + 2 * 12 * 4;
+    auto kern = bank_pipe_kernel<LOGCH, PACK, BPO>;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
-    const int per_warp = Geo<SPL>::NSLOT * PACK;
+    const int per_warp = NSLOT * PACK;
     const unsigned blocks = (unsigned)((a.n_channels + per_warp - 1) / per_warp);
     kern<<<blocks, 32, smem, st>>>(P, a);
     return cudaGetLastError();
 }
 
-template <int LOGCH, int PACK, int SPL>
-cudaError_t launch_pipe_bpo(const PipeParams &P, const BankArgs &a, cudaStream_t st) {
-    if (P.bpo == 3) return launch_pipe<LOGCH, PACK, 3, SPL>(P, a, st);
-    return launch_pipe<LOGCH, PACK, 1, SPL>(P, a, st);
-}
 template <int LOGCH, int PACK>
-cudaError_t launch_pipe_spl(const PipeParams &P, const BankArgs &a, int spl, cudaStream_t st) {
-    if (spl == 1) return launch_pipe_bpo<LOGCH, PACK, 1>(P, a, st);
-    return launch_pipe_bpo<LOGCH, PACK, 2>(P, a, st);
+cudaError_t launch_pipe_bpo(const PipeParams &P, const BankArgs &a, cudaStream_t st) {
+    if (P.bpo == 3) return launch_pipe<LOGCH, PACK, 3>(P, a, st);
+    return launch_pipe<LOGCH, PACK, 1>(P, a, st);
 }
 
 }   // namespace
@@ -776,8 +728,7 @@ cudaError_t launch_pipe_spl(const PipeParams &P, const BankArgs &a, int spl, cud
 // per step, DEC_DEPTH steps (the decimator chain) behind the previous stage; stage j > logch has one
 // sample every P_j = 2^(j-logch) steps, at steps u = T_j (mod P_j) with T_j = P_j/2 - 1 (mod P_j),
 // which makes the stages' turns disjoint (the ruler sequence JR + ctz(u+1)).
-void frt_pipe_schedule(int n_oct, int logch, int spl, long long t_total, int *T, int *n_steps) {
-    const int DEC_DEPTH = spl == 1 ? Geo<1>::DD : Geo<2>::DD, BSK = spl == 1 ? Geo<1>::BSK : Geo<2>::BSK;
+void frt_pipe_schedule(int n_oct, int logch, long long t_total, int *T, int *n_steps) {
     T[0] = 0;
     for (int j = 1; j <= BANK_MAX_OCT; j++) {
         int t = T[j - 1] + DEC_DEPTH;
@@ -791,14 +742,14 @@ void frt_pipe_schedule(int n_oct, int logch, int spl, long long t_total, int *T,
     const long long n_chunks = t_total >> logch;
     long long last = 0;
     for (int j = 0; j < n_oct; j++) {
-        const int dmax = (j == n_oct - 1) ? BSK : DEC_DEPTH - 1;
+        const int dmax = (j == n_oct - 1) ? 0 : DEC_DEPTH - 1;
         long long l;
         if (j <= logch) l = n_chunks - 1 + T[j] + dmax;
         else l = T[j] + (((t_total >> j) - 1) << (j - logch)) + dmax;
         if (l > last) last = l;
     }
     // block b's band vector is flushed at step (b+1)*NB - 1 + delta
-    const long long flush_last = n_chunks - 1 + frt_pipe_flush_delta(n_oct, logch, spl, T);
+    const long long flush_last = n_chunks - 1 + frt_pipe_flush_delta(n_oct, logch, T);
     if (flush_last > last) last = flush_last;
     *n_steps = (int)(last + 1);
 }
@@ -806,37 +757,35 @@ void frt_pipe_schedule(int n_oct, int logch, int spl, long long t_total, int *T,
 // Steps after a block's last stage-0 chunk (step (b+1)*NB - 1) at which every stage has staged the
 // block's band energies: chunked stage j reports T_j steps later, ruler stage j during step
 // T_j - P_j of that scale (readable one phase later, hence + 1).
-int frt_pipe_flush_delta(int n_oct, int logch, int spl, const int *T) {
+int frt_pipe_flush_delta(int n_oct, int logch, const int *T) {
     int delta = 0;
     for (int j = 1; j < n_oct; j++) {
         const int dj = j <= logch ? T[j] : T[j] - (1 << (j - logch)) + 1;
         if (dj > delta) delta = dj;
     }
-    return delta + (spl == 1 ? Geo<1>::BSK : Geo<2>::BSK);     // band outputs trail by BSK steps
+    return delta;
 }
 
 void frt_pipe_prepare(BankPlan *pl) {
     const BankParams &B = pl->params;
     pl->pipe_ok = (B.bpo == 1 || B.bpo == 3);
     if (!pl->pipe_ok) return;
-    for (int v = 0; v < 4; v++) {
-        const int logch = 5 + (v >> 1), CH = 1 << logch, spl = 2 - (v & 1);
+    for (int v = 0; v < 2; v++) {
+        const int logch = 5 + v, CH = 1 << logch;
         PipeParams &P = pl->pipe[v];
         memset(&P, 0, sizeof(P));
         P.n_oct = B.n_oct;
         P.bpo = B.bpo;
         for (int r = 0; r < B.nsec; r++) {
-            P.c[r] = B.coef[r][1];
             P.na1[r] = -B.coef[r][3];
             P.na2[r] = -B.coef[r][4];
             P.b1[r] = B.coef[r][5];      // c - a1, rounded once from double (frt_bank_plan)
-            P.b2[r] = B.coef[r][6];      // 1 - a2
         }
         for (int b = 0; b < B.bpo; b++) P.gband[b] = B.gband[b];
         P.gdec = B.gdec;
         for (int j = 0; j <= BANK_MAX_OCT; j++) P.alpha[j] = j < B.n_oct ? (float)pl->alphas[j] : 1.f;
-        frt_pipe_schedule(B.n_oct, logch, spl, 0, P.T, nullptr);
-        P.fdelta = frt_pipe_flush_delta(B.n_oct, logch, spl, P.T);
+        frt_pipe_schedule(B.n_oct, logch, 0, P.T, nullptr);
+        P.fdelta = frt_pipe_flush_delta(B.n_oct, logch, P.T);
         const double q0 = 1.0 - pl->alphas[0];
         P.aq0 = (float)(1.0 - pow(q0, CH));
         for (int p = 0; p < CH; p++) {
@@ -853,23 +802,22 @@ void frt_pipe_prepare(BankPlan *pl) {
     }
 }
 
-bool frt_pipe_supported(const BankPlan *pl, int block, int logch, int spl) {
+bool frt_pipe_supported(const BankPlan *pl, int block, int logch) {
     if (!pl->pipe_ok || (block & (block - 1)) || block < (4 << logch)) return false;
-    const PipeParams &P = pl->pipe[2 * (logch - 5) + (2 - spl)];
+    const PipeParams &P = pl->pipe[logch - 5];
     if ((block >> (P.n_oct - 1)) < 1) return false;
     const int nb = block >> logch;                      // steps per block
-    const int ring = spl == 1 ? EnRing<1>::N : EnRing<2>::N;
     // blocks staged but not yet flushed when a block's vector leaves, plus the one being written
     // (+1: the section loops of the next step already stage energies while a block is flushed)
-    return (P.fdelta + nb - 1) / nb + 2 <= ring;
+    return (P.fdelta + nb - 1) / nb + 2 <= EN_RING;
 }
 
-cudaError_t frt_pipe_launch(const BankPlan *pl, BankArgs a, int logch, int pack, int spl, cudaStream_t st) {
-    if (!frt_pipe_supported(pl, a.block, logch, spl)) return cudaErrorInvalidConfiguration;
-    const PipeParams &P = pl->pipe[2 * (logch - 5) + (2 - spl)];
+cudaError_t frt_pipe_launch(const BankPlan *pl, BankArgs a, int logch, int pack, cudaStream_t st) {
+    if (!frt_pipe_supported(pl, a.block, logch)) return cudaErrorInvalidConfiguration;
+    const PipeParams &P = pl->pipe[logch - 5];
     int T[BANK_MAX_OCT + 1];
-    frt_pipe_schedule(P.n_oct, logch, spl, a.t_total, T, &a.n_steps);
+    frt_pipe_schedule(P.n_oct, logch, a.t_total, T, &a.n_steps);
     if (logch == 5)
-        return pack == 2 ? launch_pipe_spl<5, 2>(P, a, spl, st) : launch_pipe_spl<5, 1>(P, a, spl, st);
-    return pack == 2 ? launch_pipe_spl<6, 2>(P, a, spl, st) : launch_pipe_spl<6, 1>(P, a, spl, st);
+        return pack == 2 ? launch_pipe_bpo<5, 2>(P, a, st) : launch_pipe_bpo<5, 1>(P, a, st);
+    return pack == 2 ? launch_pipe_bpo<6, 2>(P, a, st) : launch_pipe_bpo<6, 1>(P, a, st);
 }

@@ -5,8 +5,6 @@
 // y**2, exp_smoothed_value, 10*log10 + weighting).  The stream is cut into time segments; the H2D
 // copy of segment s+1, the two kernels of segment s and the D2H copy of segment s-1 overlap.  All channels go through every launch: the filterbank's
 // parallelism is the channel axis.
-#include <cstdlib>
-
 #include "frt_internal.cuh"
 
 namespace {
@@ -102,13 +100,10 @@ extern "C" int frt_combined_process_host(frt_handle h, const float *x_host, int6
     CombPipe &p = *reinterpret_cast<CombPipe *>(h->comb);
     // the first segment's H2D and the last segment's D2H are not overlapped with anything, short
     // segments keep that exposed part small; very short ones cost more in 2-D copy rows and kernel
-    // launches than they save.  Measured at 1024 ch x 129 blocks (0.54 GB in, 0.55 GB out;
-    // tools/perf_e2e.py): 4 segments 14.8 ms, 8: 13.5, 12: 13.0, 16: 12.9, 24: 14.7, 32: 15.0
+    // launches than they save.  Measured before the H100 port (card not recorded) at 1024 ch x 129
+    // blocks (0.54 GB in, 0.55 GB out): 4 segments 14.8 ms, 8: 13.5, 12: 13.0, 16: 12.9, 24: 14.7,
+    // 32: 15.0
     int nseg = B >= 128 ? 16 : (B >= 64 ? 8 : (B >= 8 ? 4 : 1));
-    if (const char *e = getenv("FRT_COMB_NSEG")) {      // tuning knob
-        const int v = atoi(e);
-        if (v >= 1 && v <= MAX_SEG) nseg = v;
-    }
     if (nseg > B) nseg = (int)B;
     const int64_t seg_blocks = (B + nseg - 1) / nseg;
     int64_t f_done = 0;

@@ -16,7 +16,7 @@ struct StftPlan {
     float *win_dev = nullptr;      // [n_fft] symmetric Hann (audioproc.py:76-81)
     float2 *tw_dev = nullptr;      // fast path: [32][32] W_M^(k1*t); generic: [M] W_M^k
     float2 *post_dev = nullptr;    // [M/2+1] U[k] = -j*W_N^k (real-FFT split twiddles)
-    float2 *wlane_dev = nullptr;   // fast path: per-lane Hann phase factors
+    float2 *wlane_dev = nullptr;   // N = 4096/8192: per-(warp, lane) Hann phase factors
     float2 *comb_dev = nullptr;    // N = 4096/8192: [(R-1)][1024] W_M^(w k0)
     std::vector<float> win_host;
 };

@@ -21,7 +21,6 @@
 // Generic path (N = 32): one CTA per frame, Stockham radix-4 (+ one radix-2 pass when log2(M) is
 //   odd) ping-ponging between two shared-memory buffers.
 #include <cmath>
-#include <cstdlib>
 
 #include "frt_internal.cuh"
 
@@ -81,43 +80,6 @@ __device__ __forceinline__ constexpr float sin32(int i) {
                              0.19509032201612826785f};
     return t[i];
 }
-
-// cos/sin(2*pi*m/64), m = 0..15 (split-step twiddle steps W_2048^(32 m))
-[[maybe_unused]] __device__ __forceinline__ constexpr float cos64(int m) {
-    constexpr float t[16] = {1.0f, 0.99518472667219688624f, 0.98078528040323044913f,
-                             0.95694033573220886494f, 0.92387953251128675613f,
-                             0.88192126434835502971f, 0.83146961230254523708f,
-                             0.77301045336273696081f, 0.70710678118654752440f,
-                             0.63439328416364549822f, 0.55557023301960222474f,
-                             0.47139673682599764856f, 0.38268343236508977173f,
-                             0.29028467725446236764f, 0.19509032201612826785f,
-                             0.09801714032956060199f};
-    return t[m];
-}
-[[maybe_unused]] __device__ __forceinline__ constexpr float sin64(int m) {
-    constexpr float t[16] = {0.0f, 0.09801714032956060199f, 0.19509032201612826785f,
-                             0.29028467725446236764f, 0.38268343236508977173f,
-                             0.47139673682599764856f, 0.55557023301960222474f,
-                             0.63439328416364549822f, 0.70710678118654752440f,
-                             0.77301045336273696081f, 0.83146961230254523708f,
-                             0.88192126434835502971f, 0.92387953251128675613f,
-                             0.95694033573220886494f, 0.98078528040323044913f,
-                             0.99518472667219688624f};
-    return t[m];
-}
-
-// Tuning switches (default: window, twiddle and split tables from shared memory): split twiddles
-// derived from one per-lane value; Hann window computed on the fly from per-lane phase factors
-// (needs 12 warps per CTA to avoid spills).  Both move table traffic from the LSU pipe to the FMA pipe.
-#ifndef FRT_STFT_WINDOW_ON_THE_FLY
-#define FRT_STFT_WINDOW_ON_THE_FLY 0
-#endif
-#ifndef FRT_STFT_DERIVE_POST
-#define FRT_STFT_DERIVE_POST 0
-#endif
-
-// cos/sin(64 * n1 * 2*pi/2047), n1 = 0..31: the per-register part of the Hann phase (N = 2048)
-#include "hann2048_tables.inc"
 
 __host__ __device__ constexpr int brev5(int r) {
     return ((r & 1) << 4) | ((r & 2) << 2) | (r & 4) | ((r & 8) >> 2) | ((r & 16) >> 4);
@@ -221,10 +183,7 @@ __device__ __forceinline__ void fence_proxy_async() {
 // Fast path, N = 2048.
 constexpr int FAST_N = 2048;
 constexpr int FAST_M = 1024;
-#ifndef FRT_STFT_WARPS
-#define FRT_STFT_WARPS 16
-#endif
-constexpr int FAST_WARPS = FRT_STFT_WARPS;
+constexpr int FAST_WARPS = 16;
 constexpr int FAST_TILE = 32 * 33;   // padded 32x32 complex tile per warp
 constexpr int FAST_POST = 17 * 32;
 constexpr size_t FAST_SMEM =
@@ -236,8 +195,7 @@ __global__ void __launch_bounds__(FAST_WARPS * 32, 1)
 stft2048_kernel(const float *__restrict__ x, long long x_stride, long long n_frames, int hop,
                 float *__restrict__ out, long long out_stride_c, long long out_stride_f,
                 const float2 *__restrict__ win2, const float2 *__restrict__ tw,
-                const float2 *__restrict__ post, const float2 *__restrict__ wlane,
-                long long total_items) {
+                const float2 *__restrict__ post, long long total_items) {
     extern __shared__ float2 smem[];
     float2 *s_win = smem;                 // [1024]  (w[2n], w[2n+1])
     float2 *s_tw = s_win + FAST_M;        // [32][32] W_1024^(k1*t)
@@ -280,16 +238,6 @@ stft2048_kernel(const float *__restrict__ x, long long x_stride, long long n_fra
                      bar);
         }
     }
-#if FRT_STFT_WINDOW_ON_THE_FLY
-    // Hann window w[n] = 0.5 - 0.5 cos(theta n), theta = 2 pi/(N-1), n = 64 n1 + 2 t + e:
-    // cos(theta n) = cos(A) cos(B) - sin(A) sin(B) with A = 64 theta n1 (compile-time constants in
-    // the unrolled loop) and B = theta (2t + e) (4 per-lane registers) -- no table traffic.
-    const float2 wcb = wlane[lane], wsb = wlane[32 + lane];   // (cos B_e), (sin B_e), e = 0, 1
-#endif
-#if FRT_STFT_DERIVE_POST
-    const float2 u_lane = s_post[lane];   // U[t] = -j W_2048^t; U[t + 32 m] = U[t] * W_64^m
-#endif
-
     long long c = (item < item_end) ? item / n_frames : 0;
     long long f = item - c * n_frames;
     for (; item < item_end; item++) {
@@ -312,18 +260,8 @@ stft2048_kernel(const float *__restrict__ x, long long x_stride, long long n_fra
                 v[n1].y = __ldg(p + 64 * n1 + 2 * lane + 1);
             }
         }
-#if FRT_STFT_WINDOW_ON_THE_FLY
-#pragma unroll
-        for (int n1 = 0; n1 < 32; n1++) {
-            const float ca = 0.5f * hann_cos_a(n1), sa = 0.5f * hann_sin_a(n1);
-            float2 wv = f2_fma(make_float2(-ca, -ca), wcb, make_float2(0.5f, 0.5f));
-            wv = f2_fma(make_float2(sa, sa), wsb, wv);
-            v[n1] = f2_mul(v[n1], wv);
-        }
-#else
 #pragma unroll
         for (int n1 = 0; n1 < 32; n1++) v[n1] = f2_mul(v[n1], s_win[32 * n1 + lane]);
-#endif
 
         dft32(v);   // v[r] = sum_n1 z[32 n1 + t] W_32^(n1 k1), k1 = brev5(r)
 #pragma unroll
@@ -361,12 +299,7 @@ stft2048_kernel(const float *__restrict__ x, long long x_stride, long long n_fra
             if (lane == 0) zp = (m == 0) ? v[0] : v[brev5(32 - m)];
             const float2 E = make_float2(z.x + zp.x, z.y - zp.y);
             const float2 O = make_float2(z.x - zp.x, z.y + zp.y);
-#if FRT_STFT_DERIVE_POST
-            const float2 T = (m == 0) ? cmul(O, u_lane)
-                                      : cmul(cmul(O, make_float2(cos64(m), -sin64(m))), u_lane);
-#else
             const float2 T = cmul(O, s_post[m * 32 + lane]);
-#endif
             const float2 X = cadd(E, T);
             const float2 Y = csub(E, T);
             const float p1 = fmaf(X.x, X.x, X.y * X.y);
@@ -935,7 +868,7 @@ void launch_fast(unsigned blocks, cudaStream_t st, const float *x, long long x_s
                  const StftPlan &pl, long long total) {
     stft2048_kernel<MODE, VEC><<<blocks, FAST_WARPS * 32, FAST_SMEM, st>>>(
         x, x_stride, n_frames, hop, out, osc, osf, reinterpret_cast<const float2 *>(pl.win_dev),
-        pl.tw_dev, pl.post_dev, pl.wlane_dev, total);
+        pl.tw_dev, pl.post_dev, total);
 }
 
 template <int Q>
@@ -1069,17 +1002,6 @@ extern "C" int frt_stft_plan(frt_handle h, int n_fft) {
         const double a = 2.0 * PI * (double)k / (double)N;
         post[k] = make_float2((float)(-sin(a)), (float)(-cos(a)));
     }
-    if (N == FAST_N) {   // per-lane part of the Hann phase: cos/sin(theta (2t + e)), t = 0..31
-        std::vector<float2> wl(64);
-        const double theta = 2.0 * PI / (double)(N - 1);
-        for (int t = 0; t < 32; t++) {
-            wl[t] = make_float2((float)cos(theta * (2 * t)), (float)cos(theta * (2 * t + 1)));
-            wl[32 + t] = make_float2((float)sin(theta * (2 * t)), (float)sin(theta * (2 * t + 1)));
-        }
-        FRT_CUDA(h, cudaMalloc(&pl.wlane_dev, sizeof(float2) * 64));
-        FRT_CUDA(h, cudaMemcpy(pl.wlane_dev, wl.data(), sizeof(float2) * 64,
-                               cudaMemcpyHostToDevice));
-    }
     if (N == 4096 || N == 8192) {   // stft_large_kernel: per-(warp, lane) part of the Hann phase
         const int R = N / 2048;
         std::vector<float> wl((size_t)R * 32 * 4);
@@ -1162,8 +1084,7 @@ extern "C" int frt_stft_process(frt_handle h, const float *x_dev, int64_t x_stri
     if (pl.n_fft == FAST_N) {
         int vec_ok = (((uintptr_t)x_dev & 7) == 0) && ((x_stride & 1) == 0) && ((hop & 1) == 0);
         // 16-byte aligned frames: let the TMA engine stage them (cp.async.bulk)
-        static const int no_tma = getenv("FRT_STFT_NO_TMA") ? 1 : 0;   // tuning knob
-        if (!no_tma && (((uintptr_t)x_dev & 15) == 0) && ((x_stride & 3) == 0) && ((hop & 3) == 0))
+        if ((((uintptr_t)x_dev & 15) == 0) && ((x_stride & 3) == 0) && ((hop & 3) == 0))
             vec_ok = 2;
         long long blocks = (total + FAST_WARPS - 1) / FAST_WARPS;
         if (blocks > h->sm_count) blocks = h->sm_count;
@@ -1197,7 +1118,7 @@ extern "C" int frt_stft_process(frt_handle h, const float *x_dev, int64_t x_stri
         }
 #undef FRT_LAUNCH_SMALL
     } else if ((pl.n_fft == 4096 || pl.n_fft == 8192) && (((uintptr_t)x_dev & 7) == 0) &&
-               ((x_stride & 1) == 0) && ((hop & 1) == 0) && !getenv("FRT_STFT_NO_LARGE")) {
+               ((x_stride & 1) == 0) && ((hop & 1) == 0)) {
         const int r = pl.n_fft / 2048, ng = LARGE_WARPS / r;
         long long blocks = (total + ng - 1) / ng;
         if (blocks > h->sm_count) blocks = h->sm_count;

@@ -103,11 +103,6 @@ int frt_bank_set_weighting(frt_handle h, const float *weight_db_host);
  * exported so that tests/bank_pipeline_model.py can check the model against the library.       */
 int frt_bank_schedule(int n_octaves, int log2_chunk, int64_t n_samples, int *stage_start,
                       int *n_steps);
-/* The same for either lane layout of the kernel: sections_per_lane = 2 (a half-warp per channel, what
- * frt_bank_schedule reports) or 1 (a warp per channel: band chains of two lanes, decimator chains of
- * six -- half the serial work per lane, the layout used for few channels).                         */
-int frt_bank_schedule2(int n_octaves, int log2_chunk, int sections_per_lane, int64_t n_samples,
-                       int *stage_start, int *n_steps);
 /* Process n_blocks consecutive blocks of `block` samples per channel
  * (x[c*x_stride + b*block + n]); block % 256 == 0 (the reference needs even lengths at every
  * stage, decimate.py:41).  State is carried across calls, so any blocking of a stream gives

@@ -7,13 +7,7 @@ kernel mirrors this file phase by phase (phase A = the lanes' biquad loops, phas
 accumulators, block-end reductions, input prefetch, mailbox copy); the tests run it against
 oracle/friture_oracle.py on CPU.
 
-Two layouts (spl = sections per lane).  spl = 2, one half-warp per channel: NR = bpo + 3 roles per
-group, two biquad sections chained per lane, decimator chain 3 lanes deep (described below).
-spl = 1, one WARP per channel: NR = 2*bpo + 6 roles per group, role r = section r, a band is a chain
-of two lanes (its output trails the stage input by one step: BSKEW = 1), the decimator a chain of
-six (DEC_DEPTH = 6) -- half the serial work per lane and step.
-
-Lanes of one channel (spl = 2: NR = bpo + 3 roles per group, two biquad sections chained per lane):
+Lanes of one channel (one half-warp; NR = bpo + 3 roles per group, two biquad sections chained per lane):
   roles [0, NR)      group 0: stage 0 (rate fs)
   roles [NR, 2*NR)   group 1: the same roles for ALL stages >= 1, time-multiplexed: in the CH sample
                      slots of one step, slots [CH-2*len_j, CH-len_j) belong to stage j
@@ -29,21 +23,13 @@ MAX_OCT = 10
 DEC_DEPTH = 3      # decimator chain = 3 lanes (2 sections each): a stage trails its parent by 3 steps
 
 
-def dec_depth(spl):
-    return DEC_DEPTH if spl == 2 else 2 * DEC_DEPTH
-
-
-def band_skew(spl):
-    return 0 if spl == 2 else 1
-
-
-def stage_start_steps(n_oct, logch, spl=2):
+def stage_start_steps(n_oct, logch):
     """T[j]: step at which the chain heads of stage j work on their first sample/chunk.
     Mirrors pipe_schedule() in bank_pipe.cu."""
     T = [0] * MAX_OCT
     jr = logch + 1
     for j in range(1, MAX_OCT):
-        t = T[j - 1] + dec_depth(spl)
+        t = T[j - 1] + DEC_DEPTH
         if j >= jr:
             P = 1 << (j - logch)
             a = P // 2 - 1
@@ -53,28 +39,28 @@ def stage_start_steps(n_oct, logch, spl=2):
     return T
 
 
-def n_steps_for(n_oct, logch, t_total, T, spl=2):
+def n_steps_for(n_oct, logch, t_total, T):
     ch = 1 << logch
     jr = logch + 1
     n_chunks = t_total // ch
     last = 0
     for j in range(n_oct):
-        dmax = band_skew(spl) if j == n_oct - 1 else dec_depth(spl) - 1
+        dmax = 0 if j == n_oct - 1 else DEC_DEPTH - 1
         if j < jr:
             last = max(last, n_chunks - 1 + T[j] + dmax)
         else:
             m_last = (t_total >> j) - 1
             last = max(last, T[j] + (m_last << (j - logch)) + dmax)
     # block b's band vector leaves the staging ring at step (b+1)*NB - 1 + flush_delta
-    return max(last, n_chunks - 1 + flush_delta(n_oct, logch, T, spl)) + 1
+    return max(last, n_chunks - 1 + flush_delta(n_oct, logch, T)) + 1
 
 
-def flush_delta(n_oct, logch, T, spl=2):
+def flush_delta(n_oct, logch, T):
     """Steps after a block's last stage-0 chunk until every stage has staged its band energies."""
     delta = 0
     for j in range(1, n_oct):
         delta = max(delta, T[j] if j <= logch else T[j] - (1 << (j - logch)) + 1)
-    return delta + band_skew(spl)
+    return delta
 
 
 def ctz(v):
@@ -88,7 +74,7 @@ def ctz(v):
 
 
 class PipeModel:
-    def __init__(self, sos_band, sos_dec, alphas, n_oct, logch=5, rx=8, pf=4, spl=2):
+    def __init__(self, sos_band, sos_dec, alphas, n_oct, logch=5, rx=8, pf=4):
         sos_band = np.asarray(sos_band, dtype=np.float64)
         sos_dec = np.asarray(sos_dec, dtype=np.float64)
         self.bpo = sos_band.shape[0]
@@ -96,11 +82,9 @@ class PipeModel:
         self.logch = logch
         self.CH = 1 << logch
         self.JR = logch + 1
-        self.spl = spl
-        self.DD, self.BSK = dec_depth(spl), band_skew(spl)
-        self.NR = (self.bpo + DEC_DEPTH) * (2 // spl)
-        self.NSEC = spl * self.NR
-        assert 2 * self.NR <= (16 if spl == 2 else 32)
+        self.NR = self.bpo + DEC_DEPTH
+        self.NSEC = 2 * self.NR
+        assert 2 * self.NR <= 16
         self.RX, self.PF = rx, pf
         self.alphas = np.ones(MAX_OCT)
         self.alphas[:n_oct] = np.asarray(alphas, dtype=np.float64)[:n_oct]
@@ -113,7 +97,7 @@ class PipeModel:
         self.a2 = secs[:, 5]
         self.g_band = np.array([sos_band[i, 0, 0] * sos_band[i, 1, 0] for i in range(self.bpo)])
         self.g_dec = float(np.prod(sos_dec[:, 0]))
-        self.T = stage_start_steps(n_oct, logch, spl)
+        self.T = stage_start_steps(n_oct, logch)
         # canonical state (normalised sections): z[n_oct][NSEC][2], e[n_oct][bpo] (e/alpha form)
         self.z = np.zeros((n_oct, self.NSEC, 2))
         self.e = np.zeros((n_oct, self.bpo))
@@ -130,14 +114,13 @@ class PipeModel:
         x = np.asarray(x, dtype=np.float64)
         CH, JR, NR, bpo, n_oct, logch = self.CH, self.JR, self.NR, self.bpo, self.n_oct, self.logch
         RX, PF, T = self.RX, self.PF, self.T
-        spl, BSK, RS = self.spl, self.BSK, 2 * self.spl
         t_total = x.shape[0]
         assert block & (block - 1) == 0 and block >= 256 and t_total % block == 0
         assert (block >> (n_oct - 1)) >= 1
         n_chunks = t_total // CH
         NB = block // CH
         n_blocks = t_total // block
-        n_steps = n_steps_for(n_oct, logch, t_total, T, spl)
+        n_steps = n_steps_for(n_oct, logch, t_total, T)
         nbands = n_oct * bpo
         energies = np.full((n_blocks, nbands), np.nan)
         # roles: lane = G*NR + r
@@ -146,10 +129,10 @@ class PipeModel:
         X = np.full((RX, 2 * CH), np.nan)
         L = np.full((NL, 2, CH), np.nan)                   # chain links (decimator lanes), 2 buffers
         BO = np.full((2, bpo, CH), np.nan)                 # band outputs of this step, per group
-        S = np.zeros((MAX_OCT, NR, RS))                    # z1A z2A (z1B z2B)
+        S = np.zeros((MAX_OCT, NR, 4))                     # z1A z2A z1B z2B
         ER = np.zeros((MAX_OCT, bpo))                      # smoothed energies of the ruler stages
         MB = np.full((MAX_OCT + 1, 2), np.nan)             # mailboxes, double-buffered by sample parity
-        S[:n_oct] = self.z.reshape(n_oct, NR, RS)
+        S[:n_oct] = self.z.reshape(n_oct, NR, 4)
         ER[:n_oct] = self.e
         acc0 = np.zeros((bpo, CH))
         accm = np.zeros((bpo, CH))
@@ -175,8 +158,6 @@ class PipeModel:
             return (n_oct - 1 - stage) * bpo + b, self.alphas[stage] * val
 
         def sec_coefs(r):
-            if spl == 1:
-                return (self.c[r], -self.a1[r], -self.a2[r], 0.0, 0.0, 0.0)
             i = 2 * r
             return (self.c[i], -self.a1[i], -self.a2[i], self.c[i + 1], -self.a1[i + 1], -self.a2[i + 1])
 
@@ -185,14 +166,8 @@ class PipeModel:
             Lnew, Xw, MBw, BOw = {}, {}, {}, {}
             for lane in range(NL):
                 g, r = divmod(lane, NR)
-                if spl == 2:
-                    isband = r < bpo
-                    band, isout = r, isband
-                    d = 0 if isband else r - bpo
-                else:
-                    isband = r < 2 * bpo
-                    band, isout = r // 2, isband and (r & 1) == 1
-                    d = (r & 1) if isband else r - 2 * bpo
+                isband = r < bpo                  # band r; decimator lane d = r - bpo of the chain
+                d = 0 if isband else r - bpo
                 isdec2 = (r == NR - 1)
                 maxstage = n_oct - 1 if isband else n_oct - 2
                 u = k - d
@@ -222,34 +197,28 @@ class PipeModel:
                     if d == 0:
                         inp[CH - 1] = MB[min(jr, MAX_OCT), m & 1] if valid else np.nan
                 for (st, ln, stage, cidx, valid) in segs:
-                    if spl == 2:
-                        z1a, z2a, z1b, z2b = S[stage, r]
-                    else:
-                        z1a, z2a = S[stage, r]
+                    z1a, z2a, z1b, z2b = S[stage, r]
                     for i in range(st, st + ln):
                         xv = inp[i]
                         ya = xv + z1a
                         z1a = n1A * ya + (cA * xv + z2a)
                         z2a = n2A * ya + xv
-                        if spl == 2:
-                            yb = ya + z1b
-                            z1b = n1B * yb + (cB * ya + z2b)
-                            z2b = n2B * yb + ya
-                            out[i] = yb
-                        else:
-                            out[i] = ya
+                        yb = ya + z1b
+                        z1b = n1B * yb + (cB * ya + z2b)
+                        z2b = n2B * yb + ya
+                        out[i] = yb
                     if valid:
-                        S[stage, r] = (z1a, z2a, z1b, z2b) if spl == 2 else (z1a, z2a)
-                    if st == CH - 1 and g == 1 and isout:
-                        yy = out[CH - 1] * self.g_band[band]
-                        e = ER[stage, band] * self.q[stage] + yy * yy
+                        S[stage, r] = (z1a, z2a, z1b, z2b)
+                    if st == CH - 1 and g == 1 and isband:
+                        yy = out[CH - 1] * self.g_band[r]
+                        e = ER[stage, r] * self.q[stage] + yy * yy
                         if valid:
-                            ER[stage, band] = e
+                            ER[stage, r] = e
                             if ((cidx + 1) & ((block >> stage) - 1)) == 0:
-                                kb, val = band_out(stage, band, e)
+                                kb, val = band_out(stage, r, e)
                                 energies[(cidx + 1) // (block >> stage) - 1, kb] = val
-                if isout:
-                    BOw[(g, band)] = out
+                if isband:
+                    BOw[(g, r)] = out
                 elif isdec2:
                     base = CH + g * (CH // 2)
                     for i in range(0, CH - 2, 2):
@@ -274,7 +243,7 @@ class PipeModel:
             for (j, par), v in MBw.items():
                 MB[j, par] = v
             # ---------------------------------------------------------------- phase B
-            c0 = k - BSK
+            c0 = k
             valid0 = 0 <= c0 < n_chunks
             for b in range(bpo):
                 y0 = BO[0, b] * self.g_band[b]
@@ -288,7 +257,7 @@ class PipeModel:
                         acc0[b] = 0.0
                         acc0[b, CH - 1] = tot
                 for j in range(1, min(JR, n_oct)):
-                    cm = k - BSK - T[j]
+                    cm = k - T[j]
                     if not (0 <= cm < n_chunks):
                         continue
                     lo, hi = CH - 2 * len_of(j), CH - len_of(j)

@@ -22,12 +22,12 @@ def _oracle_energies(bpo, n_oct, block, x, response_time=1.0):
     return np.array([orc.push(x[b * block:(b + 1) * block])[0] for b in range(len(x) // block)])
 
 
-def _model(bpo, n_oct, logch, response_time=1.0, spl=2):
+def _model(bpo, n_oct, logch, response_time=1.0):
     from friture_b200 import filter_data
     from friture_b200.octavefilters import smoothing_alphas
     _, _, sos_dec = filter_data.decimator()
     _, _, sos = filter_data.bands(bpo)
-    return PipeModel(sos, sos_dec, smoothing_alphas(response_time, n_oct), n_oct, logch=logch, spl=spl)
+    return PipeModel(sos, sos_dec, smoothing_alphas(response_time, n_oct), n_oct, logch=logch)
 
 
 @pytest.mark.parametrize("bpo,n_oct,block,T,logch", [
@@ -35,20 +35,18 @@ def _model(bpo, n_oct, logch, response_time=1.0, spl=2):
     (1, 9, 512, 2048, 5), (3, 3, 512, 1024, 5), (3, 1, 256, 1024, 5), (3, 7, 256, 1024, 6),
     (3, 9, 512, 2048, 6),
 ])
-@pytest.mark.parametrize("spl", [2, 1])
-def test_schedule_model_matches_oracle(bpo, n_oct, block, T, logch, spl):
+def test_schedule_model_matches_oracle(bpo, n_oct, block, T, logch):
     x = np.random.default_rng(bpo + n_oct + block).standard_normal(T) * 0.1
     E = _oracle_energies(bpo, n_oct, block, x)
-    got = _model(bpo, n_oct, logch, spl=spl).process(x, block)
+    got = _model(bpo, n_oct, logch).process(x, block)
     assert np.max(np.abs(got - E) / np.max(np.abs(E), axis=-1, keepdims=True)) < 1e-10
 
 
-@pytest.mark.parametrize("spl", [2, 1])
-def test_schedule_model_streaming_and_state(spl):
+def test_schedule_model_streaming_and_state():
     """Block-by-block launches (pipeline drained and refilled every time) == one launch."""
     x = np.random.default_rng(4).standard_normal(4096) * 0.1
     E = _oracle_energies(3, 9, 512, x)
-    m = _model(3, 9, 5, spl=spl)
+    m = _model(3, 9, 5)
     got = np.concatenate([m.process(x[i:i + 512], 512) for i in range(0, 4096, 512)])
     assert np.max(np.abs(got - E) / np.max(np.abs(E), axis=-1, keepdims=True)) < 1e-10
 
@@ -65,10 +63,5 @@ def test_library_schedule_matches_model():
                 Tm = stage_start_steps(n_oct, logch)
                 assert list(ss) == Tm[:10]
                 assert ns.value == n_steps_for(n_oct, logch, T, Tm)
-                for spl in (1, 2):
-                    assert lib.frt_bank_schedule2(n_oct, logch, spl, T, ss, ctypes.byref(ns)) == 0
-                    Tm = stage_start_steps(n_oct, logch, spl)
-                    assert list(ss) == Tm[:10]
-                    assert ns.value == n_steps_for(n_oct, logch, T, Tm, spl)
     assert lib.frt_bank_schedule(0, 5, 512, (ctypes.c_int * 10)(), None) != 0
     assert lib.frt_bank_schedule(9, 4, 512, (ctypes.c_int * 10)(), None) != 0

@@ -31,12 +31,10 @@ if __name__ == "__main__":
         for block, noct in ((512, 9), (1024, 10)):
             nblk = 256 if block == 512 else 128
             row = []
-            for kern, pack, logch, spl in (("pipe", 1, 5, 2), ("pipe", 2, 5, 2), ("pipe", 1, 6, 2), ("pipe", 2, 6, 2),
-                                           ("pipe", 1, 5, 1), ("pipe", 2, 5, 1), ("pipe", 1, 6, 1), ("pipe", 2, 6, 1)):
+            for kern, pack, logch in (("pipe", 1, 5), ("pipe", 2, 5), ("pipe", 1, 6), ("pipe", 2, 6)):
                 os.environ["FRT_BANK_KERNEL"] = kern
                 os.environ["FRT_BANK_PACK"] = str(pack)
                 os.environ["FRT_BANK_LOGCH"] = str(logch)
-                os.environ["FRT_BANK_SPL"] = str(spl)
                 r, ms = run(C, block, nblk, noct)
-                row.append("p%d/c%d/s%d %.3g (%.2f ms)" % (pack, 1 << logch, spl, r, ms))
+                row.append("p%d/c%d %.3g (%.2f ms)" % (pack, 1 << logch, r, ms))
             print("C=%d block=%d noct=%d nblk=%d: %s" % (C, block, noct, nblk, " | ".join(row)), flush=True)

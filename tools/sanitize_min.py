@@ -16,11 +16,9 @@ for n in (2048, 4096, 8192, 16384, 64):
     x = torch.randn(2, n + 2 * (n // 2), device="cuda") * 0.1
     p.stft(x, hop=n // 2, log=True)
     p.stft(x[:, 1:], hop=n // 2, log=False)
-for warps in ("1", "3"):
-    os.environ["FRT_BANK_WARPS"] = warps
-    for block in (256, 512, 1024):
-        Octave_Filters(3).filter_batch(torch.randn(2, block, device="cuda") * 0.1, block=block, want_y=True, db=True)
-        Octave_Filters(3).energies_batch(torch.randn(2, block, device="cuda") * 0.1, block=block)
+for block in (256, 512, 1024):      # 256 / 512: the three-warp scan kernel, 1024: the one-warp kernel
+    Octave_Filters(3).filter_batch(torch.randn(2, block, device="cuda") * 0.1, block=block, want_y=True, db=True)
+    Octave_Filters(3).energies_batch(torch.randn(2, block, device="cuda") * 0.1, block=block)
 g = GccPhat(1000)
 d0 = torch.randn(2, 1000, device="cuda")
 g.estimate(d0, torch.roll(d0, 5, 1), smooth=True, want_xcorr=True)

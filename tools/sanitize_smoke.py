@@ -16,12 +16,10 @@ for n in (2048, 1024, 64):
     p.stft(x, hop=n // 2, log=True)
     p.stft(x[:, 1:], hop=n // 2, log=False)
     p.stft_host(x.cpu().numpy(), hop=n // 2)
-for warps in ("1", "3"):
-    os.environ["FRT_BANK_WARPS"] = warps
-    for block in (256, 512, 1024):
-        bank = Octave_Filters(3)
-        x = torch.randn(3, 2 * block, device="cuda") * 0.1
-        bank.filter_batch(x, block=block, want_y=True, db=True)
+for block in (256, 512, 1024):      # 256 / 512: the three-warp scan kernel, 1024: the one-warp kernel
+    bank = Octave_Filters(3)
+    x = torch.randn(3, 2 * block, device="cuda") * 0.1
+    bank.filter_batch(x, block=block, want_y=True, db=True)
 bank = Octave_Filters(24, n_octaves=10)
 bank.energies_batch(torch.randn(2, 1024, device="cuda"), block=512)
 g = GccPhat(6000)
