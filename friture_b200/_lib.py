@@ -85,6 +85,9 @@ SIGNATURES = {
     "frt_spectrum_reduce": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int, c_int, c_int,
                                     c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                     c_void_p]),
+    "frt_spectrum_reduce_dual": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int, c_int,
+                                         c_int, c_float, c_void_p, c_void_p, c_void_p, c_void_p,
+                                         c_void_p, c_void_p]),
     "frt_decimate_plan": (c_int, [c_void_p, c_int, c_int, c_void_p]),
     "frt_decimate_process": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_int64, c_void_p]),
     "frt_display_columns": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int, c_int, c_int,

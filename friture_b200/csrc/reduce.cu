@@ -2,7 +2,8 @@
 // the frames of a tick, weighting, dB, arg-max and harmonic product spectrum, fused in one pass
 // over the power columns.  Stands behind friture/spectrum.py:158-181 (exp_smoothed_value_2d,
 // friture/signal/exp_smoothing.py:59-107; log_spectrogram spectrum.py:95-101;
-// harmonic_product_spectrum spectrum.py:103-123).
+// harmonic_product_spectrum spectrum.py:103-123), and in the widget's dual-channel mode the transfer
+// function between a reference and a measurement channel (spectrum.py:141-182).
 #include "frt_internal.cuh"
 
 namespace {
@@ -48,12 +49,42 @@ __device__ int block_argmax(double best, int besti, double *s_val, int *s_idx) {
     return s_idx[32];
 }
 
+// s <- alpha x + (1-alpha) s  (exp_smoothing.py:59-107), as s + alpha (x - s) in double across the
+// tick's frames of one bin of NCH channels side by side (their loads in flight together); the
+// carried states d are read and written back rounded to float32.  In float32, (1-alpha) rounded
+// biases the fixed point by about eps/alpha, and rounding every frame walks s off by about
+// eps/sqrt(alpha): 1e-4 and 4e-6 of the peak at N = 32, T = 5 s (alpha = 3.5e-5).  Here s is
+// rounded once per tick.
+template <int NCH>
+__device__ __forceinline__ void smooth_bin(const float *const (&p)[NCH], long long stride_f,
+                                           int n_frames, double a, float *const (&d)[NCH],
+                                           float (&out)[NCH]) {
+    double s[NCH];
+#pragma unroll
+    for (int i = 0; i < NCH; i++) s[i] = *d[i];
+    for (int f = 0; f < n_frames; f++) {
+#pragma unroll
+        for (int i = 0; i < NCH; i++)
+            s[i] = fma(a, (double)__ldg(p[i] + (size_t)f * stride_f) - s[i], s[i]);
+    }
+#pragma unroll
+    for (int i = 0; i < NCH; i++) {
+        out[i] = (float)s[i];
+        *d[i] = out[i];
+    }
+}
+
+// DUAL = false: one channel, dB = 10 log10(sp + 1e-30) + weight (spectrum.py:171).
+// DUAL = true: one (reference, measurement) pair, both smoothed, dB = 10 log10(sp2 + 1e-30) -
+// 10 log10(sp1 + 1e-30) without weighting (spectrum.py:168-169); the pitch comes from sp1 in both.
+template <bool DUAL>
 __global__ void __launch_bounds__(256)
-spectrum_reduce_kernel(const float *__restrict__ power, long long stride_c, long long stride_f,
-                       int n_frames, int nbins, float alpha, float *__restrict__ disp,
+spectrum_reduce_kernel(const float *__restrict__ power, const float *__restrict__ power2,
+                       long long stride_c, long long stride_f, int n_frames, int nbins, float alpha,
+                       float *__restrict__ disp, float *__restrict__ disp2,
                        const float *__restrict__ weight, float *__restrict__ db,
                        int *__restrict__ fmax_idx, int *__restrict__ pitch_idx) {
-    extern __shared__ float s_sp[];   // [nbins] smoothed power of this channel
+    extern __shared__ float s_sp[];   // [nbins] smoothed power of this channel (of sp1 when DUAL)
     __shared__ double s_val[32];
     __shared__ int s_idx[33];
     const int c = blockIdx.x;
@@ -63,20 +94,28 @@ spectrum_reduce_kernel(const float *__restrict__ power, long long stride_c, long
     float best = -INFINITY;
     int besti = 0x7fffffff;
     for (int k = threadIdx.x; k < nbins; k += blockDim.x) {
-        // s <- alpha x + (1-alpha) s  (exp_smoothing.py:59-107), as s + alpha (x - s) in double
-        // across the tick's frames.  In float32, (1-alpha) rounded biases the fixed point by about
-        // eps/alpha, and rounding every frame walks s off by about eps/sqrt(alpha): 1e-4 and 4e-6
-        // of the peak at N = 32, T = 5 s (alpha = 3.5e-5).  Here s is rounded once per tick.
-        double s = d[k];
-        for (int f = 0; f < n_frames; f++)
-            s = fma(a, (double)__ldg(p + (size_t)f * stride_f + k) - s, s);
-        const float sf = (float)s;
-        d[k] = sf;
-        s_sp[k] = sf;
-        float v = 3.01029995663981195f * lg2_fast(sf + 1e-30f);   // spectrum.py:95-101
-        if (weight) v += __ldg(weight + k);
+        float v;
+        if constexpr (DUAL) {
+            const float *const pk[2] = {p + k, power2 + (size_t)c * stride_c + k};
+            float *const dk[2] = {d + k, disp2 + (size_t)c * nbins + k};
+            float sp[2];
+            smooth_bin<2>(pk, stride_f, n_frames, a, dk, sp);
+            s_sp[k] = sp[0];
+            // the log of the ratio in double: two float32 dB values near -160 dB carry an ulp of
+            // 1.5e-5 dB each, and a silent reference against a loud measurement gives a ratio
+            // past the float32 range (1e10 / 1e-30)
+            v = (float)(10.0 * log10(((double)sp[1] + 1e-30) / ((double)sp[0] + 1e-30)));
+        } else {
+            const float *const pk[1] = {p + k};
+            float *const dk[1] = {d + k};
+            float sp[1];
+            smooth_bin<1>(pk, stride_f, n_frames, a, dk, sp);
+            s_sp[k] = sp[0];
+            v = 3.01029995663981195f * lg2_fast(sp[0] + 1e-30f);   // spectrum.py:95-101
+            if (weight) v += __ldg(weight + k);
+        }
         db[(size_t)c * nbins + k] = v;
-        if (v > best) {
+        if (v > best) {     // on the stored float32 value, so that db[imax] == max(db)
             best = v;
             besti = k;
         }
@@ -119,11 +158,37 @@ extern "C" int frt_spectrum_reduce(frt_handle h, const float *power_dev, int64_t
     FRT_CHECK_ARG(h, sizeof(float) * (size_t)nbins <= 200 * 1024, "nbins too large");
     const size_t smem = sizeof(float) * (size_t)nbins;
     if (smem > 48 * 1024)
-        FRT_CUDA(h, cudaFuncSetAttribute(spectrum_reduce_kernel,
+        FRT_CUDA(h, cudaFuncSetAttribute(spectrum_reduce_kernel<false>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    spectrum_reduce_kernel<<<n_channels, 256, smem, (cudaStream_t)stream>>>(
-        power_dev, stride_c, stride_f, n_frames, nbins, alpha, disp_dev, weight_dev, db_dev,
-        fmax_idx_dev, pitch_idx_dev);
+    spectrum_reduce_kernel<false><<<n_channels, 256, smem, (cudaStream_t)stream>>>(
+        power_dev, nullptr, stride_c, stride_f, n_frames, nbins, alpha, disp_dev, nullptr,
+        weight_dev, db_dev, fmax_idx_dev, pitch_idx_dev);
+    h->launches++;
+    FRT_CUDA(h, cudaGetLastError());
+    return FRT_OK;
+}
+
+extern "C" int frt_spectrum_reduce_dual(frt_handle h, const float *power1_dev,
+                                        const float *power2_dev, int64_t stride_c, int64_t stride_f,
+                                        int n_pairs, int n_frames, int nbins, float alpha,
+                                        float *disp1_dev, float *disp2_dev, float *db_dev,
+                                        int *fmax_idx_dev, int *pitch_idx_dev, void *stream) {
+    if (!h) return FRT_EINVAL;
+    DeviceGuard g(h->device);
+    FRT_CHECK_ARG(h, n_pairs >= 0 && n_frames >= 0 && nbins >= 3, "bad shape");
+    FRT_CHECK_ARG(h, n_frames <= 8192, "more frames than the reference's 8192-tap kernel");
+    FRT_CHECK_ARG(h, alpha > 0.f && alpha <= 1.f, "alpha must be in (0, 1]");
+    if (n_pairs == 0) return FRT_OK;
+    FRT_CHECK_ARG(h, (n_frames == 0 || (power1_dev && power2_dev)) && disp1_dev && disp2_dev &&
+                         db_dev && fmax_idx_dev && pitch_idx_dev, "NULL buffer");
+    FRT_CHECK_ARG(h, sizeof(float) * (size_t)nbins <= 200 * 1024, "nbins too large");
+    const size_t smem = sizeof(float) * (size_t)nbins;
+    if (smem > 48 * 1024)
+        FRT_CUDA(h, cudaFuncSetAttribute(spectrum_reduce_kernel<true>,
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    spectrum_reduce_kernel<true><<<n_pairs, 256, smem, (cudaStream_t)stream>>>(
+        power1_dev, power2_dev, stride_c, stride_f, n_frames, nbins, alpha, disp1_dev, disp2_dev,
+        nullptr, db_dev, fmax_idx_dev, pitch_idx_dev);
     h->launches++;
     FRT_CUDA(h, cudaGetLastError());
     return FRT_OK;

@@ -2,7 +2,11 @@
 framing + ``analyzelive`` per frame, exponential smoothing across the tick's frames, weighting,
 dB, peak frequency and harmonic-product-spectrum pitch -- one smoothed column per channel per
 tick instead of one column per frame (this is what the display consumes, and it shrinks what a
-multi-GPU gather has to move from ``frames x bins`` to ``bins`` per channel)."""
+multi-GPU gather has to move from ``frames x bins`` to ``bins`` per channel).
+
+With ``dual_channels`` (the widget's "Measurement type: Dual-channel", spectrum.py:141-171,286-293)
+each channel is a (reference, measurement) pair and the output is the transfer function between
+the two."""
 from __future__ import annotations
 
 from ctypes import c_float, c_void_p
@@ -19,13 +23,15 @@ OVERLAP = 0.75                 # friture/spectrum.py:66
 
 class SpectrumAnalyzer:
     def __init__(self, n_channels, fft_size=DEFAULT_FFT_SIZE, overlap=OVERLAP,
-                 response_time=DEFAULT_RESPONSE_TIME, weighting=0, handle=None):
+                 response_time=DEFAULT_RESPONSE_TIME, weighting=0, handle=None, dual_channels=False):
         self.n_channels = int(n_channels)
         self.proc = audioproc(handle)
         self.overlap = overlap
         self.weighting = weighting
         self.response_time = response_time
+        self.dual_channels = bool(dual_channels)
         self._disp = None
+        self._disp2 = None
         self._w_dev = None
         self.setfftsize(fft_size)
 
@@ -38,6 +44,7 @@ class SpectrumAnalyzer:
         self.setresponsetime(self.response_time)
         self.setweighting(self.weighting)
         self._disp = None                                            # update_display_buffers, :224-226
+        self._disp2 = None
 
     def setresponsetime(self, response_time):
         # spectrum.py:196-218: the newest n = T*fs/hop frames carry 65 % of the weight
@@ -53,17 +60,32 @@ class SpectrumAnalyzer:
         self.w = [0. * A, A, B, C][weighting]
         self._w_dev = None
 
+    def setdualchannels(self, dual_enabled):
+        """spectrum.py:286-293: changes the mode only; both smoothed states are kept."""
+        self.dual_channels = bool(dual_enabled)
+
     # -- one tick ----------------------------------------------------------------------------
     def process(self, x, stream=None):
-        """x: CUDA float32 [C, T] holding the tick's new frames (frame f = x[:, f*hop : f*hop+N]).
+        """x: CUDA float32 [C, T] holding the tick's new frames (frame f = x[:, f*hop : f*hop+N]),
+        or [C, 2, T], each channel a pair of rows: row 0 the reference, row 1 the measurement
+        (the widget's floatdata[0] and floatdata[1]).
         Returns (dB [C, bins] CUDA tensor, fmax [C] Hz, fpitch [C] Hz) after smoothing across
-        the frames, with the smoothing state carried from tick to tick."""
+        the frames, with the smoothing state carried from tick to tick.  In dual-channel mode with
+        [C, 2, T] input, dB is the transfer function 10 log10(sp2) - 10 log10(sp1), unweighted, and
+        fmax its peak; otherwise dB is 10 log10(sp1) + weighting of row 0.  The pitch always comes
+        from row 0 (spectrum.py:180)."""
         import torch
         if x.dim() == 1:
             x = x[None, :]
+        if x.dim() not in (2, 3) or (x.dim() == 3 and x.shape[1] != 2):
+            raise ValueError("expected [C, T] or [C, 2, T] input, got %s" % (tuple(x.shape),))
         C = x.shape[0]
         if C != self.n_channels:
             raise ValueError("expected %d channels" % self.n_channels)
+        if x.dim() == 3 and self.dual_channels:
+            return self._process_dual(x, stream)
+        if x.dim() == 3:
+            x = x[:, 0]
         nb = self.fft_size // 2 + 1
         nf = frame_count(x.shape[1], self.fft_size, self.hop)
         power = self.proc.stft(x, hop=self.hop, log=False, stream=stream)
@@ -79,6 +101,40 @@ class SpectrumAnalyzer:
                               int(nf), int(nb), c_float(self.alpha), _lib._ptr(self._disp),
                               _lib._ptr(self._w_dev) if self.weighting else None, _lib._ptr(db),
                               _lib._ptr(imax), _lib._ptr(ipitch), sp)
+        if self._disp2 is not None and nf > 0:
+            # the widget smooths an all-zero second column on every tick it does not fill
+            # (spectrum.py:142,158-159): dispbuffers2 * (1-alpha)^frames, on the kernel's stream
+            ts = torch.cuda.current_stream(x.device) if stream is None else \
+                torch.cuda.ExternalStream(int(stream), device=x.device)
+            with torch.cuda.stream(ts):
+                self._disp2.mul_((1. - self.alpha) ** nf)
+        return self._indices_to_hz(db, imax, ipitch)
+
+    def _indices_to_hz(self, db, imax, ipitch):
         fmax = self.freq[imax.cpu().numpy()]
         fpitch = np.maximum(self.freq[ipitch.cpu().numpy()], 1e-20)     # spectrum.py:181
         return db, fmax, fpitch
+
+    def _process_dual(self, x, stream):
+        """One STFT launch over the 2C rows, then one dual reduce over the C pairs."""
+        import torch
+        C, _, T = x.shape
+        nb = self.fft_size // 2 + 1
+        nf = frame_count(T, self.fft_size, self.hop)
+        power = self.proc.stft(x.view(2 * C, T), hop=self.hop, log=False, stream=stream)
+        if self._disp is None:
+            self._disp = torch.zeros((C, nb), dtype=torch.float32, device=x.device)
+        if self._disp2 is None:
+            self._disp2 = torch.zeros((C, nb), dtype=torch.float32, device=x.device)
+        db = torch.empty((C, nb), dtype=torch.float32, device=x.device)
+        imax = torch.empty(C, dtype=torch.int32, device=x.device)
+        ipitch = torch.empty(C, dtype=torch.int32, device=x.device)
+        sp = _lib.current_stream_ptr(x.device) if stream is None else c_void_p(int(stream))
+        # power [2C, nf, nb]: pair c's reference at row 2c, its measurement at row 2c + 1
+        p1 = power.data_ptr() if nf else 0
+        p2 = p1 + 4 * nf * nb if nf else 0
+        self.proc.handle.call("frt_spectrum_reduce_dual", _lib._ptr(p1), _lib._ptr(p2),
+                              int(2 * nf * nb), int(nb), int(C), int(nf), int(nb),
+                              c_float(self.alpha), _lib._ptr(self._disp), _lib._ptr(self._disp2),
+                              _lib._ptr(db), _lib._ptr(imax), _lib._ptr(ipitch), sp)
+        return self._indices_to_hz(db, imax, ipitch)

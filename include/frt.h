@@ -234,6 +234,21 @@ int frt_spectrum_reduce(frt_handle h, const float *power_dev, int64_t stride_c, 
                         const float *weight_dev, float *db_dev, int *fmax_idx_dev,
                         int *pitch_idx_dev, void *stream);
 
+/* The same tick in the widget's dual-channel measurement mode (friture/spectrum.py:141-182 with
+ * dual_channels set and two input channels): per pair, the reference channel (channel 0, sp1) and
+ * the measurement channel (channel 1, sp2) are both smoothed across the tick's frames, the output
+ * is the transfer function 10*log10(sp2+1e-30) - 10*log10(sp1+1e-30) with no weighting
+ * (spectrum.py:168-169), formed in double and stored as float32, fmax_idx its arg-max
+ * (spectrum.py:175) and pitch_idx the harmonic-product arg-max of sp1 (spectrum.py:180-181).
+ *   power1_dev / power2_dev [P][n_frames][nbins] with the same strides (in floats),
+ *   disp1_dev / disp2_dev [P][nbins] smoothed power in/out (the widget's dispbuffers1 and
+ *   dispbuffers2), db_dev [P][nbins], fmax_idx_dev / pitch_idx_dev [P].  Argument checks as for
+ *   frt_spectrum_reduce; n_pairs == 0 does nothing.                                             */
+int frt_spectrum_reduce_dual(frt_handle h, const float *power1_dev, const float *power2_dev,
+                             int64_t stride_c, int64_t stride_f, int n_pairs, int n_frames,
+                             int nbins, float alpha, float *disp1_dev, float *disp2_dev,
+                             float *db_dev, int *fmax_idx_dev, int *pitch_idx_dev, void *stream);
+
 /* ---------------------------------------------------------------- spectrogram display chain
  * The Transform_Pipeline behind the spectrogram (friture/spectrogram.py:161-169): scaling of
  * dB + weighting to [0,1] (spectrogram.py:127-129), Frequency_Resampler.push
