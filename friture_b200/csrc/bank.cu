@@ -20,7 +20,6 @@
 // serially over the <=32 samples, which are broadcast with shuffles.
 // Filter and smoothing state lives in shared memory while the kernel runs (global in between).
 #include <cmath>
-#include <cstdlib>
 
 #include "bank_internal.cuh"
 
@@ -70,6 +69,44 @@ struct WarpCtxT {
     int db;
     const float *weight;   // dB offsets per band (db mode) or NULL
 };
+
+// context of channel c for the scan kernels; energies and t_off are set per tile
+template <bool WANT_Y>
+__device__ __forceinline__ void channel_ctx(WarpCtxT<WANT_Y> &w, const BankParams &P, const BankArgs &a,
+                                            int c, int lane, float *s_z, float *s_e, const float *s_coef) {
+    w.P = &P;
+    w.s_z = s_z;
+    w.s_e = s_e;
+    w.s_coef = s_coef;
+    w.lane = lane;
+    w.db = a.db;
+    w.weight = a.weight;
+    w.t_total = a.t_total;
+    w.y = a.y ? a.y + (size_t)c * a.y_stride : nullptr;
+}
+
+// this lane's L0 samples of a tile
+template <int L0>
+__device__ __forceinline__ void load_tile(const float *xp, bool vec_ok, float (&xc)[L0]) {
+    if (vec_ok) {
+#pragma unroll
+        for (int k = 0; k < L0; k += 4) {
+            const float4 v = __ldg(reinterpret_cast<const float4 *>(xp + k));
+            xc[k] = v.x; xc[k + 1] = v.y; xc[k + 2] = v.z; xc[k + 3] = v.w;
+        }
+    } else {
+#pragma unroll
+        for (int k = 0; k < L0; k++) xc[k] = __ldg(xp + k);
+    }
+}
+
+// where channel c writes its band energies after tile t, or NULL when t does not end a block
+__device__ __forceinline__ float *block_energies(const BankArgs &a, int c, int t, int nbands) {
+    const bool block_end = ((t + 1) % a.tiles_per_block) == 0;
+    return (a.energies && block_end)
+               ? a.energies + (size_t)c * a.e_stride + (size_t)(t / a.tiles_per_block) * nbands
+               : nullptr;
+}
 
 // ---------------------------------------------------------------- scan-mode section
 template <int L> struct Log2 { static constexpr int v = 1 + Log2<L / 2>::v; };
@@ -348,34 +385,12 @@ bank_kernel(const __grid_constant__ BankParams P, const BankArgs a) {
     constexpr int TILE = 32 * L0;
     const int nbands = P.n_oct * P.bpo;
     WarpCtxT<WANT_Y> w;
-    w.P = &P;
-    w.s_z = s_z;
-    w.s_e = s_e;
-    w.s_coef = s_coef;
-    w.lane = lane;
-    w.db = a.db;
-    w.weight = a.weight;
-    w.t_total = a.t_total;
-    w.y = a.y ? a.y + (size_t)c * a.y_stride : nullptr;
+    channel_ctx<WANT_Y>(w, P, a, c, lane, s_z, s_e, s_coef);
     const float *xch = a.x + (size_t)c * a.x_stride;
-    const int n_blocks = a.n_tiles / a.tiles_per_block;
     for (int t = 0; t < a.n_tiles; t++) {
-        const float *xp = xch + (size_t)t * TILE + lane * L0;
         float xc[L0];
-        if (a.vec_ok) {
-#pragma unroll
-            for (int k = 0; k < L0; k += 4) {
-                const float4 v = __ldg(reinterpret_cast<const float4 *>(xp + k));
-                xc[k] = v.x; xc[k + 1] = v.y; xc[k + 2] = v.z; xc[k + 3] = v.w;
-            }
-        } else {
-#pragma unroll
-            for (int k = 0; k < L0; k++) xc[k] = __ldg(xp + k);
-        }
-        const bool block_end = ((t + 1) % a.tiles_per_block) == 0;
-        w.energies = (a.energies && block_end)
-                         ? a.energies + (size_t)c * a.e_stride + (size_t)(t / a.tiles_per_block) * nbands
-                         : nullptr;
+        load_tile<L0>(xch + (size_t)t * TILE + lane * L0, a.vec_ok, xc);
+        w.energies = block_energies(a, c, t, nbands);
         w.t_off = (long long)t * TILE;
         scan_stage<L0>(xc, w, 0);
         __syncwarp();
@@ -410,45 +425,20 @@ bank_kernel3(const __grid_constant__ BankParams P, const BankArgs a) {
     __syncthreads();
     const int nbands = P.n_oct * P.bpo;
     WarpCtxT<WANT_Y> w;
-    w.P = &P;
-    w.s_z = s_z;
-    w.s_e = s_e;
-    w.s_coef = s_coef;
-    w.lane = lane;
-    w.db = a.db;
-    w.weight = a.weight;
-    w.t_total = a.t_total;
-    w.y = a.y ? a.y + (size_t)c * a.y_stride : nullptr;
+    channel_ctx<WANT_Y>(w, P, a, c, lane, s_z, s_e, s_coef);
     const float *xch = a.x + (size_t)c * a.x_stride;
-    const int n_blocks = a.n_tiles / a.tiles_per_block;
     constexpr int NSCAN = Log2<L0>::v;           // scan-mode stages 0 .. NSCAN-1 (L = L0 .. 2)
     for (int t = 0; t <= a.n_tiles; t++) {
         if (role < 2 && t < a.n_tiles) {
-            const float *xp = xch + (size_t)t * TILE + lane * L0;
             float xc[L0];
-            if (a.vec_ok) {
-#pragma unroll
-                for (int k = 0; k < L0; k += 4) {
-                    const float4 v = __ldg(reinterpret_cast<const float4 *>(xp + k));
-                    xc[k] = v.x; xc[k + 1] = v.y; xc[k + 2] = v.z; xc[k + 3] = v.w;
-                }
-            } else {
-#pragma unroll
-                for (int k = 0; k < L0; k++) xc[k] = __ldg(xp + k);
-            }
-            const bool block_end = ((t + 1) % a.tiles_per_block) == 0;
-            w.energies = (a.energies && block_end)
-                             ? a.energies + (size_t)c * a.e_stride + (size_t)(t / a.tiles_per_block) * nbands
-                             : nullptr;
+            load_tile<L0>(xch + (size_t)t * TILE + lane * L0, a.vec_ok, xc);
+            w.energies = block_energies(a, c, t, nbands);
             w.t_off = (long long)t * TILE;
             if (role == 0) stage_D<L0>(xc, w, 0, s_x, s_x32 + (t & 1) * 32);
             else stage_B<L0>(xc, w, 0, s_x);
         } else if (role == 2 && t >= 1) {
             const int tp = t - 1;
-            const bool block_end = ((tp + 1) % a.tiles_per_block) == 0;
-            w.energies = (a.energies && block_end)
-                             ? a.energies + (size_t)c * a.e_stride + (size_t)(tp / a.tiles_per_block) * nbands
-                             : nullptr;
+            w.energies = block_energies(a, c, tp, nbands);
             w.t_off = (long long)tp * TILE;
             if (NSCAN < P.n_oct) serial_stages<WarpCtxT<WANT_Y>>(s_x32[(tp & 1) * 32 + lane], 32, w, NSCAN);
         }
@@ -544,6 +534,29 @@ static void mat2_mul(const double a[4], const double b[4], double o[4]) {
     o[3] = a[2] * b[1] + a[3] * b[3];
 }
 
+// Stores the SOS row s = (b0, b1, b2, a0, a1, a2) as normalised section sec of P (coefficients and
+// the powers A^(2^q) the scan uses) and its gain g in *gain.  Elliptic sections have their zeros on
+// the unit circle, b = g (1, c, 1); returns what is wrong with a row of another form, else NULL.
+static const char *set_section(BankParams &P, int sec, const double *s, double *gain) {
+    if (fabs(s[3] - 1.0) > 1e-12) return "a0 != 1";
+    if (!(fabs(s[0]) > 0.0) || fabs(s[2] / s[0] - 1.0) > 1e-7) return "b2 != b0 (zeros off the unit circle)";
+    *gain = s[0];
+    P.coef[sec][0] = 1.f; P.coef[sec][1] = (float)(s[1] / s[0]); P.coef[sec][2] = 1.f;
+    P.coef[sec][3] = (float)s[4]; P.coef[sec][4] = (float)s[5];
+    // the scan must propagate the state of the float32 filter that pass 2 runs
+    const double fb1 = P.coef[sec][1], fa1 = P.coef[sec][3], fa2 = P.coef[sec][4];
+    P.coef[sec][5] = (float)(fb1 - fa1);
+    P.coef[sec][6] = (float)(1.0 - fa2);
+    double A[4] = {-fa1, 1.0, -fa2, 0.0};
+    for (int q = 0; q < NQ; q++) {
+        for (int i = 0; i < 4; i++) P.apow[sec][q][i] = (float)A[i];
+        double A2[4];
+        mat2_mul(A, A, A2);
+        memcpy(A, A2, sizeof(A));
+    }
+    return nullptr;
+}
+
 extern "C" int frt_bank_plan(frt_handle h, int n_channels, int bands_per_octave, int n_octaves,
                              const double *sos_band, const double *sos_dec,
                              const double *alphas) {
@@ -567,30 +580,12 @@ extern "C" int frt_bank_plan(frt_handle h, int n_channels, int bands_per_octave,
     for (int sec = 0; sec < P.nsec; sec++) {
         const double *s = sec < 2 * bands_per_octave ? sos_band + (size_t)sec * 6
                                                      : sos_dec + (size_t)(sec - 2 * bands_per_octave) * 6;
-        if (fabs(s[3] - 1.0) > 1e-12) {
+        double g;
+        if (const char *why = set_section(P, sec, s, &g)) {
             delete pl;
-            return frt_fail(h, FRT_EINVAL, "SOS section %d has a0 != 1", sec);
+            return frt_fail(h, FRT_EINVAL, "SOS section %d: %s", sec, why);
         }
-        // elliptic sections have their zeros on the unit circle: b = g (1, c, 1)
-        if (!(fabs(s[0]) > 0.0) || fabs(s[2] / s[0] - 1.0) > 1e-7) {
-            delete pl;
-            return frt_fail(h, FRT_EINVAL, "SOS section %d: b2 != b0 (zeros off the unit circle)", sec);
-        }
-        gchain[sec < 2 * bands_per_octave ? sec / 2 : bands_per_octave] *= s[0];
-        const double cmid = s[1] / s[0], a1 = s[4], a2 = s[5];
-        P.coef[sec][0] = 1.f; P.coef[sec][1] = (float)cmid; P.coef[sec][2] = 1.f;
-        P.coef[sec][3] = (float)a1; P.coef[sec][4] = (float)a2;
-        // the scan must propagate the state of the float32 filter that pass 2 runs
-        const double fb1 = P.coef[sec][1], fa1 = P.coef[sec][3], fa2 = P.coef[sec][4];
-        P.coef[sec][5] = (float)(fb1 - fa1);
-        P.coef[sec][6] = (float)(1.0 - fa2);
-        double A[4] = {-fa1, 1.0, -fa2, 0.0};
-        for (int q = 0; q < NQ; q++) {
-            for (int i = 0; i < 4; i++) P.apow[sec][q][i] = (float)A[i];
-            double A2[4];
-            mat2_mul(A, A, A2);
-            memcpy(A, A2, sizeof(A));
-        }
+        gchain[sec < 2 * bands_per_octave ? sec / 2 : bands_per_octave] *= g;
     }
     for (int i = 0; i < bands_per_octave; i++) P.gband[i] = (float)gchain[i];
     P.gdec = (float)gchain[bands_per_octave];
@@ -721,9 +716,9 @@ static cudaError_t launch_bank_y(const BankPlan *pl, const BankArgs &a, cudaStre
     // per channel already saturates the schedulers with less synchronisation
     // the three-warp kernel runs all log2(L0) scan-mode stages unconditionally: it needs more
     // octaves than that (always true for the 9- and 10-octave banks of the reference)
-    const bool can_three = pl->params.n_oct > Log2<L0>::v;
-    const bool three = can_three && a.n_channels < 1536 && L0 <= 16;
-    if (three) return launch_bank3<L0, WANT_Y>(pl, a, st);
+    if constexpr (L0 <= 16) {
+        if (pl->params.n_oct > Log2<L0>::v && a.n_channels < 1536) return launch_bank3<L0, WANT_Y>(pl, a, st);
+    }
     const BankParams &P = pl->params;
     const int warps = 2;
     const size_t smem = sizeof(float) * ((size_t)P.nsec * 8 + (size_t)warps * (pl->nz + pl->ne));
@@ -813,27 +808,15 @@ static int bank_process_impl(frt_handle h, const float *x_dev, int64_t x_stride,
     // Kernel choice.  The lane-pipelined kernel (bank_pipe.cu) computes every section sample once
     // and is the fast path for the fused energies of 1- and 1/3-octave banks; the chunk-scan
     // kernels below serve the ragged band outputs (`.filter()`), 6/12/24 bands per octave and
-    // block lengths that are not a power of two.  FRT_BANK_KERNEL=scan|pipe, FRT_BANK_PACK=1|2 and
-    // FRT_BANK_LOGCH=5|6 override the choice, so that tests reach every pipelined variant (two
-    // channels per lane, 32-sample steps) at small channel counts.
-    const char *force_k = getenv("FRT_BANK_KERNEL");
-    const char *force_p = getenv("FRT_BANK_PACK");
-    const char *force_c = getenv("FRT_BANK_LOGCH");
+    // block lengths that are not a power of two.
     const bool pow2 = (block & (block - 1)) == 0;
-    bool use_pipe = pl->pipe_ok && !y_dev && pow2 && (block >> (P.n_oct - 1)) >= 1;
-    if (force_k && force_k[0] == 's') use_pipe = false;
-    if (use_pipe) {
-        // 64-sample steps up to 3072 channels, above that 32-sample steps with two channels per lane
-        // (two independent recurrences per lane once the schedulers are full).  The choice depends on
-        // the plan and the block length only, so a stream gives the same bits however it is cut into
-        // launches.
-        int pack = pl->n_channels > 3072 ? 2 : 1;
-        int logch = (block >= 512 && pl->n_channels <= 3072) ? 6 : 5;
-        if (force_p) pack = force_p[0] == '2' ? 2 : 1;
-        if (force_c) logch = force_c[0] == '6' ? 6 : 5;
-        // fall back to shorter steps when the block is too short for the variant's pipeline depth
-        // (frt_pipe_supported)
-        while (logch > 5 && !frt_pipe_supported(pl, block, logch)) logch--;
+    if (pl->pipe_ok && !y_dev && pow2 && (block >> (P.n_oct - 1)) >= 1) {
+        // 64-sample steps up to 3072 channels (32-sample steps for 256-sample blocks), above that
+        // 32-sample steps with two channels per lane (two independent recurrences per lane once the
+        // schedulers are full).  The choice depends on the plan and the block length only, so a
+        // stream gives the same bits however it is cut into launches.
+        const int pack = pl->n_channels > 3072 ? 2 : 1;
+        const int logch = (block >= 512 && pack == 1) ? 6 : 5;
         e = frt_pipe_launch(pl, a, logch, pack, st);
     } else if (tile == 1024) e = launch_bank<32>(pl, a, st);
     else if (tile == 512) e = launch_bank<16>(pl, a, st);
@@ -875,24 +858,13 @@ extern "C" int frt_decimate_plan(frt_handle h, int n_channels, int n_stages, con
     P.nsec = 6;
     double gdec = 1.0;
     for (int sec = 0; sec < 6; sec++) {
-        const double *s = sos_dec + (size_t)sec * 6;
-        if (!(fabs(s[0]) > 0.0) || fabs(s[2] / s[0] - 1.0) > 1e-7 || fabs(s[3] - 1.0) > 1e-12) {
+        double g;
+        if (const char *why = set_section(P, sec, sos_dec + (size_t)sec * 6, &g)) {
             delete pl;
-            return frt_fail(h, FRT_EINVAL, "decimator section %d is not of the form g(1,c,1)/(1,a1,a2)", sec);
+            return frt_fail(h, FRT_EINVAL, "decimator section %d is not of the form g(1,c,1)/(1,a1,a2): %s",
+                            sec, why);
         }
-        gdec *= s[0];
-        P.coef[sec][0] = 1.f; P.coef[sec][1] = (float)(s[1] / s[0]); P.coef[sec][2] = 1.f;
-        P.coef[sec][3] = (float)s[4]; P.coef[sec][4] = (float)s[5];
-        const double fb1 = P.coef[sec][1], fa1 = P.coef[sec][3], fa2 = P.coef[sec][4];
-        P.coef[sec][5] = (float)(fb1 - fa1);
-        P.coef[sec][6] = (float)(1.0 - fa2);
-        double A[4] = {-fa1, 1.0, -fa2, 0.0};
-        for (int q = 0; q < NQ; q++) {
-            for (int i = 0; i < 4; i++) P.apow[sec][q][i] = (float)A[i];
-            double A2[4];
-            mat2_mul(A, A, A2);
-            memcpy(A, A2, sizeof(A));
-        }
+        gdec *= g;
     }
     P.gdec = (float)gdec;
     pl->n_channels = n_channels;

@@ -817,7 +817,7 @@ cudaError_t frt_pipe_launch(const BankPlan *pl, BankArgs a, int logch, int pack,
     const PipeParams &P = pl->pipe[logch - 5];
     int T[BANK_MAX_OCT + 1];
     frt_pipe_schedule(P.n_oct, logch, a.t_total, T, &a.n_steps);
-    if (logch == 5)
-        return pack == 2 ? launch_pipe_bpo<5, 2>(P, a, st) : launch_pipe_bpo<5, 1>(P, a, st);
-    return pack == 2 ? launch_pipe_bpo<6, 2>(P, a, st) : launch_pipe_bpo<6, 1>(P, a, st);
+    // two channels per lane run 32-sample steps only
+    if (pack == 2) return logch == 5 ? launch_pipe_bpo<5, 2>(P, a, st) : cudaErrorInvalidConfiguration;
+    return logch == 5 ? launch_pipe_bpo<5, 1>(P, a, st) : launch_pipe_bpo<6, 1>(P, a, st);
 }

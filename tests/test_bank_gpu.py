@@ -85,7 +85,8 @@ def test_thirty_bands_ten_octaves():
 
 @pytest.mark.parametrize("noct", [1, 3, 5])
 def test_few_octaves(noct):
-    """Banks with fewer octaves than scan-mode stages (API allows 1..10) stay on the one-warp kernel."""
+    """Banks of fewer octaves (API allows 1..10); at 512-sample blocks they run the pipelined kernel
+    (64-sample steps)."""
     import torch
     from friture_b200.octavefilters import Octave_Filters
     x = make_x(2, 2048, seed=noct)
@@ -183,7 +184,7 @@ def test_unaligned_views_take_the_scalar_load_path():
     a = Octave_Filters(3).energies_batch(xd[:, 1:], block=512)                 # misaligned rows
     b = Octave_Filters(3).energies_batch(xd[:, 1:].contiguous(), block=512)    # aligned copy
     assert torch.equal(a, b)
-    big = torch.from_numpy(make_x(6200, 513, seed=13)).cuda()                  # one-warp-per-channel kernel
+    big = torch.from_numpy(make_x(6200, 513, seed=13)).cuda()                  # two channels per lane
     a = Octave_Filters(3).energies_batch(big[:, 1:], block=512)
     b = Octave_Filters(3).energies_batch(big[:, 1:].contiguous(), block=512)
     assert torch.equal(a, b)

@@ -9,7 +9,9 @@ import numpy as np
 import pytest
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-from bank_pipeline_model import PipeModel, n_steps_for, stage_start_steps  # noqa: E402
+from bank_pipeline_model import PipeModel, flush_delta, n_steps_for, stage_start_steps  # noqa: E402
+
+EN_RING = 8   # staged band-energy blocks per channel slot (bank_pipe.cu)
 
 
 def _oracle_energies(bpo, n_oct, block, x, response_time=1.0):
@@ -49,6 +51,21 @@ def test_schedule_model_streaming_and_state():
     m = _model(3, 9, 5)
     got = np.concatenate([m.process(x[i:i + 512], 512) for i in range(0, 4096, 512)])
     assert np.max(np.abs(got - E) / np.max(np.abs(E), axis=-1, keepdims=True)) < 1e-10
+
+
+def test_energy_ring_holds_every_supported_block():
+    """frt_pipe_supported's ring condition holds for every power-of-two block the pipelined kernel
+    accepts, at both step lengths and every octave count, so the library needs no fallback to shorter
+    steps: a block's vector leaves flush_delta steps after its last chunk, and the blocks staged
+    meanwhile plus the one being written fit in the ring."""
+    for n_oct in range(1, 11):
+        for logch in (5, 6):
+            fdelta = flush_delta(n_oct, logch, stage_start_steps(n_oct, logch))
+            for block in (1 << b for b in range(8, 17)):
+                if block < (4 << logch) or (block >> (n_oct - 1)) < 1:
+                    continue
+                nb = block >> logch
+                assert (fdelta + nb - 1) // nb + 2 <= EN_RING, (n_oct, logch, block, fdelta)
 
 
 def test_library_schedule_matches_model():
