@@ -102,14 +102,7 @@ extern "C" int frt_destroy(frt_handle h) {
     if (!h) return FRT_OK;
     DeviceGuard g(h->device);
     cudaDeviceSynchronize();
-    for (auto &kv : h->stft_cache) {
-        StftPlan &pl = kv.second;
-        if (pl.win_dev) cudaFree(pl.win_dev);
-        if (pl.tw_dev) cudaFree(pl.tw_dev);
-        if (pl.post_dev) cudaFree(pl.post_dev);
-        if (pl.wlane_dev) cudaFree(pl.wlane_dev);
-        if (pl.comb_dev) cudaFree(pl.comb_dev);
-    }
+    for (auto &kv : h->stft_cache) frt_stft_free_plan(kv.second);
     frt_bank_release(h);
     frt_gcc_release(h);
     frt_dec_release(h);

@@ -14,12 +14,14 @@
 struct StftPlan {
     int n_fft = 0;
     float *win_dev = nullptr;      // [n_fft] symmetric Hann (audioproc.py:76-81)
-    float2 *tw_dev = nullptr;      // fast path: [32][32] W_M^(k1*t); generic: [M] W_M^k
-    float2 *post_dev = nullptr;    // [M/2+1] U[k] = -j*W_N^k (real-FFT split twiddles)
-    float2 *wlane_dev = nullptr;   // N = 4096/8192: per-(warp, lane) Hann phase factors
-    float2 *comb_dev = nullptr;    // N = 4096/8192: [(R-1)][1024] W_M^(w k0)
+    float2 *tw_dev = nullptr;      // N = 64..2048: [M/32][32] W_M^(k1*t); N >= 4096: [32][32] W_1024^(k1*t);
+                                   // N = 32: [M] W_M^k
+    float2 *post_dev = nullptr;    // U[k] = -j*W_N^k (real-FFT split twiddles), as many as the kernels read
+    float4 *wlane_dev = nullptr;   // N = 4096/8192: per-(warp, lane) Hann phase factors
+    float2 *comb_dev = nullptr;    // N >= 4096: [(R-1)][1024] W_M^(w k0)
     std::vector<float> win_host;
 };
+void frt_stft_free_plan(StftPlan &pl);   // frees the plan's device tables
 
 struct HostPipe {                 // staging for the *_host entry points
     cudaStream_t s_in = nullptr, s_cmp = nullptr, s_out = nullptr;

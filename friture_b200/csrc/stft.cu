@@ -8,19 +8,21 @@
 //     X[k]   = (E + T)/2,  X[M-k] = conj(E - T)/2,
 //     E = Z[k] + conj(Z[M-k]),  O = Z[k] - conj(Z[M-k]),  T = (-j*W_N^k) * O.
 //
-// Fast path (N = 2048, the benchmark's size): ONE WARP PER FRAME, M = 1024 = 32 x 32.
+// N = 64 Q, Q in {1, .., 32} (64 .. 2048 points, the benchmark's size is 2048): ONE WARP PER 32/Q
+//   FRAMES (stft_small_kernel).  At N = 2048, M = 1024 = 32 x 32:
 //   lane t holds z[32*n1 + t] (n1 = 0..31) in registers -> radix-32 DFT over n1 in registers
 //   -> twiddle W_M^(k1*t) -> 32x32 transpose through a warp-private padded smem tile
 //   -> radix-32 DFT over n2 -> lane t holds X[t + 32*k2]; the split partner X[M-k] lives in
 //   lane (32-t)%32 and is fetched with warp shuffles.  Only __syncwarp(), no block barrier.
 //   Complex arithmetic is written on float2 through the component-wise f2_* helpers (two FADDs
 //   per complex add, one FMUL + one FFMA per component of a complex multiply).
-// N = 64 .. 1024: one warp per 32/Q frames (N = 64 Q), the same two register passes (stft_small_kernel).
 // N = 4096 / 8192: R = 2 / 4 warps per frame, each a 1024-point FFT of a decimated sequence, radix-R
 //   combine through shared memory (stft_large_kernel; stft_multi_kernel for unaligned input and 16384).
 // Generic path (N = 32): one CTA per frame, Stockham radix-4 (+ one radix-2 pass when log2(M) is
 //   odd) ping-ponging between two shared-memory buffers.
 #include <cmath>
+#include <type_traits>
+#include <utility>
 
 #include "frt_internal.cuh"
 
@@ -179,144 +181,29 @@ __device__ __forceinline__ void fence_proxy_async() {
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 
-// ------------------------------------------------------------------------------------------
-// Fast path, N = 2048.
-constexpr int FAST_N = 2048;
-constexpr int FAST_M = 1024;
-constexpr int FAST_WARPS = 16;
-constexpr int FAST_TILE = 32 * 33;   // padded 32x32 complex tile per warp
-constexpr int FAST_POST = 17 * 32;
-constexpr size_t FAST_SMEM =
-    sizeof(float2) * (FAST_M + FAST_M + FAST_POST + (size_t)FAST_WARPS * FAST_TILE) +
-    sizeof(unsigned long long) * FAST_WARPS;
+constexpr int TILE = 32 * 33;   // padded 32x32 complex tile per warp
 
-template <int MODE, int VEC>
-__global__ void __launch_bounds__(FAST_WARPS * 32, 1)
-stft2048_kernel(const float *__restrict__ x, long long x_stride, long long n_frames, int hop,
-                float *__restrict__ out, long long out_stride_c, long long out_stride_f,
-                const float2 *__restrict__ win2, const float2 *__restrict__ tw,
-                const float2 *__restrict__ post, long long total_items) {
-    extern __shared__ float2 smem[];
-    float2 *s_win = smem;                 // [1024]  (w[2n], w[2n+1])
-    float2 *s_tw = s_win + FAST_M;        // [32][32] W_1024^(k1*t)
-    float2 *s_post = s_tw + FAST_M;       // [17][32] U[t + 32 m] = -j W_2048^(t+32m)
-    const int lane = threadIdx.x & 31;
-    const int warp = threadIdx.x >> 5;
-    float2 *s_x = s_post + FAST_POST + warp * FAST_TILE;   // 16-byte aligned: FAST_TILE*8 % 16 == 0
-    unsigned long long *s_bar =
-        reinterpret_cast<unsigned long long *>(s_post + FAST_POST + FAST_WARPS * FAST_TILE);
-
-    for (int i = threadIdx.x; i < FAST_M; i += blockDim.x) {
-        s_win[i] = win2[i];
-        s_tw[i] = tw[i];
-    }
-    for (int i = threadIdx.x; i < FAST_POST; i += blockDim.x) s_post[i] = post[i];
-    __syncthreads();
-
-    // contiguous range of (channel, frame) items per warp: consecutive frames of a channel
-    // stay on one SM so the overlapping half of each frame is re-read from L1/L2, not HBM
-    const long long warps_total = (long long)gridDim.x * FAST_WARPS;
-    const long long gw = (long long)blockIdx.x * FAST_WARPS + warp;
-    const long long per = (total_items + warps_total - 1) / warps_total;
-    long long item = gw * per;
-    long long item_end = item + per;
-    if (item_end > total_items) item_end = total_items;
-    const float scale = 1.0f / (4.0f * (float)FAST_N * (float)FAST_N);
-    const int src_lane = (32 - lane) & 31;
-    // VEC == 2: the next frame's 8 KB of samples are fetched by the TMA engine (cp.async.bulk)
-    // into this warp's exchange tile while the current frame is in its second FFT pass and split
-    // step, so no warp ever waits on a global load with its registers tied up.
-    unsigned long long *bar = s_bar + warp;
-    unsigned parity = 0;
-    if (VEC == 2) {
-        if (lane == 0) mbar_init(bar, 1);
-        fence_proxy_async();
-        __syncwarp();
-        if (lane == 0 && item < item_end) {
-            mbar_expect_tx(bar, FAST_N * 4);
-            bulk_g2s(s_x, x + (item / n_frames) * x_stride + (item % n_frames) * hop, FAST_N * 4,
-                     bar);
+// First half of the second radix-32 pass: twiddle W_M^(k1 t) and the transpose through the warp's
+// padded tile.  Lane t holds 32/Q groups of Q bins k1 (register g*Q + r holds k1 = brevq<Q>(r) of
+// group g); afterwards lane g*Q + k1 holds the 32 values over t of group g, residue k1, and the tile
+// is free again.  The caller finishes the pass with dft32.
+template <int Q>
+__device__ __forceinline__ void twiddle_transpose(float2 (&v)[32], const float2 *s_tw, float2 *s_x,
+                                                  int lane) {
+#pragma unroll
+    for (int r = 0; r < Q; r++) {
+        const int k1 = brevq<Q>(r);
+        const float2 w = s_tw[k1 * 32 + lane];
+#pragma unroll
+        for (int g = 0; g < 32 / Q; g++) {
+            const float2 val = (k1 == 0) ? v[g * Q + r] : cmul(v[g * Q + r], w);
+            s_x[(g * Q + k1) * 33 + lane] = val;
         }
     }
-    long long c = (item < item_end) ? item / n_frames : 0;
-    long long f = item - c * n_frames;
-    for (; item < item_end; item++) {
-        const float *p = x + c * x_stride + f * hop;
-        float2 v[32];
-        if (VEC == 2) {
-            mbar_wait(bar, parity);
-            parity ^= 1;
+    __syncwarp();
 #pragma unroll
-            for (int n1 = 0; n1 < 32; n1++) v[n1] = s_x[32 * n1 + lane];
-            __syncwarp();   // every lane has its samples before the tile is reused for the exchange
-        } else if (VEC) {
-            const float2 *p2 = reinterpret_cast<const float2 *>(p);
-#pragma unroll
-            for (int n1 = 0; n1 < 32; n1++) v[n1] = __ldg(p2 + 32 * n1 + lane);
-        } else {
-#pragma unroll
-            for (int n1 = 0; n1 < 32; n1++) {
-                v[n1].x = __ldg(p + 64 * n1 + 2 * lane);
-                v[n1].y = __ldg(p + 64 * n1 + 2 * lane + 1);
-            }
-        }
-#pragma unroll
-        for (int n1 = 0; n1 < 32; n1++) v[n1] = f2_mul(v[n1], s_win[32 * n1 + lane]);
-
-        dft32(v);   // v[r] = sum_n1 z[32 n1 + t] W_32^(n1 k1), k1 = brev5(r)
-#pragma unroll
-        for (int r = 0; r < 32; r++) {
-            const int k1 = brev5(r);
-            const float2 val = (k1 == 0) ? v[r] : cmul(v[r], s_tw[k1 * 32 + lane]);
-            s_x[k1 * 33 + lane] = val;
-        }
-        __syncwarp();
-#pragma unroll
-        for (int n2 = 0; n2 < 32; n2++) v[n2] = s_x[lane * 33 + n2];
-        __syncwarp();
-        if (VEC == 2 && item + 1 < item_end) {   // tile is free: prefetch the next frame into it
-            long long cn = c, fn = f + 1;
-            if (fn == n_frames) {
-                fn = 0;
-                cn++;
-            }
-            fence_proxy_async();
-            if (lane == 0) {
-                mbar_expect_tx(bar, FAST_N * 4);
-                bulk_g2s(s_x, x + cn * x_stride + fn * hop, FAST_N * 4, bar);
-            }
-        }
-        dft32(v);   // v[r] = Z[lane + 32*brev5(r)]
-
-        float *o = out + c * out_stride_c + f * out_stride_f;
-#pragma unroll
-        for (int m = 0; m < 16; m++) {
-            const float2 z = v[brev5(m)];
-            const float2 other = v[brev5(31 - m)];
-            float2 zp;
-            zp.x = __shfl_sync(0xffffffffu, other.x, src_lane);
-            zp.y = __shfl_sync(0xffffffffu, other.y, src_lane);
-            if (lane == 0) zp = (m == 0) ? v[0] : v[brev5(32 - m)];
-            const float2 E = make_float2(z.x + zp.x, z.y - zp.y);
-            const float2 O = make_float2(z.x - zp.x, z.y + zp.y);
-            const float2 T = cmul(O, s_post[m * 32 + lane]);
-            const float2 X = cadd(E, T);
-            const float2 Y = csub(E, T);
-            const float p1 = fmaf(X.x, X.x, X.y * X.y);
-            const float p2 = fmaf(Y.x, Y.x, Y.y * Y.y);
-            const int k = lane + 32 * m;
-            o[k] = finish<MODE>(p1, scale);
-            o[FAST_M - k] = finish<MODE>(p2, scale);
-        }
-        if (lane == 0) {
-            const float2 z = v[brev5(16)];   // bin M/2: X = conj(Z)
-            o[FAST_M / 2] = finish<MODE>(4.0f * fmaf(z.x, z.x, z.y * z.y), scale);
-        }
-        if (++f == n_frames) {
-            f = 0;
-            c++;
-        }
-    }
+    for (int n2 = 0; n2 < 32; n2++) v[n2] = s_x[lane * 33 + n2];
+    __syncwarp();
 }
 
 // ------------------------------------------------------------------------------------------
@@ -358,27 +245,48 @@ template <> __device__ __forceinline__ void combine<8>(float2 (&t)[8]) {
     t[3] = cadd(e[3], o3);   t[7] = csub(e[3], o3);
 }
 
-template <int R>
-__device__ __forceinline__ void load_group(const float2 *__restrict__ tiles,
-                                           const float2 *__restrict__ comb, int k0,
-                                           float2 (&t)[R]) {
-    t[0] = tiles[k0];
+// The R-warp kernels' last stage: radix-R combine of the R natural-order tiles Z_w and the split
+// step of every bin of the frame, by thread t of the frame's 32 R threads.  comb(w, k0) and post(kk)
+// read W_M^(w k0) and U[kk] from wherever the kernel keeps those tables.
+template <int R, int MODE, class Comb, class Post>
+__device__ __forceinline__ void combine_split(float *__restrict__ o, const float2 *tiles, Comb comb,
+                                              Post post, int t, float scale) {
+    constexpr int M = 1024 * R;
+    auto load_group = [&](int k0, float2(&g)[R]) {
+        g[0] = tiles[k0];
 #pragma unroll
-    for (int w = 1; w < R; w++)
-        t[w] = cmul(tiles[w * FAST_TILE + k0], __ldg(comb + (w - 1) * 1024 + k0));
-    combine<R>(t);
-}
-
-template <int MODE>
-__device__ __forceinline__ void split_store(float *__restrict__ o, int kk, int M, float2 z, float2 zp,
-                                            const float2 *__restrict__ post, float scale) {
-    const float2 E = make_float2(z.x + zp.x, z.y - zp.y);
-    const float2 O = make_float2(z.x - zp.x, z.y + zp.y);
-    const float2 T = cmul(O, __ldg(post + kk));
-    const float2 X = cadd(E, T);
-    const float2 Y = csub(E, T);
-    o[kk] = finish<MODE>(fmaf(X.x, X.x, X.y * X.y), scale);
-    o[M - kk] = finish<MODE>(fmaf(Y.x, Y.x, Y.y * Y.y), scale);
+        for (int w = 1; w < R; w++) g[w] = cmul(tiles[w * TILE + k0], comb(w, k0));
+        combine<R>(g);
+    };
+    auto split_store = [&](int kk, float2 z, float2 zp) {
+        const float2 E = make_float2(z.x + zp.x, z.y - zp.y);
+        const float2 O = make_float2(z.x - zp.x, z.y + zp.y);
+        const float2 T = cmul(O, post(kk));
+        const float2 X = cadd(E, T);
+        const float2 Y = csub(E, T);
+        o[kk] = finish<MODE>(fmaf(X.x, X.x, X.y * X.y), scale);
+        o[M - kk] = finish<MODE>(fmaf(Y.x, Y.x, Y.y * Y.y), scale);
+    };
+    for (int k0 = 1 + t; k0 < 512; k0 += 32 * R) {
+        float2 A[R], B[R];
+        load_group(k0, A);
+        load_group(1024 - k0, B);
+#pragma unroll
+        for (int q = 0; q < R; q++) split_store(k0 + 1024 * q, A[q], B[R - 1 - q]);
+    }
+    if (t == 0) {          // k0 = 0: partners inside the group, q <-> R - q
+        float2 A[R];
+        load_group(0, A);
+        split_store(0, A[0], A[0]);
+#pragma unroll
+        for (int q = 1; q <= R / 2; q++) split_store(1024 * q, A[q], A[R - q]);
+    }
+    if (t == 32) {         // k0 = 512: partners inside the group, q <-> R - 1 - q
+        float2 A[R];
+        load_group(512, A);
+#pragma unroll
+        for (int q = 0; q < R / 2; q++) split_store(512 + 1024 * q, A[q], A[R - 1 - q]);
+    }
 }
 
 template <int R, int MODE>
@@ -391,10 +299,10 @@ stft_multi_kernel(const float *__restrict__ x, long long x_stride, long long n_f
     constexpr int M = 1024 * R, N = 2 * M;
     extern __shared__ float2 smem[];
     float2 *s_tw = smem;                       // [32][32] W_1024^(k1 t)
-    float2 *s_tiles = s_tw + FAST_M;           // R padded tiles
+    float2 *s_tiles = s_tw + 1024;             // R padded tiles
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, tid = threadIdx.x;
-    float2 *s_x = s_tiles + warp * FAST_TILE;
-    for (int i = tid; i < FAST_M; i += blockDim.x) s_tw[i] = tw32[i];
+    float2 *s_x = s_tiles + warp * TILE;
+    for (int i = tid; i < 1024; i += blockDim.x) s_tw[i] = tw32[i];
     __syncthreads();
     const float scale = 1.0f / (4.0f * (float)N * (float)N);
     for (long long item = blockIdx.x; item < total_items; item += gridDim.x) {
@@ -415,76 +323,53 @@ stft_multi_kernel(const float *__restrict__ x, long long x_stride, long long n_f
             v[n1] = f2_mul(xv, __ldg(win2 + idx));
         }
         dft32(v);
-#pragma unroll
-        for (int r = 0; r < 32; r++) {
-            const int k1 = brev5(r);
-            const float2 val = (k1 == 0) ? v[r] : cmul(v[r], s_tw[k1 * 32 + lane]);
-            s_x[k1 * 33 + lane] = val;
-        }
-        __syncwarp();
-#pragma unroll
-        for (int n2 = 0; n2 < 32; n2++) v[n2] = s_x[lane * 33 + n2];
-        __syncwarp();
+        twiddle_transpose<32>(v, s_tw, s_x, lane);
         dft32(v);   // v[r] = Z_w[lane + 32*brev5(r)]
 #pragma unroll
         for (int r = 0; r < 32; r++) s_x[lane + 32 * brev5(r)] = v[r];   // natural order
         __syncthreads();
 
-        float *o = out + c * out_stride_c + f * out_stride_f;
-        for (int k0 = 1 + tid; k0 < 512; k0 += 32 * R) {
-            float2 A[R], B[R];
-            load_group<R>(s_tiles, comb, k0, A);
-            load_group<R>(s_tiles, comb, 1024 - k0, B);
-#pragma unroll
-            for (int q = 0; q < R; q++)
-                split_store<MODE>(o, k0 + 1024 * q, M, A[q], B[R - 1 - q], post, scale);
-        }
-        if (tid == 0) {          // k0 = 0: partners inside the group, q <-> R - q
-            float2 A[R];
-            load_group<R>(s_tiles, comb, 0, A);
-            split_store<MODE>(o, 0, M, A[0], A[0], post, scale);
-#pragma unroll
-            for (int q = 1; q <= R / 2; q++) split_store<MODE>(o, 1024 * q, M, A[q], A[R - q], post, scale);
-        }
-        if (tid == 32) {         // k0 = 512: partners inside the group, q <-> R - 1 - q
-            float2 A[R];
-            load_group<R>(s_tiles, comb, 512, A);
-#pragma unroll
-            for (int q = 0; q < R / 2; q++)
-                split_store<MODE>(o, 512 + 1024 * q, M, A[q], A[R - 1 - q], post, scale);
-        }
+        combine_split<R, MODE>(out + c * out_stride_c + f * out_stride_f, s_tiles,
+                               [=](int w, int k0) { return __ldg(comb + (w - 1) * 1024 + k0); },
+                               [=](int kk) { return __ldg(post + kk); }, tid, scale);
         __syncthreads();
     }
 }
 
 // ------------------------------------------------------------------------------------------
-// N = 64 Q, Q in {1, 2, 4, 8, 16} (64 .. 1024 points): ONE WARP PER G = 32/Q FRAMES.
+// N = 64 Q, Q in {1, 2, 4, 8, 16, 32} (64 .. 2048 points): ONE WARP PER G = 32/Q FRAMES.
 // M = N/2 = 32 Q.  Lane t holds z_g[32 n1 + t] (n1 < Q) of each of the G frames in register g*Q + n1,
-// so the register file is as full as in the N = 2048 kernel: G radix-Q DFTs in registers -> twiddle
+// so the register file is as full at every size as at N = 2048: G radix-Q DFTs in registers -> twiddle
 // W_M^(k1 t) -> ONE 32x32 transpose through the warp's tile, after which lane g*Q + k1 holds the 32
 // values (over t) of frame g, residue k1 -> radix-32 DFT -> that lane owns Z_g[k1 + Q k2], k2 = 0..31.
 // The split partner M - (k1 + Q m) = (Q - k1) + Q (31 - m) lives in lane g*Q + (Q - k1) % Q (the
 // lane itself when k1 = 0), one shuffle away.  Window, twiddle and split tables are read once per
 // G frames.
-constexpr int SMALL_WARPS = 8;
+// Q = 32 (N = 2048, one frame per warp) runs one CTA of 16 warps per SM, and with TMA its 16-byte
+// aligned frames are staged by the TMA engine; smaller Q run two CTAs of 8 warps per SM.
+template <int Q> __host__ __device__ constexpr int small_warps() { return Q == 32 ? 16 : 8; }
+template <int Q> __host__ __device__ constexpr int small_ctas_per_sm() { return Q == 32 ? 1 : 2; }
 template <int Q>
 constexpr size_t small_smem() {
-    return sizeof(float2) * (32 * Q + 32 * Q + 16 * Q + (size_t)SMALL_WARPS * FAST_TILE);
+    // window, twiddle and split tables, the warps' tiles and (Q = 32) the warps' mbarriers
+    return sizeof(float2) * (32 * Q + 32 * Q + 16 * Q + (size_t)small_warps<Q>() * TILE) +
+           (Q == 32 ? sizeof(unsigned long long) * small_warps<Q>() : 0);
 }
 
-template <int Q, int MODE>
-__global__ void __launch_bounds__(SMALL_WARPS * 32, 2)
+template <int Q, int MODE, bool TMA>
+__global__ void __launch_bounds__(small_warps<Q>() * 32, small_ctas_per_sm<Q>())
 stft_small_kernel(const float *__restrict__ x, long long x_stride, long long n_frames, int hop,
                   float *__restrict__ out, long long out_stride_c, long long out_stride_f,
                   const float2 *__restrict__ win2, const float2 *__restrict__ tw,
                   const float2 *__restrict__ post, long long total_items, int vec_ok) {
-    constexpr int G = 32 / Q, M = 32 * Q, N = 2 * M;
+    static_assert(!TMA || Q == 32, "TMA staging is for one frame per warp");
+    constexpr int G = 32 / Q, M = 32 * Q, N = 2 * M, WARPS = small_warps<Q>();
     extern __shared__ float2 smem[];
     float2 *s_win = smem;              // [M]     (w[2n], w[2n+1])
     float2 *s_tw = s_win + M;          // [Q][32] W_M^(k1 t)
     float2 *s_post = s_tw + M;         // [M/2]   U[k] = -j W_N^k
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    float2 *s_x = s_post + 16 * Q + warp * FAST_TILE;
+    float2 *s_x = s_post + 16 * Q + warp * TILE;   // 16-byte aligned: 80 Q and TILE are even
     for (int i = threadIdx.x; i < M; i += blockDim.x) {
         s_win[i] = win2[i];
         s_tw[i] = tw[i];
@@ -493,8 +378,10 @@ stft_small_kernel(const float *__restrict__ x, long long x_stride, long long n_f
     __syncthreads();
 
     // contiguous range of frames per warp, a multiple of G long
-    const long long warps_total = (long long)gridDim.x * SMALL_WARPS;
-    const long long gw = (long long)blockIdx.x * SMALL_WARPS + warp;
+    // (consecutive frames of a channel stay on one SM, so the overlapping part of each frame is
+    // re-read from L1/L2, not HBM)
+    const long long warps_total = (long long)gridDim.x * WARPS;
+    const long long gw = (long long)blockIdx.x * WARPS + warp;
     long long per = (total_items + warps_total - 1) / warps_total;
     per = (per + G - 1) / G * G;
     long long item = gw * per;
@@ -506,6 +393,21 @@ stft_small_kernel(const float *__restrict__ x, long long x_stride, long long n_f
 
     long long c = (item < item_end) ? item / n_frames : 0;
     long long f = item - c * n_frames;
+    // TMA: each frame's 8 KB are fetched by the TMA engine (cp.async.bulk) into the warp's tile
+    // while the frame before it is in its second FFT pass and split step, so no warp ever waits on
+    // a global load with its registers tied up.  The first frame is fetched here, each next one
+    // once the transpose has freed the tile.
+    unsigned long long *bar = reinterpret_cast<unsigned long long *>(s_post + 16 * Q + WARPS * TILE) + warp;
+    unsigned parity = 0;
+    if (TMA) {
+        if (lane == 0) mbar_init(bar, 1);
+        fence_proxy_async();
+        __syncwarp();
+        if (lane == 0 && item < item_end) {
+            mbar_expect_tx(bar, N * 4);
+            bulk_g2s(s_x, x + c * x_stride + f * hop, N * 4, bar);
+        }
+    }
     for (; item < item_end; item += G) {
         float2 v[32];
         long long myc = 0, myf = 0;
@@ -519,7 +421,13 @@ stft_small_kernel(const float *__restrict__ x, long long x_stride, long long n_f
                 myf = f;
                 myok = ok;
             }
-            if (ok && vec_ok) {
+            if (TMA) {
+                mbar_wait(bar, parity);
+                parity ^= 1;
+#pragma unroll
+                for (int n1 = 0; n1 < 32; n1++) v[n1] = s_x[32 * n1 + lane];
+                __syncwarp();   // every lane has its samples before the tile is reused for the exchange
+            } else if (ok && vec_ok) {
 #pragma unroll
                 for (int n1 = 0; n1 < Q; n1++)
                     v[g * Q + n1] = __ldg(reinterpret_cast<const float2 *>(p) + 32 * n1 + lane);
@@ -545,20 +453,14 @@ stft_small_kernel(const float *__restrict__ x, long long x_stride, long long n_f
             for (int g = 0; g < G; g++) v[g * Q + n1] = f2_mul(v[g * Q + n1], w);
         }
         dft_groups<Q>(v);   // v[g*Q + r] = sum_n1 z_g[32 n1 + t] W_Q^(n1 k1), k1 = brevq<Q>(r)
-#pragma unroll
-        for (int r = 0; r < Q; r++) {
-            const int kk1 = brevq<Q>(r);
-            const float2 w = s_tw[kk1 * 32 + lane];
-#pragma unroll
-            for (int g = 0; g < G; g++) {
-                const float2 val = (kk1 == 0) ? v[g * Q + r] : cmul(v[g * Q + r], w);
-                s_x[(g * Q + kk1) * 33 + lane] = val;
+        twiddle_transpose<Q>(v, s_tw, s_x, lane);
+        if (TMA && item + 1 < item_end) {   // the tile is free: fetch the next frame, (c, f), into it
+            fence_proxy_async();
+            if (lane == 0) {
+                mbar_expect_tx(bar, N * 4);
+                bulk_g2s(s_x, x + c * x_stride + f * hop, N * 4, bar);
             }
         }
-        __syncwarp();
-#pragma unroll
-        for (int n2 = 0; n2 < 32; n2++) v[n2] = s_x[lane * 33 + n2];
-        __syncwarp();
         dft32(v);   // v[r] = Z_g[k1 + Q*brev5(r)] of this lane's (g, k1)
 
         float *o = out + myc * out_stride_c + myf * out_stride_f;
@@ -609,7 +511,7 @@ struct HannA {
 template <int R>
 constexpr size_t large_smem() {
     // tw [1024] + comb [R-1][1024] + post [512 R + 1 -> even] + tiles
-    return sizeof(float2) * (1024 + 1024 * (R - 1) + 512 * R + 2 + (size_t)LARGE_WARPS * FAST_TILE);
+    return sizeof(float2) * (1024 + 1024 * (R - 1) + 512 * R + 2 + (size_t)LARGE_WARPS * TILE);
 }
 
 __device__ __forceinline__ void group_barrier(int id, int nthreads) {
@@ -630,28 +532,6 @@ __device__ __forceinline__ float2 post_lookup(const float2 *s_post, int kk, int 
 }
 
 template <int R, int MODE>
-__device__ __forceinline__ void split_store_s(float *__restrict__ o, int kk, float2 z, float2 zp,
-                                              const float2 *s_post, float scale) {
-    constexpr int M = 1024 * R;
-    const float2 E = make_float2(z.x + zp.x, z.y - zp.y);
-    const float2 O = make_float2(z.x - zp.x, z.y + zp.y);
-    const float2 T = cmul(O, post_lookup(s_post, kk, M / 2));
-    const float2 X = cadd(E, T);
-    const float2 Y = csub(E, T);
-    o[kk] = finish<MODE>(fmaf(X.x, X.x, X.y * X.y), scale);
-    o[M - kk] = finish<MODE>(fmaf(Y.x, Y.x, Y.y * Y.y), scale);
-}
-
-template <int R>
-__device__ __forceinline__ void load_group_s(const float2 *tiles, const float2 *s_comb, int k0,
-                                             float2 (&t)[R]) {
-    t[0] = tiles[k0];
-#pragma unroll
-    for (int w = 1; w < R; w++) t[w] = cmul(tiles[w * FAST_TILE + k0], s_comb[(w - 1) * 1024 + k0]);
-    combine<R>(t);
-}
-
-template <int R, int MODE>
 __global__ void __launch_bounds__(LARGE_WARPS * 32, 1)
 stft_large_kernel(const float *__restrict__ x, long long x_stride, long long n_frames, int hop,
                   float *__restrict__ out, long long out_stride_c, long long out_stride_f,
@@ -668,8 +548,8 @@ stft_large_kernel(const float *__restrict__ x, long long x_stride, long long n_f
     float2 *s_tiles_all = s_post + 512 * R + 2;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int grp = warp / R, w = warp % R, gtid = tid - grp * GT;
-    float2 *s_tiles = s_tiles_all + (size_t)grp * R * FAST_TILE;   // this group's R tiles
-    float2 *s_x = s_tiles + w * FAST_TILE;
+    float2 *s_tiles = s_tiles_all + (size_t)grp * R * TILE;   // this group's R tiles
+    float2 *s_x = s_tiles + w * TILE;
     for (int i = tid; i < 1024; i += blockDim.x) s_tw[i] = tw32[i];
     for (int i = tid; i < 1024 * (R - 1); i += blockDim.x) s_comb[i] = comb[i];
     for (int i = tid; i <= 512 * R; i += blockDim.x) s_post[i] = post[i];
@@ -692,7 +572,7 @@ stft_large_kernel(const float *__restrict__ x, long long x_stride, long long n_f
 #pragma unroll 8
         for (int e = gtid; e < M; e += GT) {
             const int ww = e % R, i = e / R;
-            cp_async8(s_tiles + ww * FAST_TILE + ww * STAG + i, p2 + e);
+            cp_async8(s_tiles + ww * TILE + ww * STAG + i, p2 + e);
         }
     };
     if (item < item_end) fetch(c, f);
@@ -711,44 +591,15 @@ stft_large_kernel(const float *__restrict__ x, long long x_stride, long long n_f
             v[n1] = f2_mul(v[n1], wv);
         }
         dft32(v);
-#pragma unroll
-        for (int r = 0; r < 32; r++) {
-            const int k1 = brev5(r);
-            const float2 val = (k1 == 0) ? v[r] : cmul(v[r], s_tw[k1 * 32 + lane]);
-            s_x[k1 * 33 + lane] = val;
-        }
-        __syncwarp();
-#pragma unroll
-        for (int n2 = 0; n2 < 32; n2++) v[n2] = s_x[lane * 33 + n2];
-        __syncwarp();
+        twiddle_transpose<32>(v, s_tw, s_x, lane);
         dft32(v);   // v[r] = Z_w[lane + 32*brev5(r)]
 #pragma unroll
         for (int r = 0; r < 32; r++) s_x[lane + 32 * brev5(r)] = v[r];   // natural order
         group_barrier(1 + grp, GT);
 
-        float *o = out + c * out_stride_c + f * out_stride_f;
-        for (int k0 = 1 + gtid; k0 < 512; k0 += GT) {
-            float2 A[R], B[R];
-            load_group_s<R>(s_tiles, s_comb, k0, A);
-            load_group_s<R>(s_tiles, s_comb, 1024 - k0, B);
-#pragma unroll
-            for (int q = 0; q < R; q++)
-                split_store_s<R, MODE>(o, k0 + 1024 * q, A[q], B[R - 1 - q], s_post, scale);
-        }
-        if (gtid == 0) {           // k0 = 0: partners inside the group, q <-> R - q
-            float2 A[R];
-            load_group_s<R>(s_tiles, s_comb, 0, A);
-            split_store_s<R, MODE>(o, 0, A[0], A[0], s_post, scale);
-#pragma unroll
-            for (int q = 1; q <= R / 2; q++) split_store_s<R, MODE>(o, 1024 * q, A[q], A[R - q], s_post, scale);
-        }
-        if (gtid == 32) {          // k0 = 512: partners inside the group, q <-> R - 1 - q
-            float2 A[R];
-            load_group_s<R>(s_tiles, s_comb, 512, A);
-#pragma unroll
-            for (int q = 0; q < R / 2; q++)
-                split_store_s<R, MODE>(o, 512 + 1024 * q, A[q], A[R - 1 - q], s_post, scale);
-        }
+        combine_split<R, MODE>(out + c * out_stride_c + f * out_stride_f, s_tiles,
+                               [=](int w, int k0) { return s_comb[(w - 1) * 1024 + k0]; },
+                               [=](int kk) { return post_lookup(s_post, kk, M / 2); }, gtid, scale);
         if (++f == n_frames) {
             f = 0;
             c++;
@@ -847,81 +698,102 @@ __global__ void stft_generic_kernel(const float *__restrict__ x, long long x_str
     }
 }
 
-template <int MODE, int VEC>
-cudaError_t set_fast_smem_one() {
-    return cudaFuncSetAttribute(stft2048_kernel<MODE, VEC>,
-                                cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FAST_SMEM);
-}
-cudaError_t set_fast_smem() {
-    cudaError_t e = set_fast_smem_one<0, 0>();
-    if (e == cudaSuccess) e = set_fast_smem_one<0, 1>();
-    if (e == cudaSuccess) e = set_fast_smem_one<0, 2>();
-    if (e == cudaSuccess) e = set_fast_smem_one<1, 0>();
-    if (e == cudaSuccess) e = set_fast_smem_one<1, 1>();
-    if (e == cudaSuccess) e = set_fast_smem_one<1, 2>();
-    return e;
+size_t multi_smem(int r) { return sizeof(float2) * (1024 + (size_t)r * TILE); }
+
+// every instance's dynamic shared-memory limit: what its launch below asks for
+template <int MODE>
+cudaError_t set_smem_limits() {
+    const std::pair<const void *, size_t> limits[] = {
+        {(const void *)stft_small_kernel<1, MODE, false>, small_smem<1>()},
+        {(const void *)stft_small_kernel<2, MODE, false>, small_smem<2>()},
+        {(const void *)stft_small_kernel<4, MODE, false>, small_smem<4>()},
+        {(const void *)stft_small_kernel<8, MODE, false>, small_smem<8>()},
+        {(const void *)stft_small_kernel<16, MODE, false>, small_smem<16>()},
+        {(const void *)stft_small_kernel<32, MODE, false>, small_smem<32>()},
+        {(const void *)stft_small_kernel<32, MODE, true>, small_smem<32>()},
+        {(const void *)stft_large_kernel<2, MODE>, large_smem<2>()},
+        {(const void *)stft_large_kernel<4, MODE>, large_smem<4>()},
+        {(const void *)stft_multi_kernel<2, MODE>, multi_smem(2)},
+        {(const void *)stft_multi_kernel<4, MODE>, multi_smem(4)},
+        {(const void *)stft_multi_kernel<8, MODE>, multi_smem(8)},
+        {(const void *)stft_generic_kernel, sizeof(float2) * 2 * 8192},
+    };
+    for (const auto &l : limits) {
+        const cudaError_t e =
+            cudaFuncSetAttribute(l.first, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)l.second);
+        if (e != cudaSuccess) return e;
+    }
+    return cudaSuccess;
 }
 
-template <int MODE, int VEC>
-void launch_fast(unsigned blocks, cudaStream_t st, const float *x, long long x_stride,
-                 long long n_frames, int hop, float *out, long long osc, long long osf,
-                 const StftPlan &pl, long long total) {
-    stft2048_kernel<MODE, VEC><<<blocks, FAST_WARPS * 32, FAST_SMEM, st>>>(
-        x, x_stride, n_frames, hop, out, osc, osf, reinterpret_cast<const float2 *>(pl.win_dev),
-        pl.tw_dev, pl.post_dev, total);
-}
-
-template <int Q>
-cudaError_t set_small_smem() {
-    cudaError_t e = cudaFuncSetAttribute(stft_small_kernel<Q, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         (int)small_smem<Q>());
-    if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(stft_small_kernel<Q, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 (int)small_smem<Q>());
-    return e;
-}
-template <int R>
-cudaError_t set_large_smem() {
-    cudaError_t e = cudaFuncSetAttribute(stft_large_kernel<R, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         (int)large_smem<R>());
-    if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(stft_large_kernel<R, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 (int)large_smem<R>());
-    return e;
-}
-
-template <int Q>
-void launch_small(int mode, unsigned blocks, cudaStream_t st, const float *x, long long x_stride,
-                  long long n_frames, int hop, float *out, long long osc, long long osf,
-                  const StftPlan &pl, long long total, int vec_ok) {
-    const float2 *w2 = reinterpret_cast<const float2 *>(pl.win_dev);
+// calls launch with the mode (FRT_STFT_POWER / FRT_STFT_LOGPOWER) as a compile-time constant
+template <class F>
+void with_mode(int mode, F &&launch) {
     if (mode == FRT_STFT_POWER)
-        stft_small_kernel<Q, FRT_STFT_POWER><<<blocks, SMALL_WARPS * 32, small_smem<Q>(), st>>>(
-            x, x_stride, n_frames, hop, out, osc, osf, w2, pl.tw_dev, pl.post_dev, total, vec_ok);
+        launch(std::integral_constant<int, FRT_STFT_POWER>());
     else
-        stft_small_kernel<Q, FRT_STFT_LOGPOWER><<<blocks, SMALL_WARPS * 32, small_smem<Q>(), st>>>(
-            x, x_stride, n_frames, hop, out, osc, osf, w2, pl.tw_dev, pl.post_dev, total, vec_ok);
+        launch(std::integral_constant<int, FRT_STFT_LOGPOWER>());
+}
+
+// how far every frame's first sample is aligned: 2 = 16 bytes, 1 = 8 bytes, 0 = 4 bytes
+int frame_alignment(const float *x, long long x_stride, int hop) {
+    if ((((uintptr_t)x & 15) == 0) && ((x_stride & 3) == 0) && ((hop & 3) == 0)) return 2;
+    return (((uintptr_t)x & 7) == 0) && ((x_stride & 1) == 0) && ((hop & 1) == 0);
+}
+
+// one frt_stft_process call: total = channels x frames items, frame f of channel c at
+// x + c x_stride + f hop, its spectrum at out + c osc + f osf
+struct Frames {
+    const float *x;
+    long long x_stride, n_frames;
+    int hop;
+    float *out;
+    long long osc, osf, total;
+    int mode, vec_ok;
+    cudaStream_t st;
+};
+
+template <int Q, bool TMA = false>
+void launch_small(const frt_ctx *h, const StftPlan &pl, const Frames &a) {
+    constexpr int G = 32 / Q, WARPS = small_warps<Q>();
+    const long long max_blocks = (long long)small_ctas_per_sm<Q>() * h->sm_count;
+    long long blocks = ((a.total + G - 1) / G + WARPS - 1) / WARPS;
+    if (blocks > max_blocks) blocks = max_blocks;
+    const float2 *w2 = reinterpret_cast<const float2 *>(pl.win_dev);
+    with_mode(a.mode, [&](auto m) {
+        stft_small_kernel<Q, decltype(m)::value, TMA><<<(unsigned)blocks, WARPS * 32, small_smem<Q>(), a.st>>>(
+            a.x, a.x_stride, a.n_frames, a.hop, a.out, a.osc, a.osf, w2, pl.tw_dev, pl.post_dev, a.total,
+            a.vec_ok);
+    });
 }
 template <int R>
-void launch_large(int mode, unsigned blocks, cudaStream_t st, const float *x, long long x_stride,
-                  long long n_frames, int hop, float *out, long long osc, long long osf,
-                  const StftPlan &pl, long long total) {
-    const float4 *wl = reinterpret_cast<const float4 *>(pl.wlane_dev);
+void launch_large(const frt_ctx *h, const StftPlan &pl, const Frames &a) {
+    constexpr int NG = LARGE_WARPS / R;
+    long long blocks = (a.total + NG - 1) / NG;
+    if (blocks > h->sm_count) blocks = h->sm_count;
     HannA ha;
     const double theta = 2.0 * 3.14159265358979323846 / (double)(2048 * R - 1);
     for (int n1 = 0; n1 < 32; n1++) {
         const double a = theta * 64.0 * R * n1;
         ha.v[n1] = make_float2((float)(0.5 * cos(a)), (float)(0.5 * sin(a)));
     }
-    if (mode == FRT_STFT_POWER)
-        stft_large_kernel<R, FRT_STFT_POWER><<<blocks, LARGE_WARPS * 32, large_smem<R>(), st>>>(
-            x, x_stride, n_frames, hop, out, osc, osf, wl, pl.tw_dev, pl.comb_dev, pl.post_dev, total, ha);
-    else
-        stft_large_kernel<R, FRT_STFT_LOGPOWER><<<blocks, LARGE_WARPS * 32, large_smem<R>(), st>>>(
-            x, x_stride, n_frames, hop, out, osc, osf, wl, pl.tw_dev, pl.comb_dev, pl.post_dev, total, ha);
+    with_mode(a.mode, [&](auto m) {
+        stft_large_kernel<R, decltype(m)::value><<<(unsigned)blocks, LARGE_WARPS * 32, large_smem<R>(), a.st>>>(
+            a.x, a.x_stride, a.n_frames, a.hop, a.out, a.osc, a.osf, pl.wlane_dev, pl.tw_dev, pl.comb_dev,
+            pl.post_dev, a.total, ha);
+    });
 }
-
-size_t multi_smem(int r) { return sizeof(float2) * (FAST_M + (size_t)r * FAST_TILE); }
+template <int R>
+void launch_multi(const frt_ctx *h, const StftPlan &pl, const Frames &a) {
+    long long blocks = (long long)h->sm_count * (R == 8 ? 2 : (R == 4 ? 4 : 8));
+    if (blocks > a.total) blocks = a.total;
+    const float2 *w2 = reinterpret_cast<const float2 *>(pl.win_dev);
+    with_mode(a.mode, [&](auto m) {
+        stft_multi_kernel<R, decltype(m)::value><<<(unsigned)blocks, 32 * R, multi_smem(R), a.st>>>(
+            a.x, a.x_stride, a.n_frames, a.hop, a.out, a.osc, a.osf, w2, pl.tw_dev, pl.comb_dev, pl.post_dev,
+            a.total, a.vec_ok);
+    });
+}
 
 int ilog2(int v) {
     int l = 0;
@@ -929,7 +801,34 @@ int ilog2(int v) {
     return l;
 }
 
+// [rows][32] table of W_m^(k1 t): the twiddles between the two radix-32 passes
+std::vector<float2> row_twiddles(int rows, int m) {
+    const double PI = 3.14159265358979323846;
+    std::vector<float2> tw((size_t)rows * 32);
+    for (int k1 = 0; k1 < rows; k1++)
+        for (int t = 0; t < 32; t++) {
+            const double a = -2.0 * PI * (double)((k1 * t) % m) / (double)m;
+            tw[k1 * 32 + t] = make_float2((float)cos(a), (float)sin(a));
+        }
+    return tw;
+}
+
+template <class T>
+cudaError_t upload(T **dev, const std::vector<T> &host) {
+    cudaError_t e = cudaMalloc(dev, sizeof(T) * host.size());
+    if (e == cudaSuccess) e = cudaMemcpy(*dev, host.data(), sizeof(T) * host.size(), cudaMemcpyHostToDevice);
+    return e;
+}
+
 }   // namespace
+
+void frt_stft_free_plan(StftPlan &pl) {
+    cudaFree(pl.win_dev);
+    cudaFree(pl.tw_dev);
+    cudaFree(pl.post_dev);
+    cudaFree(pl.wlane_dev);
+    cudaFree(pl.comb_dev);
+}
 
 extern "C" int frt_stft_plan(frt_handle h, int n_fft) {
     if (!h) return FRT_EINVAL;
@@ -948,12 +847,7 @@ extern "C" int frt_stft_plan(frt_handle h, int n_fft) {
     struct PlanGuard {
         StftPlan *p;
         ~PlanGuard() {
-            if (!p) return;
-            if (p->win_dev) cudaFree(p->win_dev);
-            if (p->tw_dev) cudaFree(p->tw_dev);
-            if (p->post_dev) cudaFree(p->post_dev);
-            if (p->wlane_dev) cudaFree(p->wlane_dev);
-            if (p->comb_dev) cudaFree(p->comb_dev);
+            if (p) frt_stft_free_plan(*p);
         }
     } guard{&pl};
     const int N = n_fft, M = N / 2;
@@ -962,93 +856,50 @@ extern "C" int frt_stft_plan(frt_handle h, int n_fft) {
     pl.win_host.resize(N);
     for (int n = 0; n < N; n++)
         pl.win_host[n] = (float)(0.5 * (1.0 - cos(2.0 * PI * n / (double)(N - 1))));
+    FRT_CUDA(h, upload(&pl.win_dev, pl.win_host));
     const int multi_r = (N == 4096) ? 2 : ((N == 8192) ? 4 : ((N == 16384) ? 8 : 0));
-    std::vector<float2> tw(M), post(multi_r ? M + 33 : M / 2 + 1 + 32);
-    if (multi_r) {
-        tw.resize(FAST_M);
-        for (int k1 = 0; k1 < 32; k1++)
-            for (int t = 0; t < 32; t++) {
-                const double a = -2.0 * PI * (double)((k1 * t) % FAST_M) / (double)FAST_M;
-                tw[k1 * 32 + t] = make_float2((float)cos(a), (float)sin(a));
-            }
+    std::vector<float2> tw;
+    if (multi_r) {   // each warp's 1024-point FFT, then the radix-R combine by W_M^(w k0)
+        tw = row_twiddles(32, 1024);
         std::vector<float2> comb((size_t)(multi_r - 1) * 1024);
         for (int w = 1; w < multi_r; w++)
             for (int k0 = 0; k0 < 1024; k0++) {
                 const double a = -2.0 * PI * (double)(w * k0) / (double)M;
                 comb[(size_t)(w - 1) * 1024 + k0] = make_float2((float)cos(a), (float)sin(a));
             }
-        FRT_CUDA(h, cudaMalloc(&pl.comb_dev, sizeof(float2) * comb.size()));
-        FRT_CUDA(h, cudaMemcpy(pl.comb_dev, comb.data(), sizeof(float2) * comb.size(),
-                               cudaMemcpyHostToDevice));
-    } else if (N == FAST_N) {
-        for (int k1 = 0; k1 < 32; k1++)
-            for (int t = 0; t < 32; t++) {
-                const double a = -2.0 * PI * (double)((k1 * t) % M) / (double)M;
-                tw[k1 * 32 + t] = make_float2((float)cos(a), (float)sin(a));
-            }
-    } else if (N >= 64 && N <= 1024) {   // stft_small_kernel: [Q][32] W_M^(k1 t), M = 32 Q
-        for (int k1 = 0; k1 < M / 32; k1++)
-            for (int t = 0; t < 32; t++) {
-                const double a = -2.0 * PI * (double)((k1 * t) % M) / (double)M;
-                tw[k1 * 32 + t] = make_float2((float)cos(a), (float)sin(a));
-            }
-    } else {
+        FRT_CUDA(h, upload(&pl.comb_dev, comb));
+    } else if (N >= 64) {   // stft_small_kernel: [Q][32] W_M^(k1 t), M = 32 Q
+        tw = row_twiddles(M / 32, M);
+    } else {                // stft_generic_kernel: [M] W_M^k
+        tw.resize(M);
         for (int i = 0; i < M; i++) {
             const double a = -2.0 * PI * (double)i / (double)M;
             tw[i] = make_float2((float)cos(a), (float)sin(a));
         }
     }
-    for (size_t k = 0; k < post.size(); k++) {   // U[k] = -j * W_N^k
+    FRT_CUDA(h, upload(&pl.tw_dev, tw));
+    // U[k] = -j * W_N^k for every k a kernel reads: k < M/2 in stft_small_kernel, k <= M/2 in
+    // stft_generic_kernel and stft_large_kernel (which derives the rest), k < M - 512 in
+    // stft_multi_kernel (its largest bin with a partner is k0 + 1024 (R-1), k0 < 512)
+    std::vector<float2> post(multi_r ? M - 512 : M / 2 + 1);
+    for (size_t k = 0; k < post.size(); k++) {
         const double a = 2.0 * PI * (double)k / (double)N;
         post[k] = make_float2((float)(-sin(a)), (float)(-cos(a)));
     }
+    FRT_CUDA(h, upload(&pl.post_dev, post));
     if (N == 4096 || N == 8192) {   // stft_large_kernel: per-(warp, lane) part of the Hann phase
         const int R = N / 2048;
-        std::vector<float> wl((size_t)R * 32 * 4);
+        std::vector<float4> wl((size_t)R * 32);
         const double theta = 2.0 * PI / (double)(N - 1);
         for (int w = 0; w < R; w++)
             for (int t = 0; t < 32; t++) {
                 const double b0 = theta * (2 * R * t + 2 * w), b1 = theta * (2 * R * t + 2 * w + 1);
-                float *q = &wl[((size_t)w * 32 + t) * 4];
-                q[0] = (float)cos(b0);
-                q[1] = (float)cos(b1);
-                q[2] = (float)sin(b0);
-                q[3] = (float)sin(b1);
+                wl[(size_t)w * 32 + t] = make_float4((float)cos(b0), (float)cos(b1), (float)sin(b0), (float)sin(b1));
             }
-        FRT_CUDA(h, cudaMalloc(&pl.wlane_dev, sizeof(float) * wl.size()));
-        FRT_CUDA(h, cudaMemcpy(pl.wlane_dev, wl.data(), sizeof(float) * wl.size(), cudaMemcpyHostToDevice));
+        FRT_CUDA(h, upload(&pl.wlane_dev, wl));
     }
-    FRT_CUDA(h, cudaMalloc(&pl.win_dev, sizeof(float) * N));
-    FRT_CUDA(h, cudaMalloc(&pl.tw_dev, sizeof(float2) * tw.size()));
-    FRT_CUDA(h, cudaMalloc(&pl.post_dev, sizeof(float2) * post.size()));
-    FRT_CUDA(h, cudaMemcpy(pl.win_dev, pl.win_host.data(), sizeof(float) * N,
-                           cudaMemcpyHostToDevice));
-    FRT_CUDA(h, cudaMemcpy(pl.tw_dev, tw.data(), sizeof(float2) * tw.size(),
-                           cudaMemcpyHostToDevice));
-    FRT_CUDA(h, cudaMemcpy(pl.post_dev, post.data(), sizeof(float2) * post.size(),
-                           cudaMemcpyHostToDevice));
-    if (N == FAST_N) {
-        FRT_CUDA(h, set_fast_smem());
-    } else if (multi_r) {
-        FRT_CUDA(h, cudaFuncSetAttribute(stft_multi_kernel<2, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)multi_smem(2)));
-        FRT_CUDA(h, cudaFuncSetAttribute(stft_multi_kernel<2, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)multi_smem(2)));
-        FRT_CUDA(h, cudaFuncSetAttribute(stft_multi_kernel<4, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)multi_smem(4)));
-        FRT_CUDA(h, cudaFuncSetAttribute(stft_multi_kernel<4, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)multi_smem(4)));
-        FRT_CUDA(h, cudaFuncSetAttribute(stft_multi_kernel<8, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)multi_smem(8)));
-        FRT_CUDA(h, cudaFuncSetAttribute(stft_multi_kernel<8, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)multi_smem(8)));
-        FRT_CUDA(h, set_large_smem<2>());
-        FRT_CUDA(h, set_large_smem<4>());
-    } else if (N >= 64 && N <= 1024) {
-        FRT_CUDA(h, set_small_smem<1>());
-        FRT_CUDA(h, set_small_smem<2>());
-        FRT_CUDA(h, set_small_smem<4>());
-        FRT_CUDA(h, set_small_smem<8>());
-        FRT_CUDA(h, set_small_smem<16>());
-    } else {
-        FRT_CUDA(h, cudaFuncSetAttribute(stft_generic_kernel,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         (int)(sizeof(float2) * 2 * 8192)));
-    }
+    FRT_CUDA(h, set_smem_limits<FRT_STFT_POWER>());
+    FRT_CUDA(h, set_smem_limits<FRT_STFT_LOGPOWER>());
     pl.n_fft = n_fft;
     guard.p = nullptr;          // the cache owns the device tables from here on
     h->stft_cache[n_fft] = pl;
@@ -1080,84 +931,36 @@ extern "C" int frt_stft_process(frt_handle h, const float *x_dev, int64_t x_stri
     const int nbins = pl.n_fft / 2 + 1;
     FRT_CHECK_ARG(h, out_stride_f >= nbins, "out_stride_f smaller than n_fft/2+1");
     const long long total = (long long)n_channels * n_frames;
-    cudaStream_t st = (cudaStream_t)stream;
-    if (pl.n_fft == FAST_N) {
-        int vec_ok = (((uintptr_t)x_dev & 7) == 0) && ((x_stride & 1) == 0) && ((hop & 1) == 0);
-        // 16-byte aligned frames: let the TMA engine stage them (cp.async.bulk)
-        if ((((uintptr_t)x_dev & 15) == 0) && ((x_stride & 3) == 0) && ((hop & 3) == 0))
-            vec_ok = 2;
-        long long blocks = (total + FAST_WARPS - 1) / FAST_WARPS;
-        if (blocks > h->sm_count) blocks = h->sm_count;
-#define FRT_LAUNCH_FAST(MODE, VEC)                                                         \
-    launch_fast<MODE, VEC>((unsigned)blocks, st, x_dev, x_stride, n_frames, hop, out_dev,   \
-                           out_stride_c, out_stride_f, pl, total)
-        if (mode == FRT_STFT_POWER) {
-            if (vec_ok == 2) FRT_LAUNCH_FAST(FRT_STFT_POWER, 2);
-            else if (vec_ok) FRT_LAUNCH_FAST(FRT_STFT_POWER, 1);
-            else FRT_LAUNCH_FAST(FRT_STFT_POWER, 0);
-        } else {
-            if (vec_ok == 2) FRT_LAUNCH_FAST(FRT_STFT_LOGPOWER, 2);
-            else if (vec_ok) FRT_LAUNCH_FAST(FRT_STFT_LOGPOWER, 1);
-            else FRT_LAUNCH_FAST(FRT_STFT_LOGPOWER, 0);
+    const int N = pl.n_fft, align = frame_alignment(x_dev, x_stride, hop);
+    const Frames a{x_dev, x_stride, n_frames, hop, out_dev, out_stride_c, out_stride_f, total,
+                   mode, align >= 1, (cudaStream_t)stream};
+    if (N >= 64 && N <= 2048) {
+        switch (N / 64) {
+            case 1: launch_small<1>(h, pl, a); break;
+            case 2: launch_small<2>(h, pl, a); break;
+            case 4: launch_small<4>(h, pl, a); break;
+            case 8: launch_small<8>(h, pl, a); break;
+            case 16: launch_small<16>(h, pl, a); break;
+            default:   // 16-byte aligned frames: the TMA engine stages them (cp.async.bulk)
+                if (align == 2) launch_small<32, true>(h, pl, a);
+                else launch_small<32>(h, pl, a);
         }
-#undef FRT_LAUNCH_FAST
-    } else if (pl.n_fft >= 64 && pl.n_fft <= 1024) {
-        const int vec_ok = (((uintptr_t)x_dev & 7) == 0) && ((x_stride & 1) == 0) && ((hop & 1) == 0);
-        const int q = pl.n_fft / 64, gframes = 32 / q;
-        long long blocks = ((total + gframes - 1) / gframes + SMALL_WARPS - 1) / SMALL_WARPS;
-        if (blocks > 2LL * h->sm_count) blocks = 2LL * h->sm_count;
-#define FRT_LAUNCH_SMALL(QQ)                                                                    \
-    launch_small<QQ>(mode, (unsigned)blocks, st, x_dev, x_stride, n_frames, hop, out_dev,        \
-                     out_stride_c, out_stride_f, pl, total, vec_ok)
-        switch (q) {
-            case 1: FRT_LAUNCH_SMALL(1); break;
-            case 2: FRT_LAUNCH_SMALL(2); break;
-            case 4: FRT_LAUNCH_SMALL(4); break;
-            case 8: FRT_LAUNCH_SMALL(8); break;
-            default: FRT_LAUNCH_SMALL(16); break;
-        }
-#undef FRT_LAUNCH_SMALL
-    } else if ((pl.n_fft == 4096 || pl.n_fft == 8192) && (((uintptr_t)x_dev & 7) == 0) &&
-               ((x_stride & 1) == 0) && ((hop & 1) == 0)) {
-        const int r = pl.n_fft / 2048, ng = LARGE_WARPS / r;
-        long long blocks = (total + ng - 1) / ng;
-        if (blocks > h->sm_count) blocks = h->sm_count;
-        if (r == 2)
-            launch_large<2>(mode, (unsigned)blocks, st, x_dev, x_stride, n_frames, hop, out_dev, out_stride_c,
-                            out_stride_f, pl, total);
-        else
-            launch_large<4>(mode, (unsigned)blocks, st, x_dev, x_stride, n_frames, hop, out_dev, out_stride_c,
-                            out_stride_f, pl, total);
-    } else if (pl.n_fft == 4096 || pl.n_fft == 8192 || pl.n_fft == 16384) {
-        const int r = pl.n_fft / 2048;
-        const int vec_ok = (((uintptr_t)x_dev & 7) == 0) && ((x_stride & 1) == 0) && ((hop & 1) == 0);
-        long long blocks = (long long)h->sm_count * (r == 8 ? 2 : (r == 4 ? 4 : 8));
-        if (blocks > total) blocks = total;
-        const float2 *w2 = reinterpret_cast<const float2 *>(pl.win_dev);
-#define FRT_LAUNCH_MULTI(RR, MODE)                                                          \
-    stft_multi_kernel<RR, MODE><<<(unsigned)blocks, 32 * RR, multi_smem(RR), st>>>(          \
-        x_dev, x_stride, n_frames, hop, out_dev, out_stride_c, out_stride_f, w2, pl.tw_dev,  \
-        pl.comb_dev, pl.post_dev, total, vec_ok)
-        if (r == 2) {
-            if (mode == FRT_STFT_POWER) FRT_LAUNCH_MULTI(2, FRT_STFT_POWER);
-            else FRT_LAUNCH_MULTI(2, FRT_STFT_LOGPOWER);
-        } else if (r == 4) {
-            if (mode == FRT_STFT_POWER) FRT_LAUNCH_MULTI(4, FRT_STFT_POWER);
-            else FRT_LAUNCH_MULTI(4, FRT_STFT_LOGPOWER);
-        } else {
-            if (mode == FRT_STFT_POWER) FRT_LAUNCH_MULTI(8, FRT_STFT_POWER);
-            else FRT_LAUNCH_MULTI(8, FRT_STFT_LOGPOWER);
-        }
-#undef FRT_LAUNCH_MULTI
+    } else if ((N == 4096 || N == 8192) && a.vec_ok) {
+        if (N == 4096) launch_large<2>(h, pl, a);
+        else launch_large<4>(h, pl, a);
+    } else if (N >= 4096) {
+        if (N == 4096) launch_multi<2>(h, pl, a);
+        else if (N == 8192) launch_multi<4>(h, pl, a);
+        else launch_multi<8>(h, pl, a);
     } else {
         FRT_CHECK_ARG(h, total <= 0x7fffffffLL, "too many frames for one launch");
-        const int M = pl.n_fft / 2;
+        const int M = N / 2;
         int threads = M / 4;
         if (threads < 32) threads = 32;
         if (threads > 512) threads = 512;
-        stft_generic_kernel<<<(unsigned)total, threads, sizeof(float2) * 2 * M, st>>>(
+        stft_generic_kernel<<<(unsigned)total, threads, sizeof(float2) * 2 * M, a.st>>>(
             x_dev, x_stride, n_frames, hop, out_dev, out_stride_c, out_stride_f, pl.win_dev,
-            pl.tw_dev, pl.post_dev, mode, pl.n_fft, ilog2(M));
+            pl.tw_dev, pl.post_dev, mode, N, ilog2(M));
     }
     h->launches++;
     FRT_CUDA(h, cudaGetLastError());

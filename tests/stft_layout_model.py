@@ -5,14 +5,15 @@ which lane holds which sample, where the split-step partner of a bin lives, wher
 cp.async scatter puts an element -- so that the decompositions are checked against numpy.fft on
 the CPU, independently of the GPU parity tests.
 
-  small_frames(x, Q)   stft_small_kernel<Q>: N = 64 Q, one warp per G = 32/Q frames
+  small_frames(x, Q)   stft_small_kernel<Q>: N = 64 Q, one warp per G = 32/Q frames; Q = 32 is the
+                       N = 2048 path, one frame per warp
   large_frame(x, R)    stft_large_kernel<R>: N = 2048 R, R warps per frame
 Both return |X|^2 / N^2 of the Hann-windowed frame(s), the reference's audioproc.analyzelive
 (friture/audioproc.py:42-50).
 """
 import numpy as np
 
-FAST_TILE = 32 * 33      # float2 elements per warp tile (stft.cu)
+TILE = 32 * 33           # float2 elements per warp tile (stft.cu)
 
 
 def hann(n):
@@ -113,7 +114,7 @@ def large_frame(x, R):
     assert x.shape == (N,)
     z = (x * hann_on_the_fly(R)).reshape(M, 2)
     z = z[:, 0] + 1j * z[:, 1]
-    tiles = np.zeros((R, FAST_TILE), dtype=np.complex128)
+    tiles = np.zeros((R, TILE), dtype=np.complex128)
     for e in range(M):
         w, pos = scatter_position(e, R)
         tiles[w, pos] = z[e]

@@ -16,7 +16,7 @@ def reference(x):
     return np.abs(np.fft.rfft(x * m.hann(n))) ** 2 / n ** 2      # friture/audioproc.py:42-50
 
 
-@pytest.mark.parametrize("Q", [1, 2, 4, 8, 16])
+@pytest.mark.parametrize("Q", [1, 2, 4, 8, 16, 32])
 def test_small_kernel_layout(Q):
     G, N = 32 // Q, 64 * Q
     x = np.random.default_rng(Q).standard_normal((G, N))
@@ -26,7 +26,7 @@ def test_small_kernel_layout(Q):
     assert np.max(np.abs(got - ref)) < 1e-12 * np.max(ref)
 
 
-@pytest.mark.parametrize("Q", [2, 4, 8, 16])
+@pytest.mark.parametrize("Q", [2, 4, 8, 16, 32])
 def test_small_kernel_partner_identity(Q):
     """bin of (lane, register m) + bin of (partner lane, register 31 - m) = M for k1 > 0."""
     M = 32 * Q
@@ -57,7 +57,7 @@ def test_on_the_fly_window_is_the_symmetric_hann(R):
 def test_scatter_is_bank_conflict_free_per_half_warp(R):
     """8-byte shared accesses are served per half-warp: the 16 elements a half-warp scatters must
     fall on 16 different 8-byte bank pairs of the 128-byte bank line."""
-    tile_bytes = m.FAST_TILE * 8
+    tile_bytes = m.TILE * 8
     for base in range(0, 1024 * R, 16):
         pairs = set()
         for e in range(base, base + 16):
@@ -67,4 +67,4 @@ def test_scatter_is_bank_conflict_free_per_half_warp(R):
     # and every element lands inside its tile, below the region the transposes use afterwards
     for e in range(1024 * R):
         w, pos = m.scatter_position(e, R)
-        assert 0 <= pos < m.FAST_TILE
+        assert 0 <= pos < m.TILE
