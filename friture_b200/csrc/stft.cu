@@ -503,7 +503,10 @@ stft_small_kernel(const float *__restrict__ x, long long x_stride, long long n_f
 // the FMA pipe): w[n] = 0.5 - 0.5 cos(theta n), theta = 2 pi/(N-1), and for warp w, lane t, register
 // n1, element e the sample index is n = 64 R n1 + (2 R t + 2 w + e) = A-part + B-part, so
 // cos(theta n) = cos A cos B - sin A sin B with 32 (cos A, sin A)/2 pairs passed as a kernel
-// argument (constant bank) and the four B factors of a lane held in registers.
+// argument (constant bank) and the four B factors of a lane held in registers.  Near both ends of
+// the frame 0.5 - 0.5 cos(theta n) cancels (a relative error of up to 1.5e-2, and w[N-1] = 1e-8
+// instead of 0), so register blocks n1 = 0 and 31 take float32(Hann) from the window table, read
+// once per thread; the other blocks stay within 2.4e-6 of the exact window.
 constexpr int LARGE_WARPS = 16;
 struct HannA {
     float2 v[32];     // (0.5 cos(theta 64 R n1), 0.5 sin(theta 64 R n1))
@@ -535,9 +538,10 @@ template <int R, int MODE>
 __global__ void __launch_bounds__(LARGE_WARPS * 32, 1)
 stft_large_kernel(const float *__restrict__ x, long long x_stride, long long n_frames, int hop,
                   float *__restrict__ out, long long out_stride_c, long long out_stride_f,
-                  const float4 *__restrict__ wlane, const float2 *__restrict__ tw32,
-                  const float2 *__restrict__ comb, const float2 *__restrict__ post,
-                  long long total_items, const __grid_constant__ HannA hann_a) {
+                  const float2 *__restrict__ win2, const float4 *__restrict__ wlane,
+                  const float2 *__restrict__ tw32, const float2 *__restrict__ comb,
+                  const float2 *__restrict__ post, long long total_items,
+                  const __grid_constant__ HannA hann_a) {
     // STAG: 8-byte shared accesses are served per half-warp; the 16/R elements a half-warp sends to
     // each of the R tiles must fall on different banks
     constexpr int M = 1024 * R, N = 2 * M, NG = LARGE_WARPS / R, GT = 32 * R, STAG = 16 / R;
@@ -566,6 +570,8 @@ stft_large_kernel(const float *__restrict__ x, long long x_stride, long long n_f
     long long f = item - c * n_frames;
     const float4 wb = wlane[w * 32 + lane];       // cos B (e = 0, 1), sin B (e = 0, 1)
     const float2 wcb = make_float2(wb.x, wb.y), wsb = make_float2(wb.z, wb.w);
+    // (w[n], w[n+1]) of register blocks 0 and 31: z index R (32 n1 + lane) + w
+    const float2 wfirst = __ldg(win2 + R * lane + w), wlast = __ldg(win2 + R * (32 * 31 + lane) + w);
 
     auto fetch = [&](long long cc, long long ff) {
         const float2 *p2 = reinterpret_cast<const float2 *>(x + cc * x_stride + ff * hop);
@@ -585,9 +591,16 @@ stft_large_kernel(const float *__restrict__ x, long long x_stride, long long n_f
         __syncwarp();                        // inputs are in registers: the tile becomes the exchange buffer
 #pragma unroll
         for (int n1 = 0; n1 < 32; n1++) {
-            const float ca = hann_a.v[n1].x, sa = hann_a.v[n1].y;
-            float2 wv = f2_fma(make_float2(-ca, -ca), wcb, make_float2(0.5f, 0.5f));
-            wv = f2_fma(make_float2(sa, sa), wsb, wv);
+            float2 wv;
+            if (n1 == 0) {
+                wv = wfirst;
+            } else if (n1 == 31) {
+                wv = wlast;
+            } else {
+                const float ca = hann_a.v[n1].x, sa = hann_a.v[n1].y;
+                wv = f2_fma(make_float2(-ca, -ca), wcb, make_float2(0.5f, 0.5f));
+                wv = f2_fma(make_float2(sa, sa), wsb, wv);
+            }
             v[n1] = f2_mul(v[n1], wv);
         }
         dft32(v);
@@ -779,8 +792,9 @@ void launch_large(const frt_ctx *h, const StftPlan &pl, const Frames &a) {
     }
     with_mode(a.mode, [&](auto m) {
         stft_large_kernel<R, decltype(m)::value><<<(unsigned)blocks, LARGE_WARPS * 32, large_smem<R>(), a.st>>>(
-            a.x, a.x_stride, a.n_frames, a.hop, a.out, a.osc, a.osf, pl.wlane_dev, pl.tw_dev, pl.comb_dev,
-            pl.post_dev, a.total, ha);
+            a.x, a.x_stride, a.n_frames, a.hop, a.out, a.osc, a.osf,
+            reinterpret_cast<const float2 *>(pl.win_dev), pl.wlane_dev, pl.tw_dev, pl.comb_dev, pl.post_dev,
+            a.total, ha);
     });
 }
 template <int R>

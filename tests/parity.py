@@ -78,3 +78,41 @@ def assert_logpower_parity(got_db, ref_db, min_frac=0.9999, strict=None, floor_d
         strict = np.asarray(ref_db).size <= STRICT_MAX_BINS and min_frac > 0
     assert logpower_ok(e, min_frac, strict), e
     return e
+
+
+# Power mode (|X|^2 / N^2, no log) is judged bin by bin on the amplitude scale:
+#     |sqrt(P[k]) - sqrt(Pr[k])| <= AMP_TOL * rms + REL_AMP_TOL * sqrt(Pr[k])
+# with rms = sqrt(mean_k Pr[k]) of the frame.  AMP_TOL is the float32 transform's amplitude noise
+# allowance above; REL_AMP_TOL covers the rounding of a strong bin's own value (float32 window,
+# |X|^2 and the 1/N^2 scale).  The bound is scale-free, so it means the same at every FFT size and
+# level, and a frame whose reference is exactly zero must come out exactly zero.  numpy's float32
+# rfft of float32-windowed frames uses at most 8 % of it on noise, tones, bin-centred cosines, a
+# Nyquist sequence and impulses at N = 32 .. 16384 (tests/test_stft_bins_gpu.py checks that, and
+# what the bound rejects).
+REL_AMP_TOL = 1e-6
+
+
+def power_errors(got, ref):
+    """got, ref: [..., bins] power.  Returns worst_ratio (largest error over the bound above, inf
+    for a NaN, a negative value, or anything but 0 where the reference frame is exactly 0) and the
+    index of that bin."""
+    got = np.asarray(got, dtype=np.float64)
+    ref = np.asarray(ref, dtype=np.float64)
+    assert got.shape == ref.shape, (got.shape, ref.shape)
+    if got.size == 0:
+        return {"worst_ratio": 0.0, "worst_index": None}
+    amp_ref = np.sqrt(ref)
+    rms = np.sqrt(np.mean(ref, axis=-1, keepdims=True))
+    allowed = AMP_TOL * rms + REL_AMP_TOL * amp_ref
+    with np.errstate(invalid="ignore", divide="ignore"):
+        err = np.abs(np.sqrt(got) - amp_ref)
+        ratio = np.where(allowed > 0, err / allowed, np.where(err == 0, 0.0, np.inf))
+    ratio = np.where(np.isnan(ratio), np.inf, ratio)
+    i = int(np.argmax(ratio))
+    return {"worst_ratio": float(ratio.flat[i]), "worst_index": np.unravel_index(i, ratio.shape)}
+
+
+def assert_power_parity(got, ref):
+    e = power_errors(got, ref)
+    assert e["worst_ratio"] <= 1.0, e
+    return e

@@ -88,11 +88,16 @@ def small_frames(x, Q):
 
 def hann_on_the_fly(R):
     """The window as stft_large_kernel computes it: n = 64 R n1 + (2 R t + 2 w + e),
-    cos(theta n) = cos A cos B - sin A sin B.  Returns w[n] for n < N."""
+    cos(theta n) = cos A cos B - sin A sin B, except register blocks 0 and 31, which read the window
+    table (the formula cancels there).  Returns w[n] for n < N."""
     N = 2048 * R
     theta = 2.0 * np.pi / (N - 1)
     out = np.zeros(N)
     for n1 in range(32):
+        if n1 in (0, 31):
+            blk = slice(64 * R * n1, 64 * R * (n1 + 1))
+            out[blk] = hann(N)[blk]
+            continue
         ca, sa = 0.5 * np.cos(theta * 64 * R * n1), 0.5 * np.sin(theta * 64 * R * n1)
         for w in range(R):
             for t in range(32):

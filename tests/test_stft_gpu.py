@@ -9,7 +9,7 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
 pytestmark = pytest.mark.gpu
 
-from parity import TOL, rel_err, assert_logpower_parity  # noqa: E402
+from parity import TOL, assert_logpower_parity, assert_power_parity  # noqa: E402
 
 
 def make_input(kind, C, T, seed):
@@ -42,7 +42,7 @@ def test_power_all_sizes(n_fft):
     got = run_gpu(x, n_fft, n_fft // 4, log=False)       # 75 % overlap (spectrum.py:66)
     ref = fo.stft_power_batch(x, n_fft, n_fft // 4)
     assert got.shape == ref.shape
-    assert rel_err(got, ref) < TOL
+    assert_power_parity(got, ref)
     got = run_gpu(x, n_fft, n_fft // 4, log=True)
     # few bins per frame at the small sizes: allow more of them below the floor
     assert_logpower_parity(got, fo.log_spectrogram(ref), min_frac=0.95 if n_fft < 1024 else 0.9999)
@@ -109,7 +109,7 @@ def test_analyzelive_dropin_plumbing():
     assert sp.dtype == np.float64 and sp.shape == (513,)
     ref = fo.analyzelive(x.astype(np.float32))
     assert_logpower_parity(10 * np.log10(sp + 1e-30), fo.log_spectrogram(ref))
-    assert rel_err(sp, ref) < TOL
+    assert_power_parity(sp, ref)
     with pytest.raises(ValueError):
         proc.analyzelive(x[:100])
 
@@ -171,7 +171,7 @@ def test_ragged_frame_counts_all_kernels(n_fft, hop, C, F):
     got = run_gpu(x, n_fft, hop, log=False)
     ref = fo.stft_power_batch(x, n_fft, hop)
     assert got.shape == ref.shape == (C, F, n_fft // 2 + 1)
-    assert rel_err(got, ref) < TOL
+    assert_power_parity(got, ref)
     got = run_gpu(x, n_fft, hop, log=True)
     assert_logpower_parity(got, fo.log_spectrogram(ref), min_frac=0.95 if n_fft < 1024 else 0.9999)
 

@@ -10,12 +10,17 @@ from friture_b200.correlation import GccPhat
 
 torch.manual_seed(0)
 p = audioproc()
-for n in (2048, 1024, 64):
+# every STFT instance once: all ten sizes x both modes x 16-, 8- and 4-byte aligned frames (first
+# sample at float offset 0, 2, 1 of a 16-byte aligned buffer whose row stride is a multiple of 4)
+for n in (32, 64, 128, 256, 512, 1024, 2048, 4096, 8192, 16384):
     p.set_fftsize(n)
-    x = torch.randn(3, n + 5 * (n // 2), device="cuda") * 0.1
-    p.stft(x, hop=n // 2, log=True)
-    p.stft(x[:, 1:], hop=n // 2, log=False)
-    p.stft_host(x.cpu().numpy(), hop=n // 2)
+    T = n + 5 * (n // 2)
+    x = torch.randn(3, T + 4, device="cuda") * 0.1
+    for off in (0, 2, 1):
+        for log in (False, True):
+            p.stft(x[:, off:off + T], hop=n // 2, log=log)
+p.set_fftsize(2048)
+p.stft_host(x[:, :2048 * 3].cpu().numpy(), hop=1024)
 for block in (256, 512, 1024):      # 256 / 512: the three-warp scan kernel, 1024: the one-warp kernel
     bank = Octave_Filters(3)
     x = torch.randn(3, 2 * block, device="cuda") * 0.1
