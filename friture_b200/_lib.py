@@ -4,7 +4,7 @@ from __future__ import annotations
 import ctypes
 import os
 import threading
-from ctypes import (POINTER, c_char_p, c_float, c_int, c_int64, c_size_t, c_void_p)
+from ctypes import (POINTER, c_char_p, c_double, c_float, c_int, c_int64, c_size_t, c_void_p)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB_NAME = "libfrt_b200.so"
@@ -88,6 +88,9 @@ SIGNATURES = {
     "frt_spectrum_reduce_dual": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int, c_int,
                                          c_int, c_float, c_void_p, c_void_p, c_void_p, c_void_p,
                                          c_void_p, c_void_p]),
+    "frt_plot_curves": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int, c_int, c_int, c_double,
+                                c_double, c_double, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                                c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "frt_decimate_plan": (c_int, [c_void_p, c_int, c_int, c_void_p]),
     "frt_decimate_process": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_int64, c_void_p]),
     "frt_display_columns": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int, c_int, c_int,

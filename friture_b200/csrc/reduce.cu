@@ -195,6 +195,108 @@ extern "C" int frt_spectrum_reduce_dual(frt_handle h, const float *power1_dev,
 }
 
 // ---------------------------------------------------------------------------------------------
+// Plotted curves and peak hold of the spectrum and octave widgets (SpectrumPlotWidget.setdata and
+// compute_peaks, friture/spectrumPlotWidget.py:122-200; HistPlot.setdata and compute_peaks,
+// friture/histplot.py:77-130).  One CTA per channel; each bin's peak state is stepped through the
+// call's dB vectors in registers, read once and written once.  All arithmetic in double with the
+// rounding intrinsics, so that no contraction changes a bit against the reference's NumPy.
+namespace {
+
+// 1 - toScreen(v) on the linear vertical scale of range [m, mx] (plotting/coordinateTransform.py:
+// 62-83 with length 1 and no borders: (v - m) * 1 / (mx - m) + 0); toScreen is 0 when mx == m.
+__device__ __forceinline__ double screen_y(double v, double m, double mx) {
+    if (mx == m) return 1.0;
+    return __dsub_rn(1.0, __ddiv_rn(__dsub_rn(v, m), __dsub_rn(mx, m)));
+}
+
+__global__ void __launch_bounds__(256)
+plot_curves_kernel(const float *__restrict__ y, long long stride_c, long long stride_s, int n_steps,
+                   int nbins, double m, double mx, double d0, int peaks, int reset,
+                   double *__restrict__ peak, double *__restrict__ peak_int,
+                   double *__restrict__ decay, float *__restrict__ scaled_y, float *__restrict__ z,
+                   float *__restrict__ scaled_peak, float *__restrict__ z_peak) {
+    __shared__ float s_max[32];
+    const int c = blockIdx.x;
+    const float *yc = y + (size_t)c * stride_c;
+    const float *ylast = yc + (size_t)(n_steps - 1) * stride_s;
+    const size_t o = (size_t)c * nbins;
+    float best = -INFINITY;
+    for (int k = threadIdx.x; k < nbins; k += blockDim.x) {
+        const double v = __ldg(ylast + k);
+        best = fmaxf(best, (float)v);
+        scaled_y[o + k] = (float)screen_y(v, m, mx);
+        if (!peaks) continue;         // compute_peaks is not called: the state stays frozen
+        double p = -500.0, pi = 0.0, dk = d0;     // the reset of compute_peaks
+        if (!reset) {
+            p = peak[o + k];
+            pi = peak_int[o + k];
+            dk = decay[o + k];
+        }
+        for (int s = 0; s < n_steps; s++) {
+            const double ys = __ldg(yc + (size_t)s * stride_s + k);
+            if (p < ys) {             // rise
+                p = ys;
+                pi = 1.0;
+                dk = d0;
+            } else if (pi < 0.2) {    // fall, faster every step
+                p = __dadd_rn(p, dk);
+                dk = __dadd_rn(dk, d0);
+            } else {                  // hold
+                pi = __dmul_rn(pi, 0.975);
+            }
+        }
+        peak[o + k] = p;
+        peak_int[o + k] = pi;
+        decay[o + k] = dk;
+        scaled_peak[o + k] = (float)screen_y(p, m, mx);
+        z_peak[o + k] = (float)pi;
+    }
+    // M = max(y) of the last step; the max of float32 values is exact
+    for (int off = 16; off > 0; off >>= 1) best = fmaxf(best, __shfl_xor_sync(0xffffffffu, best, off));
+    const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
+    if (l == 0) s_max[w] = best;
+    __syncthreads();
+    if (w == 0) {
+        best = l < (int)(blockDim.x >> 5) ? s_max[l] : -INFINITY;
+        for (int off = 16; off > 0; off >>= 1)
+            best = fmaxf(best, __shfl_xor_sync(0xffffffffu, best, off));
+        if (l == 0) s_max[0] = best;
+    }
+    __syncthreads();
+    // z = (y - m) / (|M - m| + 1e-3)
+    const double den = __dadd_rn(fabs(__dsub_rn((double)s_max[0], m)), 1e-3);
+    for (int k = threadIdx.x; k < nbins; k += blockDim.x)
+        z[o + k] = (float)__ddiv_rn(__dsub_rn((double)__ldg(ylast + k), m), den);
+}
+
+}   // namespace
+
+extern "C" int frt_plot_curves(frt_handle h, const float *y_dev, int64_t stride_c, int64_t stride_s,
+                               int n_channels, int n_steps, int nbins, double spec_min,
+                               double spec_max, double d0, int peaks, int reset, double *peak_dev,
+                               double *peak_int_dev, double *decay_dev, float *scaled_y_dev,
+                               float *z_dev, float *scaled_peak_dev, float *z_peak_dev,
+                               void *stream) {
+    if (!h) return FRT_EINVAL;
+    DeviceGuard g(h->device);
+    FRT_CHECK_ARG(h, n_channels >= 0 && n_steps >= 1 && nbins >= 1, "bad shape");
+    // y is only read, so rows may overlap (a broadcast dB vector has stride 0)
+    FRT_CHECK_ARG(h, stride_c >= 0 && stride_s >= 0, "negative stride");
+    FRT_CHECK_ARG(h, spec_min <= spec_max, "spec_min > spec_max");
+    if (n_channels == 0) return FRT_OK;
+    FRT_CHECK_ARG(h, y_dev && scaled_y_dev && z_dev, "NULL buffer");
+    FRT_CHECK_ARG(h, !peaks || (peak_dev && peak_int_dev && decay_dev && scaled_peak_dev && z_peak_dev),
+                  "NULL peak buffer");
+    plot_curves_kernel<<<n_channels, 256, 0, (cudaStream_t)stream>>>(
+        y_dev, stride_c, stride_s, n_steps, nbins, spec_min, spec_max, d0, peaks ? 1 : 0,
+        reset ? 1 : 0, peak_dev, peak_int_dev, decay_dev, scaled_y_dev, z_dev, scaled_peak_dev,
+        z_peak_dev);
+    h->launches++;
+    FRT_CUDA(h, cudaGetLastError());
+    return FRT_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
 // Spectrogram display chain (SURVEY 8f-2): dB + weighting -> [0,1] scaling
 // (friture/spectrogram.py:127-129,161-162) -> frequency-axis interpolation to the screen rows
 // (np.interp on a Mel/Log/... grid, friture/signal/frequency_resampler.py:67-83) -> online linear

@@ -249,6 +249,29 @@ int frt_spectrum_reduce_dual(frt_handle h, const float *power1_dev, const float 
                              int nbins, float alpha, float *disp1_dev, float *disp2_dev,
                              float *db_dev, int *fmax_idx_dev, int *pitch_idx_dev, void *stream);
 
+/* ---------------------------------------------------------------- plotted curves and peak hold
+ * The last numeric step of the spectrum and octave widgets: SpectrumPlotWidget.setdata and
+ * compute_peaks (friture/spectrumPlotWidget.py:122-200), HistPlot.setdata and compute_peaks
+ * (friture/histplot.py:77-130), with the linear vertical scale of
+ * friture/plotting/coordinateTransform.py:62-83.  Per channel, the peak state machine is run over
+ * the n_steps dB vectors in order (rise when peak < y: peak = y, peak_int = 1, decay = d0; else
+ * when peak_int < 0.2: peak += decay, decay += d0; else peak_int *= 0.975), in double.  Then, for
+ * the last step only: scaled_y = 1 - (y - spec_min) / (spec_max - spec_min) (1 when the range is
+ * empty), z = (y - spec_min) / (|max(y) - spec_min| + 1e-3), scaled_peak = 1 - toScreen(peak),
+ * z_peak = peak_int, all rounded once to float32.
+ *   y_dev [C][n_steps][nbins] dB (strides in floats, >= 0; y is only read, so rows may overlap);
+ *   spec_min <= spec_max (the widget's setspecrange sorts them); d0 the decay step
+ *   20*log10(1 - 3e-6)*5000, computed by the caller.
+ *   peak_dev / peak_int_dev / decay_dev [C][nbins] state in/out; reset != 0 starts it from the
+ *   widget's reset (-500, 0, d0) instead of reading it.  peaks == 0: compute_peaks is skipped, the
+ *   state and the peak outputs are neither read nor written (they may be NULL).
+ *   scaled_y_dev / z_dev / scaled_peak_dev / z_peak_dev [C][nbins] float32.                      */
+int frt_plot_curves(frt_handle h, const float *y_dev, int64_t stride_c, int64_t stride_s,
+                    int n_channels, int n_steps, int nbins, double spec_min, double spec_max,
+                    double d0, int peaks, int reset, double *peak_dev, double *peak_int_dev,
+                    double *decay_dev, float *scaled_y_dev, float *z_dev, float *scaled_peak_dev,
+                    float *z_peak_dev, void *stream);
+
 /* ---------------------------------------------------------------- spectrogram display chain
  * The Transform_Pipeline behind the spectrogram (friture/spectrogram.py:161-169): scaling of
  * dB + weighting to [0,1] (spectrogram.py:127-129), Frequency_Resampler.push
