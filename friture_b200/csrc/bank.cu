@@ -309,7 +309,10 @@ __device__ __forceinline__ void serial_stages(float xin, int n, const W &w, int 
         }
         const float om = P.omq[j][0];
         const float gout = is_band ? P.gband[is_band ? lane : 0] : P.gdec;   // chain gain
-        float e = is_band ? w.s_e[j * bpo + lane] : 0.f;
+        // smoothing: this call's n samples are summed from zero and folded into the carried e once
+        // (e <- q^n e + s, complement form), as the scan-mode stages do per chunk; a per-sample
+        // recursion on the carried e rounds it once per sample over the 1/alpha samples it remembers
+        float s = 0.f;
         const int kband = (P.n_oct - 1 - j) * bpo + (is_band ? lane : 0);
         float *yp = nullptr;
         if constexpr (W::kWantY) {
@@ -329,7 +332,7 @@ __device__ __forceinline__ void serial_stages(float xin, int n, const W &w, int 
                 }
             }
             if (is_band) {
-                e = fmaf(-om, e, e) + v * v;      // raw units; gain applied to the outputs
+                s = fmaf(-om, s, s) + v * v;      // raw units; gain applied to the outputs
                 if constexpr (W::kWantY) {
                     if (yp) yp[m] = v * gout;
                 }
@@ -351,6 +354,8 @@ __device__ __forceinline__ void serial_stages(float xin, int n, const W &w, int 
             }
         }
         if (is_band) {
+            float e = w.s_e[j * bpo + lane];
+            e = fmaf(-P.omq[j][__ffs(n) - 1], e, e) + s;   // n is a power of two, at most 32
             w.s_e[j * bpo + lane] = e;
             if (w.energies) w.energies[kband] = energy_out(P.alpha[j] * gout * gout * e, w.db, w.weight, kband);
         }
