@@ -1,4 +1,4 @@
-// Handle lifecycle, error reporting and the host-staging pipeline of libfrt_b200.so.
+// Handle lifecycle, error reporting and the NVLink peer buffers of libfrt_b200.so.
 #include <cstdarg>
 #include <mutex>
 
@@ -52,63 +52,11 @@ extern "C" int frt_create(int device, frt_handle *out) {
     return FRT_OK;
 }
 
-static void pipe_release(frt_ctx *h) {
-    HostPipe &p = h->pipe;
-    for (int i = 0; i < 2; i++) {
-        if (p.d_in[i]) cudaFree(p.d_in[i]);
-        if (p.d_out[i]) cudaFree(p.d_out[i]);
-        if (p.ev_in[i]) cudaEventDestroy(p.ev_in[i]);
-        if (p.ev_cmp[i]) cudaEventDestroy(p.ev_cmp[i]);
-        if (p.ev_out[i]) cudaEventDestroy(p.ev_out[i]);
-    }
-    if (p.s_in) cudaStreamDestroy(p.s_in);
-    if (p.s_cmp) cudaStreamDestroy(p.s_cmp);
-    if (p.s_out) cudaStreamDestroy(p.s_out);
-    p = HostPipe();
-}
-
-int frt_pipe_ensure(frt_ctx *h, size_t in_bytes, size_t out_bytes) {
-    HostPipe &p = h->pipe;
-    if (!p.s_in) {
-        FRT_CUDA(h, cudaStreamCreateWithFlags(&p.s_in, cudaStreamNonBlocking));
-        FRT_CUDA(h, cudaStreamCreateWithFlags(&p.s_cmp, cudaStreamNonBlocking));
-        FRT_CUDA(h, cudaStreamCreateWithFlags(&p.s_out, cudaStreamNonBlocking));
-        for (int i = 0; i < 2; i++) {
-            FRT_CUDA(h, cudaEventCreateWithFlags(&p.ev_in[i], cudaEventDisableTiming));
-            FRT_CUDA(h, cudaEventCreateWithFlags(&p.ev_cmp[i], cudaEventDisableTiming));
-            FRT_CUDA(h, cudaEventCreateWithFlags(&p.ev_out[i], cudaEventDisableTiming));
-        }
-    }
-    if (in_bytes > p.in_bytes) {
-        for (int i = 0; i < 2; i++) {
-            if (p.d_in[i]) cudaFree(p.d_in[i]);
-            p.d_in[i] = nullptr;
-            FRT_CUDA(h, cudaMalloc(&p.d_in[i], in_bytes));
-        }
-        p.in_bytes = in_bytes;
-    }
-    if (out_bytes > p.out_bytes) {
-        for (int i = 0; i < 2; i++) {
-            if (p.d_out[i]) cudaFree(p.d_out[i]);
-            p.d_out[i] = nullptr;
-            FRT_CUDA(h, cudaMalloc(&p.d_out[i], out_bytes));
-        }
-        p.out_bytes = out_bytes;
-    }
-    return FRT_OK;
-}
-
+// the handle's members free its plans, buffers, streams and events on the handle's device
 extern "C" int frt_destroy(frt_handle h) {
     if (!h) return FRT_OK;
     DeviceGuard g(h->device);
     cudaDeviceSynchronize();
-    for (auto &kv : h->stft_cache) frt_stft_free_plan(kv.second);
-    frt_bank_release(h);
-    frt_gcc_release(h);
-    frt_dec_release(h);
-    frt_comb_release(h);
-    frt_fir_release(h);
-    pipe_release(h);
     delete h;
     return FRT_OK;
 }

@@ -523,14 +523,7 @@ decimate_kernel(const __grid_constant__ BankParams P, const DecArgs a) {
 
 }   // namespace
 
-void frt_bank_release(frt_ctx *h) {
-    if (!h->bank) return;
-    if (h->bank->zstate) cudaFree(h->bank->zstate);
-    if (h->bank->ema) cudaFree(h->bank->ema);
-    if (h->bank->weight) cudaFree(h->bank->weight);
-    delete h->bank;
-    h->bank = nullptr;
-}
+void PlanDelete::operator()(BankPlan *p) const { delete p; }
 
 static void mat2_mul(const double a[4], const double b[4], double o[4]) {
     o[0] = a[0] * b[0] + a[1] * b[2];
@@ -572,8 +565,7 @@ extern "C" int frt_bank_plan(frt_handle h, int n_channels, int bands_per_octave,
                   "bands_per_octave must be in [1, 24]");
     FRT_CHECK_ARG(h, n_octaves >= 1 && n_octaves <= MAX_OCT, "n_octaves must be in [1, 10]");
     FRT_CHECK_ARG(h, sos_band && sos_dec && alphas, "NULL coefficient table");
-    frt_bank_release(h);
-    BankPlan *pl = new (std::nothrow) BankPlan();
+    PlanPtr<BankPlan> pl(new (std::nothrow) BankPlan());
     if (!pl) return frt_fail(h, FRT_ENOMEM, "out of host memory");
     BankParams &P = pl->params;
     memset(&P, 0, sizeof(P));
@@ -586,19 +578,15 @@ extern "C" int frt_bank_plan(frt_handle h, int n_channels, int bands_per_octave,
         const double *s = sec < 2 * bands_per_octave ? sos_band + (size_t)sec * 6
                                                      : sos_dec + (size_t)(sec - 2 * bands_per_octave) * 6;
         double g;
-        if (const char *why = set_section(P, sec, s, &g)) {
-            delete pl;
+        if (const char *why = set_section(P, sec, s, &g))
             return frt_fail(h, FRT_EINVAL, "SOS section %d: %s", sec, why);
-        }
         gchain[sec < 2 * bands_per_octave ? sec / 2 : bands_per_octave] *= g;
     }
     for (int i = 0; i < bands_per_octave; i++) P.gband[i] = (float)gchain[i];
     P.gdec = (float)gchain[bands_per_octave];
     for (int j = 0; j < n_octaves; j++) {
-        if (!(alphas[j] > 0.0 && alphas[j] <= 1.0)) {
-            delete pl;
+        if (!(alphas[j] > 0.0 && alphas[j] <= 1.0))
             return frt_fail(h, FRT_EINVAL, "alpha[%d] must be in (0, 1]", j);
-        }
         P.alpha[j] = (float)alphas[j];
         pl->alphas[j] = alphas[j];
         double q = 1.0 - alphas[j];
@@ -607,23 +595,17 @@ extern "C" int frt_bank_plan(frt_handle h, int n_channels, int bands_per_octave,
             q *= q;
         }
     }
-    frt_pipe_prepare(pl);
+    frt_pipe_prepare(pl.get());
     pl->n_channels = n_channels;
     pl->nz = (size_t)n_octaves * P.nsec * 2;
     pl->ne = (size_t)n_octaves * bands_per_octave;
-    cudaError_t e = cudaMalloc(&pl->zstate, sizeof(float) * pl->nz * n_channels);
-    if (e == cudaSuccess) e = cudaMalloc(&pl->ema, sizeof(float) * pl->ne * n_channels);
-    if (e == cudaSuccess) e = cudaMemset(pl->zstate, 0, sizeof(float) * pl->nz * n_channels);
-    if (e == cudaSuccess) e = cudaMemset(pl->ema, 0, sizeof(float) * pl->ne * n_channels);
+    FRT_CUDA(h, pl->zstate.alloc(pl->nz * n_channels));
+    FRT_CUDA(h, pl->ema.alloc(pl->ne * n_channels));
+    FRT_CUDA(h, cudaMemset(pl->zstate.get(), 0, sizeof(float) * pl->nz * n_channels));
+    FRT_CUDA(h, cudaMemset(pl->ema.get(), 0, sizeof(float) * pl->ne * n_channels));
     // the memsets run on the legacy stream; callers process on their own (possibly non-blocking) streams
-    if (e == cudaSuccess) e = cudaDeviceSynchronize();
-    if (e != cudaSuccess) {
-        if (pl->zstate) cudaFree(pl->zstate);
-        if (pl->ema) cudaFree(pl->ema);
-        delete pl;
-        return frt_fail(h, FRT_ECUDA, "frt_bank_plan: %s", cudaGetErrorString(e));
-    }
-    h->bank = pl;
+    FRT_CUDA(h, cudaDeviceSynchronize());
+    h->bank = std::move(pl);
     return FRT_OK;
 }
 
@@ -631,9 +613,9 @@ extern "C" int frt_bank_reset(frt_handle h) {
     if (!h) return FRT_EINVAL;
     if (!h->bank) return frt_fail(h, FRT_ESTATE, "frt_bank_reset: no plan");
     DeviceGuard g(h->device);
-    BankPlan *pl = h->bank;
-    FRT_CUDA(h, cudaMemset(pl->zstate, 0, sizeof(float) * pl->nz * pl->n_channels));
-    FRT_CUDA(h, cudaMemset(pl->ema, 0, sizeof(float) * pl->ne * pl->n_channels));
+    BankPlan *pl = h->bank.get();
+    FRT_CUDA(h, cudaMemset(pl->zstate.get(), 0, sizeof(float) * pl->nz * pl->n_channels));
+    FRT_CUDA(h, cudaMemset(pl->ema.get(), 0, sizeof(float) * pl->ne * pl->n_channels));
     FRT_CUDA(h, cudaDeviceSynchronize());
     return FRT_OK;
 }
@@ -642,16 +624,15 @@ extern "C" int frt_bank_set_weighting(frt_handle h, const float *weight_db_host)
     if (!h) return FRT_EINVAL;
     if (!h->bank) return frt_fail(h, FRT_ESTATE, "frt_bank_set_weighting: no plan");
     DeviceGuard g(h->device);
-    BankPlan *pl = h->bank;
+    BankPlan *pl = h->bank.get();
     const size_t nb = (size_t)pl->params.n_oct * pl->params.bpo;
     FRT_CUDA(h, cudaDeviceSynchronize());
     if (!weight_db_host) {
-        if (pl->weight) cudaFree(pl->weight);
-        pl->weight = nullptr;
+        pl->weight = {};
         return FRT_OK;
     }
-    if (!pl->weight) FRT_CUDA(h, cudaMalloc(&pl->weight, sizeof(float) * nb));
-    FRT_CUDA(h, cudaMemcpy(pl->weight, weight_db_host, sizeof(float) * nb, cudaMemcpyHostToDevice));
+    if (!pl->weight.get()) FRT_CUDA(h, pl->weight.alloc(nb));
+    FRT_CUDA(h, cudaMemcpy(pl->weight.get(), weight_db_host, sizeof(float) * nb, cudaMemcpyHostToDevice));
     return FRT_OK;
 }
 
@@ -678,13 +659,13 @@ extern "C" int frt_bank_get_state(frt_handle h, float *z_host, float *ema_host) 
     if (!h) return FRT_EINVAL;
     if (!h->bank) return frt_fail(h, FRT_ESTATE, "frt_bank_get_state: no plan");
     DeviceGuard g(h->device);
-    BankPlan *pl = h->bank;
+    BankPlan *pl = h->bank.get();
     FRT_CUDA(h, cudaDeviceSynchronize());
     if (z_host)
-        FRT_CUDA(h, cudaMemcpy(z_host, pl->zstate, sizeof(float) * pl->nz * pl->n_channels,
+        FRT_CUDA(h, cudaMemcpy(z_host, pl->zstate.get(), sizeof(float) * pl->nz * pl->n_channels,
                                cudaMemcpyDeviceToHost));
     if (ema_host)
-        FRT_CUDA(h, cudaMemcpy(ema_host, pl->ema, sizeof(float) * pl->ne * pl->n_channels,
+        FRT_CUDA(h, cudaMemcpy(ema_host, pl->ema.get(), sizeof(float) * pl->ne * pl->n_channels,
                                cudaMemcpyDeviceToHost));
     return FRT_OK;
 }
@@ -693,13 +674,13 @@ extern "C" int frt_bank_set_state(frt_handle h, const float *z_host, const float
     if (!h) return FRT_EINVAL;
     if (!h->bank) return frt_fail(h, FRT_ESTATE, "frt_bank_set_state: no plan");
     DeviceGuard g(h->device);
-    BankPlan *pl = h->bank;
+    BankPlan *pl = h->bank.get();
     FRT_CUDA(h, cudaDeviceSynchronize());
     if (z_host)
-        FRT_CUDA(h, cudaMemcpy(pl->zstate, z_host, sizeof(float) * pl->nz * pl->n_channels,
+        FRT_CUDA(h, cudaMemcpy(pl->zstate.get(), z_host, sizeof(float) * pl->nz * pl->n_channels,
                                cudaMemcpyHostToDevice));
     if (ema_host)
-        FRT_CUDA(h, cudaMemcpy(pl->ema, ema_host, sizeof(float) * pl->ne * pl->n_channels,
+        FRT_CUDA(h, cudaMemcpy(pl->ema.get(), ema_host, sizeof(float) * pl->ne * pl->n_channels,
                                cudaMemcpyHostToDevice));
     return FRT_OK;
 }
@@ -772,7 +753,7 @@ static int bank_process_impl(frt_handle h, const float *x_dev, int64_t x_stride,
     if (!h) return FRT_EINVAL;
     if (!h->bank) return frt_fail(h, FRT_ESTATE, "frt_bank_process: call frt_bank_plan first");
     DeviceGuard g(h->device);
-    BankPlan *pl = h->bank;
+    BankPlan *pl = h->bank.get();
     const BankParams &P = pl->params;
     FRT_CHECK_ARG(h, n_blocks >= 0 && block >= 0, "negative shape");
     if (n_blocks == 0 || block == 0) return FRT_OK;   // empty chunk: octavespectrum.py:94-95
@@ -795,8 +776,8 @@ static int bank_process_impl(frt_handle h, const float *x_dev, int64_t x_stride,
     a.n_channels = pl->n_channels;
     a.n_tiles = (int)(t_total / tile);
     a.tiles_per_block = block / tile;
-    a.zstate = pl->zstate;
-    a.ema = pl->ema;
+    a.zstate = pl->zstate.get();
+    a.ema = pl->ema.get();
     a.energies = energies_dev;
     a.e_stride = e_stride;
     a.y = y_dev;
@@ -804,7 +785,7 @@ static int bank_process_impl(frt_handle h, const float *x_dev, int64_t x_stride,
     a.t_total = t_total;
     a.db = db;
     a.vec_ok = (((uintptr_t)x_dev & 15) == 0) && ((x_stride & 3) == 0);
-    a.weight = db ? pl->weight : nullptr;
+    a.weight = db ? pl->weight.get() : nullptr;
     a.block = block;
     a.n_blocks = n_blocks;
     a.n_steps = 0;
@@ -836,16 +817,10 @@ static int bank_process_impl(frt_handle h, const float *x_dev, int64_t x_stride,
 struct DecPlan {
     BankParams params;
     int n_channels = 0, n_stages = 0;
-    float *zstate = nullptr;
+    DeviceArray<float> zstate;
 };
 
-void frt_dec_release(frt_ctx *h) {
-    DecPlan *pl = reinterpret_cast<DecPlan *>(h->dec);
-    if (!pl) return;
-    if (pl->zstate) cudaFree(pl->zstate);
-    delete pl;
-    h->dec = nullptr;
-}
+void PlanDelete::operator()(DecPlan *p) const { delete p; }
 
 extern "C" int frt_decimate_plan(frt_handle h, int n_channels, int n_stages, const double *sos_dec) {
     if (!h) return FRT_EINVAL;
@@ -853,8 +828,7 @@ extern "C" int frt_decimate_plan(frt_handle h, int n_channels, int n_stages, con
     FRT_CHECK_ARG(h, n_channels >= 1, "n_channels must be >= 1");
     FRT_CHECK_ARG(h, n_stages >= 1 && n_stages <= 2, "n_stages must be 1 or 2");
     FRT_CHECK_ARG(h, sos_dec != nullptr, "NULL coefficient table");
-    frt_dec_release(h);
-    DecPlan *pl = new (std::nothrow) DecPlan();
+    PlanPtr<DecPlan> pl(new (std::nothrow) DecPlan());
     if (!pl) return frt_fail(h, FRT_ENOMEM, "out of host memory");
     BankParams &P = pl->params;
     memset(&P, 0, sizeof(P));
@@ -864,26 +838,19 @@ extern "C" int frt_decimate_plan(frt_handle h, int n_channels, int n_stages, con
     double gdec = 1.0;
     for (int sec = 0; sec < 6; sec++) {
         double g;
-        if (const char *why = set_section(P, sec, sos_dec + (size_t)sec * 6, &g)) {
-            delete pl;
+        if (const char *why = set_section(P, sec, sos_dec + (size_t)sec * 6, &g))
             return frt_fail(h, FRT_EINVAL, "decimator section %d is not of the form g(1,c,1)/(1,a1,a2): %s",
                             sec, why);
-        }
         gdec *= g;
     }
     P.gdec = (float)gdec;
     pl->n_channels = n_channels;
     pl->n_stages = n_stages;
     const size_t nz = (size_t)n_stages * 6 * 2 * n_channels;
-    cudaError_t e = cudaMalloc(&pl->zstate, sizeof(float) * nz);
-    if (e == cudaSuccess) e = cudaMemset(pl->zstate, 0, sizeof(float) * nz);
-    if (e == cudaSuccess) e = cudaDeviceSynchronize();
-    if (e != cudaSuccess) {
-        if (pl->zstate) cudaFree(pl->zstate);
-        delete pl;
-        return frt_fail(h, FRT_ECUDA, "frt_decimate_plan: %s", cudaGetErrorString(e));
-    }
-    h->dec = pl;
+    FRT_CUDA(h, pl->zstate.alloc(nz));
+    FRT_CUDA(h, cudaMemset(pl->zstate.get(), 0, sizeof(float) * nz));
+    FRT_CUDA(h, cudaDeviceSynchronize());
+    h->dec = std::move(pl);
     return FRT_OK;
 }
 
@@ -891,7 +858,7 @@ extern "C" int frt_decimate_process(frt_handle h, const float *x_dev, int64_t x_
                                     int64_t n_samples, float *out_dev, int64_t out_stride,
                                     void *stream) {
     if (!h) return FRT_EINVAL;
-    DecPlan *pl = reinterpret_cast<DecPlan *>(h->dec);
+    const DecPlan *pl = h->dec.get();
     if (!pl) return frt_fail(h, FRT_ESTATE, "frt_decimate_process: call frt_decimate_plan first");
     DeviceGuard g(h->device);
     FRT_CHECK_ARG(h, n_samples >= 0, "negative length");
@@ -908,7 +875,7 @@ extern "C" int frt_decimate_process(frt_handle h, const float *x_dev, int64_t x_
     a.n_channels = pl->n_channels;
     a.n_tiles = (int)(n_samples / 256);
     a.n_stages = pl->n_stages;
-    a.zstate = pl->zstate;
+    a.zstate = pl->zstate.get();
     const int warps = 2;
     const size_t smem = sizeof(float) * warps * pl->n_stages * 12;
     decimate_kernel<<<(pl->n_channels + warps - 1) / warps, warps * 32, smem,

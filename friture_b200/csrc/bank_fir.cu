@@ -255,32 +255,17 @@ __global__ void __launch_bounds__(FIR_THREADS, R == 1 ? 4 : 2) fir_bank_kernel(c
 
 struct FirPlan {
     int n_channels = 0, bpo = 0, n_oct = 0, L = 0;
-    double *taps = nullptr;
-    float *hist = nullptr;
-    double *sp = nullptr;          // [C][nbands]
-    double *alpha = nullptr;       // [n_oct]
-    double *decay = nullptr;       // [n_oct][FIR_DECAY_STRIDE]
-    float *weight_db = nullptr;    // [nbands]
-    bool smoothing = false;        // frt_firbank_set_smoothing has been called
+    DeviceArray<double> taps;
+    DeviceArray<float> hist;
+    DeviceArray<double> sp;          // [C][nbands]
+    DeviceArray<double> alpha;       // [n_oct]
+    DeviceArray<double> decay;       // [n_oct][FIR_DECAY_STRIDE]
+    DeviceArray<float> weight_db;    // [nbands]
+    bool smoothing = false;          // frt_firbank_set_smoothing has been called
     bool weighted = false;
 };
 
-static void fir_plan_free(FirPlan *pl) {
-    if (pl->taps) cudaFree(pl->taps);
-    if (pl->hist) cudaFree(pl->hist);
-    if (pl->sp) cudaFree(pl->sp);
-    if (pl->alpha) cudaFree(pl->alpha);
-    if (pl->decay) cudaFree(pl->decay);
-    if (pl->weight_db) cudaFree(pl->weight_db);
-    delete pl;
-}
-
-void frt_fir_release(frt_ctx *h) {
-    FirPlan *pl = reinterpret_cast<FirPlan *>(h->fir);
-    if (!pl) return;
-    fir_plan_free(pl);
-    h->fir = nullptr;
-}
+void PlanDelete::operator()(FirPlan *p) const { delete p; }
 
 extern "C" int frt_firbank_plan(frt_handle h, int n_channels, int bands_per_octave, int n_octaves,
                                 int n_taps, const double *fir_band, const double *fir_dec) {
@@ -291,8 +276,7 @@ extern "C" int frt_firbank_plan(frt_handle h, int n_channels, int bands_per_octa
     FRT_CHECK_ARG(h, n_octaves >= 1 && n_octaves <= FIR_MAX_OCT, "n_octaves must be in [1, 10]");
     FRT_CHECK_ARG(h, n_taps >= 2 && n_taps <= 1024, "n_taps must be in [2, 1024]");
     FRT_CHECK_ARG(h, fir_band && fir_dec, "NULL tap table");
-    frt_fir_release(h);
-    FirPlan *pl = new (std::nothrow) FirPlan();
+    PlanPtr<FirPlan> pl(new (std::nothrow) FirPlan());
     if (!pl) return frt_fail(h, FRT_ENOMEM, "out of host memory");
     pl->n_channels = n_channels;
     pl->bpo = bands_per_octave;
@@ -301,42 +285,37 @@ extern "C" int frt_firbank_plan(frt_handle h, int n_channels, int bands_per_octa
     const size_t nt = (size_t)(bands_per_octave + 1) * n_taps;
     const size_t nh = (size_t)n_channels * n_octaves * (n_taps - 1);
     const size_t nb = (size_t)bands_per_octave * n_octaves;
-    cudaError_t e = cudaMalloc(&pl->taps, sizeof(double) * nt);
-    if (e == cudaSuccess) e = cudaMalloc(&pl->hist, sizeof(float) * nh);
-    if (e == cudaSuccess) e = cudaMalloc(&pl->sp, sizeof(double) * n_channels * nb);
-    if (e == cudaSuccess) e = cudaMalloc(&pl->alpha, sizeof(double) * n_octaves);
-    if (e == cudaSuccess) e = cudaMalloc(&pl->decay, sizeof(double) * n_octaves * FIR_DECAY_STRIDE);
-    if (e == cudaSuccess) e = cudaMalloc(&pl->weight_db, sizeof(float) * nb);
-    if (e == cudaSuccess)
-        e = cudaMemcpy(pl->taps, fir_band, sizeof(double) * (size_t)bands_per_octave * n_taps, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess)
-        e = cudaMemcpy(pl->taps + (size_t)bands_per_octave * n_taps, fir_dec, sizeof(double) * n_taps,
-                       cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemset(pl->hist, 0, sizeof(float) * nh);
-    if (e == cudaSuccess) e = cudaMemset(pl->sp, 0, sizeof(double) * n_channels * nb);
-    if (e == cudaSuccess) e = cudaDeviceSynchronize();
-    if (e != cudaSuccess) {
-        fir_plan_free(pl);
-        return frt_fail(h, FRT_ECUDA, "frt_firbank_plan: %s", cudaGetErrorString(e));
-    }
-    h->fir = pl;
+    FRT_CUDA(h, pl->taps.alloc(nt));
+    FRT_CUDA(h, pl->hist.alloc(nh));
+    FRT_CUDA(h, pl->sp.alloc(n_channels * nb));
+    FRT_CUDA(h, pl->alpha.alloc(n_octaves));
+    FRT_CUDA(h, pl->decay.alloc((size_t)n_octaves * FIR_DECAY_STRIDE));
+    FRT_CUDA(h, pl->weight_db.alloc(nb));
+    FRT_CUDA(h, cudaMemcpy(pl->taps.get(), fir_band, sizeof(double) * (size_t)bands_per_octave * n_taps,
+                           cudaMemcpyHostToDevice));
+    FRT_CUDA(h, cudaMemcpy(pl->taps.get() + (size_t)bands_per_octave * n_taps, fir_dec, sizeof(double) * n_taps,
+                           cudaMemcpyHostToDevice));
+    FRT_CUDA(h, cudaMemset(pl->hist.get(), 0, sizeof(float) * nh));
+    FRT_CUDA(h, cudaMemset(pl->sp.get(), 0, sizeof(double) * n_channels * nb));
+    FRT_CUDA(h, cudaDeviceSynchronize());
+    h->fir = std::move(pl);
     return FRT_OK;
 }
 
 extern "C" int frt_firbank_reset(frt_handle h) {
     if (!h) return FRT_EINVAL;
-    FirPlan *pl = reinterpret_cast<FirPlan *>(h->fir);
+    FirPlan *pl = h->fir.get();
     if (!pl) return frt_fail(h, FRT_ESTATE, "frt_firbank_reset: no plan");
     DeviceGuard g(h->device);
-    FRT_CUDA(h, cudaMemset(pl->hist, 0, sizeof(float) * (size_t)pl->n_channels * pl->n_oct * (pl->L - 1)));
-    FRT_CUDA(h, cudaMemset(pl->sp, 0, sizeof(double) * (size_t)pl->n_channels * pl->n_oct * pl->bpo));
+    FRT_CUDA(h, cudaMemset(pl->hist.get(), 0, sizeof(float) * (size_t)pl->n_channels * pl->n_oct * (pl->L - 1)));
+    FRT_CUDA(h, cudaMemset(pl->sp.get(), 0, sizeof(double) * (size_t)pl->n_channels * pl->n_oct * pl->bpo));
     FRT_CUDA(h, cudaDeviceSynchronize());
     return FRT_OK;
 }
 
 extern "C" int frt_firbank_set_smoothing(frt_handle h, const double *alphas, const float *weight_db) {
     if (!h) return FRT_EINVAL;
-    FirPlan *pl = reinterpret_cast<FirPlan *>(h->fir);
+    FirPlan *pl = h->fir.get();
     if (!pl) return frt_fail(h, FRT_ESTATE, "frt_firbank_set_smoothing: call frt_firbank_plan first");
     DeviceGuard g(h->device);
     FRT_CHECK_ARG(h, alphas, "NULL alphas");
@@ -346,10 +325,10 @@ extern "C" int frt_firbank_set_smoothing(frt_handle h, const double *alphas, con
     for (int j = 0; j < pl->n_oct; j++)
         for (int m = 0; m < FIR_DECAY_STRIDE; m++)
             decay[(size_t)j * FIR_DECAY_STRIDE + m] = std::pow(1.0 - alphas[j], (double)m);
-    FRT_CUDA(h, cudaMemcpy(pl->alpha, alphas, sizeof(double) * pl->n_oct, cudaMemcpyHostToDevice));
-    FRT_CUDA(h, cudaMemcpy(pl->decay, decay.data(), sizeof(double) * decay.size(), cudaMemcpyHostToDevice));
+    FRT_CUDA(h, cudaMemcpy(pl->alpha.get(), alphas, sizeof(double) * pl->n_oct, cudaMemcpyHostToDevice));
+    FRT_CUDA(h, cudaMemcpy(pl->decay.get(), decay.data(), sizeof(double) * decay.size(), cudaMemcpyHostToDevice));
     if (weight_db)
-        FRT_CUDA(h, cudaMemcpy(pl->weight_db, weight_db, sizeof(float) * (size_t)pl->n_oct * pl->bpo,
+        FRT_CUDA(h, cudaMemcpy(pl->weight_db.get(), weight_db, sizeof(float) * (size_t)pl->n_oct * pl->bpo,
                                cudaMemcpyHostToDevice));
     pl->weighted = weight_db != nullptr;
     pl->smoothing = true;
@@ -360,8 +339,8 @@ static int fir_launch(frt_handle h, FirPlan *pl, FirArgs &a, void *stream) {
     a.L = pl->L;
     a.bpo = pl->bpo;
     a.n_oct = pl->n_oct;
-    a.taps = pl->taps;
-    a.hist = pl->hist;
+    a.taps = pl->taps.get();
+    a.hist = pl->hist.get();
     const size_t smem = FirSmem(pl->L, pl->bpo, pl->n_oct, a.block).total;
     // a bank of one or two filter groups (bpo <= 7) leaves most threads idle at four outputs per
     // thread: on an H100 (400 W) at 1024 channels, 512-sample blocks, 3 and 6 bands per octave ran 40 % and
@@ -377,7 +356,7 @@ static int fir_launch(frt_handle h, FirPlan *pl, FirArgs &a, void *stream) {
 extern "C" int frt_firbank_process(frt_handle h, const float *x_dev, int64_t x_stride, int n_samples,
                                    float *y_dev, int64_t y_stride, void *stream) {
     if (!h) return FRT_EINVAL;
-    FirPlan *pl = reinterpret_cast<FirPlan *>(h->fir);
+    FirPlan *pl = h->fir.get();
     if (!pl) return frt_fail(h, FRT_ESTATE, "frt_firbank_process: call frt_firbank_plan first");
     DeviceGuard g(h->device);
     FRT_CHECK_ARG(h, n_samples >= 0, "negative length");
@@ -403,7 +382,7 @@ extern "C" int frt_firbank_process(frt_handle h, const float *x_dev, int64_t x_s
 extern "C" int frt_firbank_levels(frt_handle h, const float *x_dev, int64_t x_stride, int block, int n_blocks,
                                   float *levels_dev, int db, void *stream) {
     if (!h) return FRT_EINVAL;
-    FirPlan *pl = reinterpret_cast<FirPlan *>(h->fir);
+    FirPlan *pl = h->fir.get();
     if (!pl) return frt_fail(h, FRT_ESTATE, "frt_firbank_levels: call frt_firbank_plan first");
     if (!pl->smoothing) return frt_fail(h, FRT_ESTATE, "frt_firbank_levels: call frt_firbank_set_smoothing first");
     DeviceGuard g(h->device);
@@ -424,10 +403,10 @@ extern "C" int frt_firbank_levels(frt_handle h, const float *x_dev, int64_t x_st
     a.x_stride = x_stride;
     a.block = block;
     a.n_blocks = n_blocks;
-    a.alpha = pl->alpha;
-    a.decay = pl->decay;
-    a.weight_db = pl->weighted ? pl->weight_db : nullptr;
-    a.sp = pl->sp;
+    a.alpha = pl->alpha.get();
+    a.decay = pl->decay.get();
+    a.weight_db = pl->weighted ? pl->weight_db.get() : nullptr;
+    a.sp = pl->sp.get();
     a.levels = levels_dev;
     a.db = db;
     return fir_launch(h, pl, a, stream);

@@ -74,9 +74,8 @@ struct BankPlan {
     PipeParams pipe[2];    // [logch - 5]: 32 / 64-sample steps
     bool pipe_ok = false;  // the lane-pipelined kernel supports this bank
     int n_channels = 0;
-    float *zstate = nullptr;
-    float *ema = nullptr;
-    float *weight = nullptr;   // device copy of the dB weighting vector, or NULL
+    DeviceArray<float> zstate, ema;
+    DeviceArray<float> weight;   // device copy of the dB weighting vector, or empty
     size_t nz = 0, ne = 0;     // floats per channel
     double alphas[BANK_MAX_OCT];
 };

@@ -6,48 +6,144 @@
 #include <cstdio>
 #include <cstring>
 #include <map>
+#include <memory>
 #include <string>
 #include <vector>
 
 #include "../../include/frt.h"
 
+// ---- owning types.  Device memory, streams and events are released only by these destructors;
+// they run inside the caller's DeviceGuard (frt_destroy holds one).
+struct CudaFree {
+    void operator()(void *p) const { cudaFree(p); }
+};
+struct StreamDestroy {
+    void operator()(cudaStream_t s) const { cudaStreamDestroy(s); }
+};
+struct EventDestroy {
+    void operator()(cudaEvent_t e) const { cudaEventDestroy(e); }
+};
+
+// One cudaMalloc allocation of n elements of T, or none.  Move-only.
+template <class T>
+struct DeviceArray {
+    std::unique_ptr<T[], CudaFree> p;
+    size_t n = 0;
+
+    T *get() const { return p.get(); }
+    cudaError_t alloc(size_t count) {   // frees what it held first
+        p.reset();
+        n = 0;
+        T *d = nullptr;
+        cudaError_t e = cudaMalloc(&d, sizeof(T) * count);
+        if (e != cudaSuccess) return e;
+        p.reset(d);
+        n = count;
+        return cudaSuccess;
+    }
+    cudaError_t upload(const std::vector<T> &host) {
+        cudaError_t e = alloc(host.size());
+        if (e != cudaSuccess) return e;
+        return cudaMemcpy(get(), host.data(), sizeof(T) * host.size(), cudaMemcpyHostToDevice);
+    }
+    // staging: reallocates only when a call needs more than it holds, so steady-state calls do not
+    cudaError_t grow(size_t count) { return count <= n ? cudaSuccess : alloc(count); }
+};
+
+struct Stream {   // non-blocking
+    std::unique_ptr<CUstream_st, StreamDestroy> s;
+    cudaStream_t get() const { return s.get(); }
+    cudaError_t create() {
+        cudaStream_t r = nullptr;
+        cudaError_t e = cudaStreamCreateWithFlags(&r, cudaStreamNonBlocking);
+        if (e == cudaSuccess) s.reset(r);
+        return e;
+    }
+};
+
+struct Event {    // timing disabled
+    std::unique_ptr<CUevent_st, EventDestroy> ev;
+    cudaEvent_t get() const { return ev.get(); }
+    cudaError_t create() {
+        cudaEvent_t r = nullptr;
+        cudaError_t e = cudaEventCreateWithFlags(&r, cudaEventDisableTiming);
+        if (e == cudaSuccess) ev.reset(r);
+        return e;
+    }
+};
+
+// Staging of a *_host entry point: streams for the H2D copies, the kernels and the D2H copies, NEV
+// events of each kind between them, created on the first call; the device buffers grow as needed.
+template <int NEV>
+struct HostStaging {
+    Stream s_in, s_cmp, s_out;
+    Event ev_in[NEV], ev_cmp[NEV], ev_out[NEV];
+
+    cudaError_t create() {
+        if (ev_out[NEV - 1].get()) return cudaSuccess;   // created last: the set is complete
+        cudaError_t e = s_in.create();
+        if (e == cudaSuccess) e = s_cmp.create();
+        if (e == cudaSuccess) e = s_out.create();
+        for (int i = 0; i < NEV && e == cudaSuccess; i++) {
+            e = ev_in[i].create();
+            if (e == cudaSuccess) e = ev_cmp[i].create();
+            if (e == cudaSuccess) e = ev_out[i].create();
+        }
+        return e;
+    }
+};
+
+// frt_stft_process_host: chunks alternate between two input and two output buffers
+struct StftStaging : HostStaging<2> {
+    DeviceArray<float> d_in[2], d_out[2];
+};
+
+// frt_combined_process_host: one event of each kind per time segment
+constexpr int COMB_MAX_SEG = 32;
+struct CombStaging : HostStaging<COMB_MAX_SEG> {
+    DeviceArray<float> d_x, d_spec, d_bands;
+};
+
 struct StftPlan {
     int n_fft = 0;
-    float *win_dev = nullptr;      // [n_fft] symmetric Hann (audioproc.py:76-81)
-    float2 *tw_dev = nullptr;      // N = 64..2048: [M/32][32] W_M^(k1*t); N >= 4096: [32][32] W_1024^(k1*t);
-                                   // N = 32: [M] W_M^k
-    float2 *post_dev = nullptr;    // U[k] = -j*W_N^k (real-FFT split twiddles), as many as the kernels read
-    float4 *wlane_dev = nullptr;   // N = 4096/8192: per-(warp, lane) Hann phase factors
-    float2 *comb_dev = nullptr;    // N >= 4096: [(R-1)][1024] W_M^(w k0)
+    DeviceArray<float> win_dev;     // [n_fft] symmetric Hann (audioproc.py:76-81)
+    DeviceArray<float2> tw_dev;     // N = 64..2048: [M/32][32] W_M^(k1*t); N >= 4096: [32][32] W_1024^(k1*t);
+                                    // N = 32: [M] W_M^k
+    DeviceArray<float2> post_dev;   // U[k] = -j*W_N^k (real-FFT split twiddles), as many as the kernels read
+    DeviceArray<float4> wlane_dev;  // N = 4096/8192: per-(warp, lane) Hann phase factors
+    DeviceArray<float2> comb_dev;   // N >= 4096: [(R-1)][1024] W_M^(w k0)
     std::vector<float> win_host;
 };
-void frt_stft_free_plan(StftPlan &pl);   // frees the plan's device tables
 
-struct HostPipe {                 // staging for the *_host entry points
-    cudaStream_t s_in = nullptr, s_cmp = nullptr, s_out = nullptr;
-    float *d_in[2] = {nullptr, nullptr};
-    float *d_out[2] = {nullptr, nullptr};
-    size_t in_bytes = 0, out_bytes = 0;
-    cudaEvent_t ev_in[2] = {nullptr, nullptr}, ev_cmp[2] = {nullptr, nullptr},
-                ev_out[2] = {nullptr, nullptr};
-};
-
-struct BankPlan;   // bank.cu
+// The other plans are private to their .cu files; each defines its deleter next to the struct.
+struct BankPlan;   // bank_internal.cuh
+struct DecPlan;    // bank.cu
+struct FirPlan;    // bank_fir.cu
 struct GccPlan;    // gcc_phat.cu
+struct PlanDelete {
+    void operator()(BankPlan *p) const;
+    void operator()(DecPlan *p) const;
+    void operator()(FirPlan *p) const;
+    void operator()(GccPlan *p) const;
+};
+template <class Plan>
+using PlanPtr = std::unique_ptr<Plan, PlanDelete>;
 
+// A plan call builds into a local PlanPtr and moves it into its slot only on success, so a call
+// that fails leaves the previous plan of that kind in place.
 struct frt_ctx {
     int device = 0;
     int sm_count = 0;
     int64_t launches = 0;
     std::string err;
-    StftPlan stft;                       // current plan (a copy of one cache entry)
-    std::map<int, StftPlan> stft_cache;  // every size planned so far owns its device tables
-    HostPipe pipe;
-    BankPlan *bank = nullptr;
-    GccPlan *gcc = nullptr;
-    void *dec = nullptr;          // DecPlan (bank.cu)
-    void *comb = nullptr;         // CombPipe (combined.cu)
-    void *fir = nullptr;          // FirPlan (bank_fir.cu)
+    std::map<int, StftPlan> stft_cache;  // every size planned so far
+    const StftPlan *stft = nullptr;      // current plan: an entry of stft_cache (std::map keeps it in place)
+    PlanPtr<BankPlan> bank;
+    PlanPtr<DecPlan> dec;
+    PlanPtr<FirPlan> fir;
+    PlanPtr<GccPlan> gcc;
+    StftStaging stft_host;
+    CombStaging comb_host;
 };
 
 int frt_fail(frt_ctx *h, int code, const char *fmt, ...);
@@ -87,11 +183,3 @@ __device__ __forceinline__ float2 f2_mul(float2 a, float2 b) { return make_float
 __device__ __forceinline__ float2 f2_fma(float2 a, float2 b, float2 c) {
     return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
 }
-
-// bank.cu / gcc_phat.cu clean-up hooks
-void frt_bank_release(frt_ctx *h);
-void frt_gcc_release(frt_ctx *h);
-void frt_dec_release(frt_ctx *h);
-void frt_comb_release(frt_ctx *h);
-void frt_fir_release(frt_ctx *h);
-int frt_pipe_ensure(frt_ctx *h, size_t in_bytes, size_t out_bytes);

@@ -383,20 +383,13 @@ __global__ void __launch_bounds__(GCC_THREADS, 1) gcc_phat_kernel(const GccArgs 
 
 struct GccPlan {
     int L = 0;
-    float *window = nullptr;
-    float2 *tw = nullptr;
-    int *perm = nullptr;
+    DeviceArray<float> window;
+    DeviceArray<float2> tw;
+    DeviceArray<int> perm;
     GccRadices rd;
 };
 
-void frt_gcc_release(frt_ctx *h) {
-    if (!h->gcc) return;
-    if (h->gcc->window) cudaFree(h->gcc->window);
-    if (h->gcc->tw) cudaFree(h->gcc->tw);
-    if (h->gcc->perm) cudaFree(h->gcc->perm);
-    delete h->gcc;
-    h->gcc = nullptr;
-}
+void PlanDelete::operator()(GccPlan *p) const { delete p; }
 
 extern "C" int frt_gcc_plan(frt_handle h, int length) {
     if (!h) return FRT_EINVAL;
@@ -429,8 +422,7 @@ extern "C" int frt_gcc_plan(frt_handle h, int length) {
             nn = n_next;
         }
     }
-    frt_gcc_release(h);
-    GccPlan *pl = new (std::nothrow) GccPlan();
+    PlanPtr<GccPlan> pl(new (std::nothrow) GccPlan());
     if (!pl) return frt_fail(h, FRT_ENOMEM, "out of host memory");
     pl->L = length;
     pl->rd = rd;
@@ -445,26 +437,12 @@ extern "C" int frt_gcc_plan(frt_handle h, int length) {
     }
     std::vector<int> perm(length);
     for (int i = 0; i < length; i++) perm[i] = digit_reverse(i, length, rd);
-    cudaError_t e = cudaMalloc(&pl->window, sizeof(float) * length);
-    if (e == cudaSuccess) e = cudaMalloc(&pl->perm, sizeof(int) * length);
-    if (e == cudaSuccess)
-        e = cudaMemcpy(pl->perm, perm.data(), sizeof(int) * length, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMalloc(&pl->tw, sizeof(float2) * length);
-    if (e == cudaSuccess)
-        e = cudaMemcpy(pl->window, win.data(), sizeof(float) * length, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess)
-        e = cudaMemcpy(pl->tw, tw.data(), sizeof(float2) * length, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(gcc_phat_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 (int)(sizeof(float2) * length));
-    if (e != cudaSuccess) {
-        if (pl->window) cudaFree(pl->window);
-        if (pl->tw) cudaFree(pl->tw);
-        if (pl->perm) cudaFree(pl->perm);
-        delete pl;
-        return frt_fail(h, FRT_ECUDA, "frt_gcc_plan: %s", cudaGetErrorString(e));
-    }
-    h->gcc = pl;
+    FRT_CUDA(h, pl->window.upload(win));
+    FRT_CUDA(h, pl->perm.upload(perm));
+    FRT_CUDA(h, pl->tw.upload(tw));
+    FRT_CUDA(h, cudaFuncSetAttribute(gcc_phat_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)(sizeof(float2) * length)));
+    h->gcc = std::move(pl);
     return FRT_OK;
 }
 
@@ -474,7 +452,7 @@ extern "C" int frt_gcc_phat(frt_handle h, const float *d0_dev, const float *d1_d
     if (!h) return FRT_EINVAL;
     if (!h->gcc) return frt_fail(h, FRT_ESTATE, "frt_gcc_phat: call frt_gcc_plan first");
     DeviceGuard g(h->device);
-    GccPlan *pl = h->gcc;
+    const GccPlan *pl = h->gcc.get();
     FRT_CHECK_ARG(h, n_pairs >= 0, "negative n_pairs");
     if (n_pairs == 0) return FRT_OK;
     FRT_CHECK_ARG(h, d0_dev && d1_dev && idx_dev && val_dev, "NULL buffer");
@@ -487,9 +465,9 @@ extern "C" int frt_gcc_phat(frt_handle h, const float *d0_dev, const float *d1_d
     a.stride = stride;
     a.n_pairs = n_pairs;
     a.L = pl->L;
-    a.window = pl->window;
-    a.tw = pl->tw;
-    a.perm = pl->perm;
+    a.window = pl->window.get();
+    a.tw = pl->tw.get();
+    a.perm = pl->perm.get();
     a.xcorr = xcorr_dev;
     a.smoothed = smoothed_dev;
     a.have_prev = have_prev;

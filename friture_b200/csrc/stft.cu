@@ -772,11 +772,11 @@ void launch_small(const frt_ctx *h, const StftPlan &pl, const Frames &a) {
     const long long max_blocks = (long long)small_ctas_per_sm<Q>() * h->sm_count;
     long long blocks = ((a.total + G - 1) / G + WARPS - 1) / WARPS;
     if (blocks > max_blocks) blocks = max_blocks;
-    const float2 *w2 = reinterpret_cast<const float2 *>(pl.win_dev);
+    const float2 *w2 = reinterpret_cast<const float2 *>(pl.win_dev.get());
     with_mode(a.mode, [&](auto m) {
         stft_small_kernel<Q, decltype(m)::value, TMA><<<(unsigned)blocks, WARPS * 32, small_smem<Q>(), a.st>>>(
-            a.x, a.x_stride, a.n_frames, a.hop, a.out, a.osc, a.osf, w2, pl.tw_dev, pl.post_dev, a.total,
-            a.vec_ok);
+            a.x, a.x_stride, a.n_frames, a.hop, a.out, a.osc, a.osf, w2, pl.tw_dev.get(), pl.post_dev.get(),
+            a.total, a.vec_ok);
     });
 }
 template <int R>
@@ -793,19 +793,19 @@ void launch_large(const frt_ctx *h, const StftPlan &pl, const Frames &a) {
     with_mode(a.mode, [&](auto m) {
         stft_large_kernel<R, decltype(m)::value><<<(unsigned)blocks, LARGE_WARPS * 32, large_smem<R>(), a.st>>>(
             a.x, a.x_stride, a.n_frames, a.hop, a.out, a.osc, a.osf,
-            reinterpret_cast<const float2 *>(pl.win_dev), pl.wlane_dev, pl.tw_dev, pl.comb_dev, pl.post_dev,
-            a.total, ha);
+            reinterpret_cast<const float2 *>(pl.win_dev.get()), pl.wlane_dev.get(), pl.tw_dev.get(),
+            pl.comb_dev.get(), pl.post_dev.get(), a.total, ha);
     });
 }
 template <int R>
 void launch_multi(const frt_ctx *h, const StftPlan &pl, const Frames &a) {
     long long blocks = (long long)h->sm_count * (R == 8 ? 2 : (R == 4 ? 4 : 8));
     if (blocks > a.total) blocks = a.total;
-    const float2 *w2 = reinterpret_cast<const float2 *>(pl.win_dev);
+    const float2 *w2 = reinterpret_cast<const float2 *>(pl.win_dev.get());
     with_mode(a.mode, [&](auto m) {
         stft_multi_kernel<R, decltype(m)::value><<<(unsigned)blocks, 32 * R, multi_smem(R), a.st>>>(
-            a.x, a.x_stride, a.n_frames, a.hop, a.out, a.osc, a.osf, w2, pl.tw_dev, pl.comb_dev, pl.post_dev,
-            a.total, a.vec_ok);
+            a.x, a.x_stride, a.n_frames, a.hop, a.out, a.osc, a.osf, w2, pl.tw_dev.get(), pl.comb_dev.get(),
+            pl.post_dev.get(), a.total, a.vec_ok);
     });
 }
 
@@ -827,50 +827,28 @@ std::vector<float2> row_twiddles(int rows, int m) {
     return tw;
 }
 
-template <class T>
-cudaError_t upload(T **dev, const std::vector<T> &host) {
-    cudaError_t e = cudaMalloc(dev, sizeof(T) * host.size());
-    if (e == cudaSuccess) e = cudaMemcpy(*dev, host.data(), sizeof(T) * host.size(), cudaMemcpyHostToDevice);
-    return e;
-}
-
 }   // namespace
-
-void frt_stft_free_plan(StftPlan &pl) {
-    cudaFree(pl.win_dev);
-    cudaFree(pl.tw_dev);
-    cudaFree(pl.post_dev);
-    cudaFree(pl.wlane_dev);
-    cudaFree(pl.comb_dev);
-}
 
 extern "C" int frt_stft_plan(frt_handle h, int n_fft) {
     if (!h) return FRT_EINVAL;
     DeviceGuard g(h->device);
     FRT_CHECK_ARG(h, n_fft >= 32 && n_fft <= 16384 && (n_fft & (n_fft - 1)) == 0,
                   "n_fft must be a power of two in [32, 16384]");
-    if (h->stft.n_fft == n_fft) return FRT_OK;
+    if (h->stft && h->stft->n_fft == n_fft) return FRT_OK;
     // plans are cached per size: the spectrum (8192) and spectrogram (4096) widgets share a handle
     auto cached = h->stft_cache.find(n_fft);
     if (cached != h->stft_cache.end()) {
-        h->stft = cached->second;
+        h->stft = &cached->second;
         return FRT_OK;
     }
     StftPlan pl;
-    // a failed cudaMalloc / cudaMemcpy below returns early: free what the half-built plan owns
-    struct PlanGuard {
-        StftPlan *p;
-        ~PlanGuard() {
-            if (p) frt_stft_free_plan(*p);
-        }
-    } guard{&pl};
     const int N = n_fft, M = N / 2;
     const double PI = 3.14159265358979323846;
     // symmetric Hann, friture/audioproc.py:76-81
     pl.win_host.resize(N);
     for (int n = 0; n < N; n++)
         pl.win_host[n] = (float)(0.5 * (1.0 - cos(2.0 * PI * n / (double)(N - 1))));
-    FRT_CUDA(h, upload(&pl.win_dev, pl.win_host));
+    FRT_CUDA(h, pl.win_dev.upload(pl.win_host));
     const int multi_r = (N == 4096) ? 2 : ((N == 8192) ? 4 : ((N == 16384) ? 8 : 0));
     std::vector<float2> tw;
     if (multi_r) {   // each warp's 1024-point FFT, then the radix-R combine by W_M^(w k0)
@@ -881,7 +859,7 @@ extern "C" int frt_stft_plan(frt_handle h, int n_fft) {
                 const double a = -2.0 * PI * (double)(w * k0) / (double)M;
                 comb[(size_t)(w - 1) * 1024 + k0] = make_float2((float)cos(a), (float)sin(a));
             }
-        FRT_CUDA(h, upload(&pl.comb_dev, comb));
+        FRT_CUDA(h, pl.comb_dev.upload(comb));
     } else if (N >= 64) {   // stft_small_kernel: [Q][32] W_M^(k1 t), M = 32 Q
         tw = row_twiddles(M / 32, M);
     } else {                // stft_generic_kernel: [M] W_M^k
@@ -891,7 +869,7 @@ extern "C" int frt_stft_plan(frt_handle h, int n_fft) {
             tw[i] = make_float2((float)cos(a), (float)sin(a));
         }
     }
-    FRT_CUDA(h, upload(&pl.tw_dev, tw));
+    FRT_CUDA(h, pl.tw_dev.upload(tw));
     // U[k] = -j * W_N^k for every k a kernel reads: k < M/2 in stft_small_kernel, k <= M/2 in
     // stft_generic_kernel and stft_large_kernel (which derives the rest), k < M - 512 in
     // stft_multi_kernel (its largest bin with a partner is k0 + 1024 (R-1), k0 < 512)
@@ -900,7 +878,7 @@ extern "C" int frt_stft_plan(frt_handle h, int n_fft) {
         const double a = 2.0 * PI * (double)k / (double)N;
         post[k] = make_float2((float)(-sin(a)), (float)(-cos(a)));
     }
-    FRT_CUDA(h, upload(&pl.post_dev, post));
+    FRT_CUDA(h, pl.post_dev.upload(post));
     if (N == 4096 || N == 8192) {   // stft_large_kernel: per-(warp, lane) part of the Hann phase
         const int R = N / 2048;
         std::vector<float4> wl((size_t)R * 32);
@@ -910,22 +888,20 @@ extern "C" int frt_stft_plan(frt_handle h, int n_fft) {
                 const double b0 = theta * (2 * R * t + 2 * w), b1 = theta * (2 * R * t + 2 * w + 1);
                 wl[(size_t)w * 32 + t] = make_float4((float)cos(b0), (float)cos(b1), (float)sin(b0), (float)sin(b1));
             }
-        FRT_CUDA(h, upload(&pl.wlane_dev, wl));
+        FRT_CUDA(h, pl.wlane_dev.upload(wl));
     }
     FRT_CUDA(h, set_smem_limits<FRT_STFT_POWER>());
     FRT_CUDA(h, set_smem_limits<FRT_STFT_LOGPOWER>());
     pl.n_fft = n_fft;
-    guard.p = nullptr;          // the cache owns the device tables from here on
-    h->stft_cache[n_fft] = pl;
-    h->stft = pl;
+    h->stft = &h->stft_cache.emplace(n_fft, std::move(pl)).first->second;
     return FRT_OK;
 }
 
 extern "C" int frt_stft_window(frt_handle h, float *window_host) {
     if (!h) return FRT_EINVAL;
-    if (!h->stft.n_fft) return frt_fail(h, FRT_ESTATE, "frt_stft_window: no plan");
+    if (!h->stft) return frt_fail(h, FRT_ESTATE, "frt_stft_window: no plan");
     FRT_CHECK_ARG(h, window_host != nullptr, "window_host is NULL");
-    memcpy(window_host, h->stft.win_host.data(), sizeof(float) * h->stft.n_fft);
+    memcpy(window_host, h->stft->win_host.data(), sizeof(float) * h->stft->n_fft);
     return FRT_OK;
 }
 
@@ -935,8 +911,8 @@ extern "C" int frt_stft_process(frt_handle h, const float *x_dev, int64_t x_stri
                                 void *stream) {
     if (!h) return FRT_EINVAL;
     DeviceGuard g(h->device);
-    const StftPlan &pl = h->stft;
-    if (!pl.n_fft) return frt_fail(h, FRT_ESTATE, "frt_stft_process: call frt_stft_plan first");
+    if (!h->stft) return frt_fail(h, FRT_ESTATE, "frt_stft_process: call frt_stft_plan first");
+    const StftPlan &pl = *h->stft;
     FRT_CHECK_ARG(h, n_channels >= 0 && n_frames >= 0, "negative shape");
     FRT_CHECK_ARG(h, hop >= 1, "hop must be >= 1");
     FRT_CHECK_ARG(h, mode == FRT_STFT_POWER || mode == FRT_STFT_LOGPOWER, "unknown mode");
@@ -973,8 +949,8 @@ extern "C" int frt_stft_process(frt_handle h, const float *x_dev, int64_t x_stri
         if (threads < 32) threads = 32;
         if (threads > 512) threads = 512;
         stft_generic_kernel<<<(unsigned)total, threads, sizeof(float2) * 2 * M, a.st>>>(
-            x_dev, x_stride, n_frames, hop, out_dev, out_stride_c, out_stride_f, pl.win_dev,
-            pl.tw_dev, pl.post_dev, mode, N, ilog2(M));
+            x_dev, x_stride, n_frames, hop, out_dev, out_stride_c, out_stride_f, pl.win_dev.get(),
+            pl.tw_dev.get(), pl.post_dev.get(), mode, N, ilog2(M));
     }
     h->launches++;
     FRT_CUDA(h, cudaGetLastError());
@@ -986,8 +962,8 @@ extern "C" int frt_stft_process_host(frt_handle h, const float *x_host, int64_t 
                                      float *out_host, int mode) {
     if (!h) return FRT_EINVAL;
     DeviceGuard g(h->device);
-    const StftPlan &pl = h->stft;
-    if (!pl.n_fft) return frt_fail(h, FRT_ESTATE, "frt_stft_process_host: no plan");
+    if (!h->stft) return frt_fail(h, FRT_ESTATE, "frt_stft_process_host: no plan");
+    const StftPlan &pl = *h->stft;
     FRT_CHECK_ARG(h, n_channels >= 0 && n_samples >= 0 && hop >= 1, "bad shape");
     const int N = pl.n_fft, nbins = N / 2 + 1;
     if (n_channels == 0 || n_samples < N) return FRT_OK;
@@ -1007,11 +983,12 @@ extern "C" int frt_stft_process_host(frt_handle h, const float *x_host, int64_t 
         if (cgroup > n_channels) cgroup = n_channels;
     }
     const int64_t chunk_samples = (fchunk - 1) * (int64_t)hop + N;
-    const size_t in_bytes = sizeof(float) * (size_t)cgroup * chunk_samples;
-    const size_t out_bytes = (size_t)cgroup * fchunk * out_per_frame;
-    int rc = frt_pipe_ensure(h, in_bytes, out_bytes);
-    if (rc) return rc;
-    HostPipe &p = h->pipe;
+    StftStaging &p = h->stft_host;
+    FRT_CUDA(h, p.create());
+    for (auto &d : p.d_in) FRT_CUDA(h, d.grow((size_t)cgroup * chunk_samples));
+    for (auto &d : p.d_out) FRT_CUDA(h, d.grow((size_t)cgroup * fchunk * nbins));
+    const cudaStream_t s_in = p.s_in.get(), s_cmp = p.s_cmp.get(), s_out = p.s_out.get();
+    int rc;
     int it = 0;
     for (int c0 = 0; c0 < n_channels; c0 += cgroup) {
         const int nc = (c0 + cgroup <= n_channels) ? cgroup : (n_channels - c0);
@@ -1020,29 +997,29 @@ extern "C" int frt_stft_process_host(frt_handle h, const float *x_host, int64_t 
             const int64_t ns = (nf - 1) * (int64_t)hop + N;
             const int b = it & 1;
             // the H2D may only overwrite d_in[b] after the kernel that read it has finished
-            FRT_CUDA(h, cudaStreamWaitEvent(p.s_in, p.ev_cmp[b], 0));
-            FRT_CUDA(h, cudaMemcpy2DAsync(p.d_in[b], sizeof(float) * ns,
+            FRT_CUDA(h, cudaStreamWaitEvent(s_in, p.ev_cmp[b].get(), 0));
+            FRT_CUDA(h, cudaMemcpy2DAsync(p.d_in[b].get(), sizeof(float) * ns,
                                           x_host + (size_t)c0 * x_stride + f0 * hop,
                                           sizeof(float) * x_stride, sizeof(float) * ns, nc,
-                                          cudaMemcpyHostToDevice, p.s_in));
-            FRT_CUDA(h, cudaEventRecord(p.ev_in[b], p.s_in));
-            FRT_CUDA(h, cudaStreamWaitEvent(p.s_cmp, p.ev_in[b], 0));
-            FRT_CUDA(h, cudaStreamWaitEvent(p.s_cmp, p.ev_out[b], 0));   // d_out[b] drained
-            rc = frt_stft_process(h, p.d_in[b], ns, nc, nf, hop, p.d_out[b],
-                                  nf * (int64_t)nbins, nbins, mode, p.s_cmp);
+                                          cudaMemcpyHostToDevice, s_in));
+            FRT_CUDA(h, cudaEventRecord(p.ev_in[b].get(), s_in));
+            FRT_CUDA(h, cudaStreamWaitEvent(s_cmp, p.ev_in[b].get(), 0));
+            FRT_CUDA(h, cudaStreamWaitEvent(s_cmp, p.ev_out[b].get(), 0));   // d_out[b] drained
+            rc = frt_stft_process(h, p.d_in[b].get(), ns, nc, nf, hop, p.d_out[b].get(),
+                                  nf * (int64_t)nbins, nbins, mode, s_cmp);
             if (rc) return rc;
-            FRT_CUDA(h, cudaEventRecord(p.ev_cmp[b], p.s_cmp));
-            FRT_CUDA(h, cudaStreamWaitEvent(p.s_out, p.ev_cmp[b], 0));
+            FRT_CUDA(h, cudaEventRecord(p.ev_cmp[b].get(), s_cmp));
+            FRT_CUDA(h, cudaStreamWaitEvent(s_out, p.ev_cmp[b].get(), 0));
             FRT_CUDA(h, cudaMemcpy2DAsync(out_host + ((size_t)c0 * frames + f0) * nbins,
-                                          sizeof(float) * frames * nbins, p.d_out[b],
+                                          sizeof(float) * frames * nbins, p.d_out[b].get(),
                                           sizeof(float) * nf * nbins,
                                           sizeof(float) * nf * nbins, nc,
-                                          cudaMemcpyDeviceToHost, p.s_out));
-            FRT_CUDA(h, cudaEventRecord(p.ev_out[b], p.s_out));
+                                          cudaMemcpyDeviceToHost, s_out));
+            FRT_CUDA(h, cudaEventRecord(p.ev_out[b].get(), s_out));
         }
     }
-    FRT_CUDA(h, cudaStreamSynchronize(p.s_out));
-    FRT_CUDA(h, cudaStreamSynchronize(p.s_cmp));
-    FRT_CUDA(h, cudaStreamSynchronize(p.s_in));
+    FRT_CUDA(h, cudaStreamSynchronize(s_out));
+    FRT_CUDA(h, cudaStreamSynchronize(s_cmp));
+    FRT_CUDA(h, cudaStreamSynchronize(s_in));
     return FRT_OK;
 }

@@ -15,6 +15,7 @@
  *     the caller's host buffer;
  *   - the library never owns caller buffers; plans, coefficient tables and filter / smoothing
  *     state live in the handle;
+ *   - a plan call that fails leaves the handle's previous plan of that kind in place;
  *   - every function returns FRT_OK (0) or a negative FRT_E* code; frt_last_error(h) gives the
  *     message.  There is no CPU fallback anywhere: without a CUDA device frt_create fails.
  */
