@@ -193,8 +193,5 @@ extern "C" int frt_peer_push(frt_handle h, const void *src, void *const *peer_ds
     a.n_peers = n_peers;
     a.n_vec = (long long)(bytes / 16);
     if (n_ctas < 1) n_ctas = 64;
-    peer_push_kernel<<<n_ctas, 256, 0, (cudaStream_t)stream>>>(a);
-    h->launches++;
-    FRT_CUDA(h, cudaGetLastError());
-    return FRT_OK;
+    return frt_launch(h, peer_push_kernel, n_ctas, 256, 0, (cudaStream_t)stream, a);
 }

@@ -29,16 +29,10 @@ constexpr int MAX_BPO = BANK_MAX_BPO;
 constexpr int MAX_OCT = BANK_MAX_OCT;
 constexpr int NQ = BANK_NQ;
 
-__device__ __forceinline__ float lg2_fast(float v) {
-    float r;
-    asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(v));
-    return r;
-}
-
 __device__ __forceinline__ float energy_out(float e, int db, const float *weight, int kband) {
     // friture/octavespectrum.py:119-121: 10*log10(sp + 1e-30) + w
     if (!db) return e;
-    float v = 3.01029995663981195f * lg2_fast(e + 1e-30f);
+    float v = kLog10Scale * lg2_fast(e + 1e-30f);
     if (weight) v += __ldg(weight + kband);
     return v;
 }
@@ -686,39 +680,31 @@ extern "C" int frt_bank_set_state(frt_handle h, const float *z_host, const float
 }
 
 template <int L0, bool WANT_Y>
-static cudaError_t launch_bank3(const BankPlan *pl, const BankArgs &a, cudaStream_t st) {
+static int launch_bank3(frt_handle h, const BankPlan *pl, const BankArgs &a, cudaStream_t st) {
     const BankParams &P = pl->params;
     const size_t smem = sizeof(float) * ((size_t)P.nsec * 8 + pl->nz + pl->ne + 32 * L0 + 64);
-    cudaError_t e = cudaFuncSetAttribute(bank_kernel3<L0, WANT_Y>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    bank_kernel3<L0, WANT_Y><<<(unsigned)a.n_channels, 96, smem, st>>>(P, a);
-    return cudaGetLastError();
+    return frt_launch(h, bank_kernel3<L0, WANT_Y>, (unsigned)a.n_channels, 96, smem, st, P, a);
 }
 
 template <int L0, bool WANT_Y>
-static cudaError_t launch_bank_y(const BankPlan *pl, const BankArgs &a, cudaStream_t st) {
+static int launch_bank_y(frt_handle h, const BankPlan *pl, const BankArgs &a, cudaStream_t st) {
     // few channels: three warps per channel (latency-bound regime); many channels: one warp
     // per channel already saturates the schedulers with less synchronisation
     // the three-warp kernel runs all log2(L0) scan-mode stages unconditionally: it needs more
     // octaves than that (always true for the 9- and 10-octave banks of the reference)
     if constexpr (L0 <= 16) {
-        if (pl->params.n_oct > Log2<L0>::v && a.n_channels < 1536) return launch_bank3<L0, WANT_Y>(pl, a, st);
+        if (pl->params.n_oct > Log2<L0>::v && a.n_channels < 1536) return launch_bank3<L0, WANT_Y>(h, pl, a, st);
     }
     const BankParams &P = pl->params;
     const int warps = 2;
     const size_t smem = sizeof(float) * ((size_t)P.nsec * 8 + (size_t)warps * (pl->nz + pl->ne));
-    cudaError_t e = cudaFuncSetAttribute(bank_kernel<L0, WANT_Y>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
     const unsigned blocks = (unsigned)((a.n_channels + warps - 1) / warps);
-    bank_kernel<L0, WANT_Y><<<blocks, warps * 32, smem, st>>>(P, a);
-    return cudaGetLastError();
+    return frt_launch(h, bank_kernel<L0, WANT_Y>, blocks, warps * 32, smem, st, P, a);
 }
 
 template <int L0>
-static cudaError_t launch_bank(const BankPlan *pl, const BankArgs &a, cudaStream_t st) {
-    return a.y ? launch_bank_y<L0, true>(pl, a, st) : launch_bank_y<L0, false>(pl, a, st);
+static int launch_bank(frt_handle h, const BankPlan *pl, const BankArgs &a, cudaStream_t st) {
+    return a.y ? launch_bank_y<L0, true>(h, pl, a, st) : launch_bank_y<L0, false>(h, pl, a, st);
 }
 
 static int bank_process_impl(frt_handle h, const float *x_dev, int64_t x_stride, int block,
@@ -789,7 +775,6 @@ static int bank_process_impl(frt_handle h, const float *x_dev, int64_t x_stride,
     a.block = block;
     a.n_blocks = n_blocks;
     a.n_steps = 0;
-    cudaError_t e;
     cudaStream_t st = (cudaStream_t)stream;
     // Kernel choice.  The lane-pipelined kernel (bank_pipe.cu) computes every section sample once
     // and is the fast path for the fused energies of 1- and 1/3-octave banks; the chunk-scan
@@ -803,14 +788,11 @@ static int bank_process_impl(frt_handle h, const float *x_dev, int64_t x_stride,
         // stream gives the same bits however it is cut into launches.
         const int pack = pl->n_channels > 3072 ? 2 : 1;
         const int logch = (block >= 512 && pack == 1) ? 6 : 5;
-        e = frt_pipe_launch(pl, a, logch, pack, st);
-    } else if (tile == 1024) e = launch_bank<32>(pl, a, st);
-    else if (tile == 512) e = launch_bank<16>(pl, a, st);
-    else e = launch_bank<8>(pl, a, st);
-    h->launches++;
-    if (e != cudaSuccess)
-        return frt_fail(h, FRT_ECUDA, "bank kernel launch: %s", cudaGetErrorString(e));
-    return FRT_OK;
+        return frt_pipe_launch(h, pl, a, logch, pack, st);
+    }
+    if (tile == 1024) return launch_bank<32>(h, pl, a, st);
+    if (tile == 512) return launch_bank<16>(h, pl, a, st);
+    return launch_bank<8>(h, pl, a, st);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -878,9 +860,6 @@ extern "C" int frt_decimate_process(frt_handle h, const float *x_dev, int64_t x_
     a.zstate = pl->zstate.get();
     const int warps = 2;
     const size_t smem = sizeof(float) * warps * pl->n_stages * 12;
-    decimate_kernel<<<(pl->n_channels + warps - 1) / warps, warps * 32, smem,
-                      (cudaStream_t)stream>>>(pl->params, a);
-    h->launches++;
-    FRT_CUDA(h, cudaGetLastError());
-    return FRT_OK;
+    return frt_launch(h, decimate_kernel, (pl->n_channels + warps - 1) / warps, warps * 32, smem,
+                      (cudaStream_t)stream, pl->params, a);
 }

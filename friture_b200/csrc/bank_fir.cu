@@ -346,11 +346,7 @@ static int fir_launch(frt_handle h, FirPlan *pl, FirArgs &a, void *stream) {
     // thread: on an H100 (400 W) at 1024 channels, 512-sample blocks, 3 and 6 bands per octave ran 40 % and
     // 20 % slower than one output per thread; 12 and 24 bands per octave ran 1.6x and 1.7x faster
     auto kernel = pl->bpo + 1 <= 2 * FIR_F ? fir_bank_kernel<1> : fir_bank_kernel<FIR_R>;
-    FRT_CUDA(h, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    kernel<<<pl->n_channels, FIR_THREADS, smem, (cudaStream_t)stream>>>(a);
-    h->launches++;
-    FRT_CUDA(h, cudaGetLastError());
-    return FRT_OK;
+    return frt_launch(h, kernel, pl->n_channels, FIR_THREADS, smem, (cudaStream_t)stream, a);
 }
 
 extern "C" int frt_firbank_process(frt_handle h, const float *x_dev, int64_t x_stride, int n_samples,

@@ -85,4 +85,4 @@ void frt_pipe_prepare(BankPlan *pl);
 void frt_pipe_schedule(int n_oct, int logch, long long t_total, int *T /*[BANK_MAX_OCT+1]*/, int *n_steps);
 int frt_pipe_flush_delta(int n_oct, int logch, const int *T);
 bool frt_pipe_supported(const BankPlan *pl, int block, int logch);
-cudaError_t frt_pipe_launch(const BankPlan *pl, BankArgs a, int logch, int pack, cudaStream_t st);
+int frt_pipe_launch(frt_ctx *h, const BankPlan *pl, BankArgs a, int logch, int pack, cudaStream_t st);

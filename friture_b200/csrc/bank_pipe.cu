@@ -107,25 +107,6 @@ __device__ __forceinline__ void st2(float2 *p, float2 a, float2 b) {
     *reinterpret_cast<float4 *>(p) = make_float4(a.x, a.y, b.x, b.y);
 }
 
-__device__ __forceinline__ void cp_async4(void *smem, const void *gmem) {
-    const unsigned s = (unsigned)__cvta_generic_to_shared(smem);
-    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(s), "l"(gmem) : "memory");
-}
-__device__ __forceinline__ void cp_async16(void *smem, const void *gmem) {
-    const unsigned s = (unsigned)__cvta_generic_to_shared(smem);
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(s), "l"(gmem) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N> __device__ __forceinline__ void cp_async_wait() {
-    asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
-}
-
-__device__ __forceinline__ float lg2_fast(float v) {
-    float r;
-    asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(v));
-    return r;
-}
-
 // blocks of band energies staged in shared memory before the flush: a block's vector leaves fdelta
 // steps after its last stage-0 chunk, meanwhile stage 0 keeps staging newer blocks
 // (frt_pipe_supported checks that the ring is deep enough for the block length)
@@ -618,8 +599,8 @@ bank_pipe_kernel(const __grid_constant__ PipeParams P, const BankArgs a) {
                             float e0 = v_x(v), e1 = v_y(v);
                             if (a.db) {     // friture/octavespectrum.py:119-121: 10*log10(sp + 1e-30) + w
                                 const float w = wreg[t];
-                                e0 = fmaf(3.01029995663981195f, lg2_fast(e0 + 1e-30f), w);
-                                e1 = fmaf(3.01029995663981195f, lg2_fast(e1 + 1e-30f), w);
+                                e0 = fmaf(kLog10Scale, lg2_fast(e0 + 1e-30f), w);
+                                e1 = fmaf(kLog10Scale, lg2_fast(e1 + 1e-30f), w);
                             }
                             float *o = eout0 + (size_t)blk * nbands + i;
                             o[0] = e0;
@@ -703,22 +684,18 @@ bank_pipe_kernel(const __grid_constant__ PipeParams P, const BankArgs a) {
 }
 
 template <int LOGCH, int PACK, int BPO>
-cudaError_t launch_pipe(const PipeParams &P, const BankArgs &a, cudaStream_t st) {
+int launch_pipe(frt_ctx *h, const PipeParams &P, const BankArgs &a, cudaStream_t st) {
     using LY = PipeLayout<LOGCH, PACK, BPO>;
     const size_t smem = (size_t)LY::TB * NSLOT * LY::TOTAL + 2 * 12 * 4;
-    auto kern = bank_pipe_kernel<LOGCH, PACK, BPO>;
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
     const int per_warp = NSLOT * PACK;
     const unsigned blocks = (unsigned)((a.n_channels + per_warp - 1) / per_warp);
-    kern<<<blocks, 32, smem, st>>>(P, a);
-    return cudaGetLastError();
+    return frt_launch(h, bank_pipe_kernel<LOGCH, PACK, BPO>, blocks, 32, smem, st, P, a);
 }
 
 template <int LOGCH, int PACK>
-cudaError_t launch_pipe_bpo(const PipeParams &P, const BankArgs &a, cudaStream_t st) {
-    if (P.bpo == 3) return launch_pipe<LOGCH, PACK, 3>(P, a, st);
-    return launch_pipe<LOGCH, PACK, 1>(P, a, st);
+int launch_pipe_bpo(frt_ctx *h, const PipeParams &P, const BankArgs &a, cudaStream_t st) {
+    if (P.bpo == 3) return launch_pipe<LOGCH, PACK, 3>(h, P, a, st);
+    return launch_pipe<LOGCH, PACK, 1>(h, P, a, st);
 }
 
 }   // namespace
@@ -812,12 +789,14 @@ bool frt_pipe_supported(const BankPlan *pl, int block, int logch) {
     return (P.fdelta + nb - 1) / nb + 2 <= EN_RING;
 }
 
-cudaError_t frt_pipe_launch(const BankPlan *pl, BankArgs a, int logch, int pack, cudaStream_t st) {
-    if (!frt_pipe_supported(pl, a.block, logch)) return cudaErrorInvalidConfiguration;
+int frt_pipe_launch(frt_ctx *h, const BankPlan *pl, BankArgs a, int logch, int pack, cudaStream_t st) {
+    // two channels per lane run 32-sample steps only
+    if (!frt_pipe_supported(pl, a.block, logch) || (pack == 2 && logch != 5))
+        return frt_fail(h, FRT_EINVAL, "the pipelined filterbank kernel has no %d-sample steps with %d channels "
+                        "per lane for %d-sample blocks", 1 << logch, pack, a.block);
     const PipeParams &P = pl->pipe[logch - 5];
     int T[BANK_MAX_OCT + 1];
     frt_pipe_schedule(P.n_oct, logch, a.t_total, T, &a.n_steps);
-    // two channels per lane run 32-sample steps only
-    if (pack == 2) return logch == 5 ? launch_pipe_bpo<5, 2>(P, a, st) : cudaErrorInvalidConfiguration;
-    return logch == 5 ? launch_pipe_bpo<5, 1>(P, a, st) : launch_pipe_bpo<6, 1>(P, a, st);
+    if (pack == 2) return launch_pipe_bpo<5, 2>(h, P, a, st);
+    return logch == 5 ? launch_pipe_bpo<5, 1>(h, P, a, st) : launch_pipe_bpo<6, 1>(h, P, a, st);
 }

@@ -8,6 +8,7 @@
 #include <map>
 #include <memory>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/frt.h"
@@ -174,6 +175,32 @@ struct DeviceGuard {
     }
 };
 
+// Without an opt-in a kernel may use 48 KiB of shared memory, static and dynamic together.  No kernel
+// here declares more than 1 KiB of static shared memory (400 B at most), so launches up to 47 KiB of
+// dynamic shared memory need no opt-in.
+constexpr size_t FRT_SMEM_NO_OPT_IN = 47 * 1024;
+
+// Every kernel launch of the library: kernel<<<grid, block, smem, st>>>(args...), reported through
+// frt_fail and counted in frt_launch_count once it has been accepted.  A launch above
+// FRT_SMEM_NO_OPT_IN first sets the kernel's dynamic shared-memory limit to exactly what it asks for.
+// The limit is a per-device attribute of the kernel, shared by every handle: the values set are all
+// above FRT_SMEM_NO_OPT_IN, so a launch that sets none never finds the limit below its need.
+template <class... Params, class... Args>
+int frt_launch(frt_ctx *h, void (*kernel)(Params...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
+               Args &&...args) {
+    if (smem > FRT_SMEM_NO_OPT_IN) {
+        const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess)
+            return frt_fail(h, FRT_ECUDA, "cudaFuncSetAttribute(%zu bytes of dynamic shared memory) failed: %s",
+                            smem, cudaGetErrorString(e));
+    }
+    kernel<<<grid, block, smem, st>>>(std::forward<Args>(args)...);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return frt_fail(h, FRT_ECUDA, "kernel launch failed: %s", cudaGetErrorString(e));
+    h->launches++;
+    return FRT_OK;
+}
+
 // Component-wise float2 arithmetic (sm_90 has no packed FP32 instructions: one scalar FADD / FMUL /
 // FFMA per component).  Plain operators on purpose: the compiler contracts a product that feeds a
 // sum into one FFMA (e.g. the Hann window into the first butterfly), one rounding fewer, and the
@@ -182,4 +209,31 @@ __device__ __forceinline__ float2 f2_add(float2 a, float2 b) { return make_float
 __device__ __forceinline__ float2 f2_mul(float2 a, float2 b) { return make_float2(a.x * b.x, a.y * b.y); }
 __device__ __forceinline__ float2 f2_fma(float2 a, float2 b, float2 c) {
     return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
+}
+
+// MUFU.LG2.  Every caller's argument is >= 1e-30 (normal), so the denormal fix-up of __log2f is not
+// needed.
+__device__ __forceinline__ float lg2_fast(float v) {
+    float r;
+    asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(v));
+    return r;
+}
+constexpr float kLog10Scale = 3.01029995663981195f;   // 10 / log2(10): 10 log10(v) = kLog10Scale log2(v)
+
+// cp.async: global -> shared copies that bypass the registers, waited for by commit group
+__device__ __forceinline__ unsigned smem_u32(const void *p) {
+    return (unsigned)__cvta_generic_to_shared(p);
+}
+__device__ __forceinline__ void cp_async4(void *smem, const void *gmem) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(smem_u32(smem)), "l"(gmem) : "memory");
+}
+__device__ __forceinline__ void cp_async8(void *smem, const void *gmem) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(smem_u32(smem)), "l"(gmem) : "memory");
+}
+__device__ __forceinline__ void cp_async16(void *smem, const void *gmem) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem)), "l"(gmem) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void cp_async_wait() {   // all but the N newest groups landed
+    asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
 }

@@ -440,8 +440,6 @@ extern "C" int frt_gcc_plan(frt_handle h, int length) {
     FRT_CUDA(h, pl->window.upload(win));
     FRT_CUDA(h, pl->perm.upload(perm));
     FRT_CUDA(h, pl->tw.upload(tw));
-    FRT_CUDA(h, cudaFuncSetAttribute(gcc_phat_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     (int)(sizeof(float2) * length)));
     h->gcc = std::move(pl);
     return FRT_OK;
 }
@@ -475,12 +473,5 @@ extern "C" int frt_gcc_phat(frt_handle h, const float *d0_dev, const float *d1_d
     a.val = val_dev;
     a.rd = pl->rd;
     int blocks = n_pairs < h->sm_count ? n_pairs : h->sm_count;
-    // the dynamic shared-memory limit is a per-device attribute of the kernel: another handle that
-    // planned a shorter frame may have lowered it since this plan was built
-    FRT_CUDA(h, cudaFuncSetAttribute(gcc_phat_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     (int)(sizeof(float2) * pl->L)));
-    gcc_phat_kernel<<<blocks, GCC_THREADS, sizeof(float2) * pl->L, (cudaStream_t)stream>>>(a);
-    h->launches++;
-    FRT_CUDA(h, cudaGetLastError());
-    return FRT_OK;
+    return frt_launch(h, gcc_phat_kernel, blocks, GCC_THREADS, sizeof(float2) * pl->L, (cudaStream_t)stream, a);
 }

@@ -8,12 +8,6 @@
 
 namespace {
 
-__device__ __forceinline__ float lg2_fast(float v) {
-    float r;
-    asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(v));
-    return r;
-}
-
 __device__ __forceinline__ void argmax_merge(double &best, int &besti, double ob, int oi) {
     if (ob > best || (ob == best && oi < besti)) {
         best = ob;
@@ -111,7 +105,7 @@ spectrum_reduce_kernel(const float *__restrict__ power, const float *__restrict_
             float sp[1];
             smooth_bin<1>(pk, stride_f, n_frames, a, dk, sp);
             s_sp[k] = sp[0];
-            v = 3.01029995663981195f * lg2_fast(sp[0] + 1e-30f);   // spectrum.py:95-101
+            v = kLog10Scale * lg2_fast(sp[0] + 1e-30f);   // spectrum.py:95-101
             if (weight) v += __ldg(weight + k);
         }
         db[(size_t)c * nbins + k] = v;
@@ -157,15 +151,9 @@ extern "C" int frt_spectrum_reduce(frt_handle h, const float *power_dev, int64_t
                          pitch_idx_dev, "NULL buffer");
     FRT_CHECK_ARG(h, sizeof(float) * (size_t)nbins <= 200 * 1024, "nbins too large");
     const size_t smem = sizeof(float) * (size_t)nbins;
-    if (smem > 48 * 1024)
-        FRT_CUDA(h, cudaFuncSetAttribute(spectrum_reduce_kernel<false>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    spectrum_reduce_kernel<false><<<n_channels, 256, smem, (cudaStream_t)stream>>>(
-        power_dev, nullptr, stride_c, stride_f, n_frames, nbins, alpha, disp_dev, nullptr,
-        weight_dev, db_dev, fmax_idx_dev, pitch_idx_dev);
-    h->launches++;
-    FRT_CUDA(h, cudaGetLastError());
-    return FRT_OK;
+    return frt_launch(h, spectrum_reduce_kernel<false>, n_channels, 256, smem, (cudaStream_t)stream,
+                      power_dev, nullptr, stride_c, stride_f, n_frames, nbins, alpha, disp_dev, nullptr,
+                      weight_dev, db_dev, fmax_idx_dev, pitch_idx_dev);
 }
 
 extern "C" int frt_spectrum_reduce_dual(frt_handle h, const float *power1_dev,
@@ -183,15 +171,9 @@ extern "C" int frt_spectrum_reduce_dual(frt_handle h, const float *power1_dev,
                          db_dev && fmax_idx_dev && pitch_idx_dev, "NULL buffer");
     FRT_CHECK_ARG(h, sizeof(float) * (size_t)nbins <= 200 * 1024, "nbins too large");
     const size_t smem = sizeof(float) * (size_t)nbins;
-    if (smem > 48 * 1024)
-        FRT_CUDA(h, cudaFuncSetAttribute(spectrum_reduce_kernel<true>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    spectrum_reduce_kernel<true><<<n_pairs, 256, smem, (cudaStream_t)stream>>>(
-        power1_dev, power2_dev, stride_c, stride_f, n_frames, nbins, alpha, disp1_dev, disp2_dev,
-        nullptr, db_dev, fmax_idx_dev, pitch_idx_dev);
-    h->launches++;
-    FRT_CUDA(h, cudaGetLastError());
-    return FRT_OK;
+    return frt_launch(h, spectrum_reduce_kernel<true>, n_pairs, 256, smem, (cudaStream_t)stream,
+                      power1_dev, power2_dev, stride_c, stride_f, n_frames, nbins, alpha, disp1_dev, disp2_dev,
+                      nullptr, db_dev, fmax_idx_dev, pitch_idx_dev);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -287,13 +269,10 @@ extern "C" int frt_plot_curves(frt_handle h, const float *y_dev, int64_t stride_
     FRT_CHECK_ARG(h, y_dev && scaled_y_dev && z_dev, "NULL buffer");
     FRT_CHECK_ARG(h, !peaks || (peak_dev && peak_int_dev && decay_dev && scaled_peak_dev && z_peak_dev),
                   "NULL peak buffer");
-    plot_curves_kernel<<<n_channels, 256, 0, (cudaStream_t)stream>>>(
-        y_dev, stride_c, stride_s, n_steps, nbins, spec_min, spec_max, d0, peaks ? 1 : 0,
-        reset ? 1 : 0, peak_dev, peak_int_dev, decay_dev, scaled_y_dev, z_dev, scaled_peak_dev,
-        z_peak_dev);
-    h->launches++;
-    FRT_CUDA(h, cudaGetLastError());
-    return FRT_OK;
+    return frt_launch(h, plot_curves_kernel, n_channels, 256, 0, (cudaStream_t)stream,
+                      y_dev, stride_c, stride_s, n_steps, nbins, spec_min, spec_max, d0, peaks ? 1 : 0,
+                      reset ? 1 : 0, peak_dev, peak_int_dev, decay_dev, scaled_y_dev, z_dev, scaled_peak_dev,
+                      z_peak_dev);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -377,19 +356,15 @@ extern "C" int frt_display_columns(frt_handle h, const float *db_dev, int64_t st
     if (n_out > 0) {
         const long long total = (long long)height * n_out;
         dim3 grid((unsigned)((total + 255) / 256), (unsigned)n_channels);
-        display_kernel<<<grid, 256, 0, st>>>(db_dev, stride_c, stride_f, n_frames, weight_dev,
-                                             spec_min, inv_range, row_i0_dev, row_t_dev, height,
-                                             out_col_dev, out_a_dev, n_out, old_data_dev,
-                                             reinterpret_cast<const unsigned *>(lut_dev),
-                                             reinterpret_cast<unsigned *>(pixels_dev));
-        h->launches++;
+        const int rc = frt_launch(h, display_kernel, grid, 256, 0, st, db_dev, stride_c, stride_f, n_frames,
+                                  weight_dev, spec_min, inv_range, row_i0_dev, row_t_dev, height,
+                                  out_col_dev, out_a_dev, n_out, old_data_dev,
+                                  reinterpret_cast<const unsigned *>(lut_dev),
+                                  reinterpret_cast<unsigned *>(pixels_dev));
+        if (rc) return rc;
     }
     dim3 grid2((unsigned)((height + 255) / 256), (unsigned)n_channels);
-    display_kernel<<<grid2, 256, 0, st>>>(db_dev, stride_c, stride_f, n_frames, weight_dev, spec_min,
-                                          inv_range, row_i0_dev, row_t_dev, height, nullptr, nullptr,
-                                          0, old_data_dev, reinterpret_cast<const unsigned *>(lut_dev),
-                                          nullptr);
-    h->launches++;
-    FRT_CUDA(h, cudaGetLastError());
-    return FRT_OK;
+    return frt_launch(h, display_kernel, grid2, 256, 0, st, db_dev, stride_c, stride_f, n_frames, weight_dev,
+                      spec_min, inv_range, row_i0_dev, row_t_dev, height, nullptr, nullptr, 0, old_data_dev,
+                      reinterpret_cast<const unsigned *>(lut_dev), nullptr);
 }

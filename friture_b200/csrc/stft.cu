@@ -28,7 +28,6 @@
 
 namespace {
 
-constexpr float kLog10Scale = 3.01029995663981195f;   // 10 / log2(10)
 constexpr float kEps = 1e-30f;                        // friture/spectrogram.py:124
 
 __device__ __forceinline__ float2 cadd(float2 a, float2 b) { return f2_add(a, b); }
@@ -128,14 +127,6 @@ __host__ __device__ constexpr int brevq(int r) {
     return o;
 }
 
-__device__ __forceinline__ float lg2_fast(float v) {
-    // MUFU.LG2; the argument is always >= 1e-30 (normal), so the denormal fix-up of
-    // __log2f is not needed
-    float r;
-    asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(v));
-    return r;
-}
-
 template <int MODE>
 __device__ __forceinline__ float finish(float mag2, float scale) {
     // mag2*scale = |X|^2/N^2 (audioproc.py:49-50); log mode: spectrogram.py:119-125
@@ -144,9 +135,6 @@ __device__ __forceinline__ float finish(float mag2, float scale) {
 }
 
 // ---- TMA bulk copy (cp.async.bulk, SASS UBLKCP) + mbarrier helpers ------------------------------
-__device__ __forceinline__ unsigned smem_u32(const void *p) {
-    return (unsigned)__cvta_generic_to_shared(p);
-}
 __device__ __forceinline__ void mbar_init(unsigned long long *bar, unsigned count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
 }
@@ -520,12 +508,6 @@ constexpr size_t large_smem() {
 __device__ __forceinline__ void group_barrier(int id, int nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
-__device__ __forceinline__ void cp_async8(void *dst_smem, const void *src) {
-    asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(smem_u32(dst_smem)), "l"(src) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit_wait_all() {
-    asm volatile("cp.async.commit_group;\ncp.async.wait_group 0;" ::: "memory");
-}
 
 // split twiddle U[kk] = -j W_N^kk for kk in [0, M] from a table of M/2 + 1 entries:
 // U[kk + M/2] = -j U[kk]
@@ -583,7 +565,8 @@ stft_large_kernel(const float *__restrict__ x, long long x_stride, long long n_f
     };
     if (item < item_end) fetch(c, f);
     for (; item < item_end; item++) {
-        cp_async_commit_wait_all();
+        cp_async_commit();
+        cp_async_wait<0>();
         group_barrier(1 + grp, GT);          // the whole frame has landed
         float2 v[32];
 #pragma unroll
@@ -713,39 +696,11 @@ __global__ void stft_generic_kernel(const float *__restrict__ x, long long x_str
 
 size_t multi_smem(int r) { return sizeof(float2) * (1024 + (size_t)r * TILE); }
 
-// every instance's dynamic shared-memory limit: what its launch below asks for
-template <int MODE>
-cudaError_t set_smem_limits() {
-    const std::pair<const void *, size_t> limits[] = {
-        {(const void *)stft_small_kernel<1, MODE, false>, small_smem<1>()},
-        {(const void *)stft_small_kernel<2, MODE, false>, small_smem<2>()},
-        {(const void *)stft_small_kernel<4, MODE, false>, small_smem<4>()},
-        {(const void *)stft_small_kernel<8, MODE, false>, small_smem<8>()},
-        {(const void *)stft_small_kernel<16, MODE, false>, small_smem<16>()},
-        {(const void *)stft_small_kernel<32, MODE, false>, small_smem<32>()},
-        {(const void *)stft_small_kernel<32, MODE, true>, small_smem<32>()},
-        {(const void *)stft_large_kernel<2, MODE>, large_smem<2>()},
-        {(const void *)stft_large_kernel<4, MODE>, large_smem<4>()},
-        {(const void *)stft_multi_kernel<2, MODE>, multi_smem(2)},
-        {(const void *)stft_multi_kernel<4, MODE>, multi_smem(4)},
-        {(const void *)stft_multi_kernel<8, MODE>, multi_smem(8)},
-        {(const void *)stft_generic_kernel, sizeof(float2) * 2 * 8192},
-    };
-    for (const auto &l : limits) {
-        const cudaError_t e =
-            cudaFuncSetAttribute(l.first, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)l.second);
-        if (e != cudaSuccess) return e;
-    }
-    return cudaSuccess;
-}
-
 // calls launch with the mode (FRT_STFT_POWER / FRT_STFT_LOGPOWER) as a compile-time constant
 template <class F>
-void with_mode(int mode, F &&launch) {
-    if (mode == FRT_STFT_POWER)
-        launch(std::integral_constant<int, FRT_STFT_POWER>());
-    else
-        launch(std::integral_constant<int, FRT_STFT_LOGPOWER>());
+int with_mode(int mode, F &&launch) {
+    if (mode == FRT_STFT_POWER) return launch(std::integral_constant<int, FRT_STFT_POWER>());
+    return launch(std::integral_constant<int, FRT_STFT_LOGPOWER>());
 }
 
 // how far every frame's first sample is aligned: 2 = 16 bytes, 1 = 8 bytes, 0 = 4 bytes
@@ -767,20 +722,20 @@ struct Frames {
 };
 
 template <int Q, bool TMA = false>
-void launch_small(const frt_ctx *h, const StftPlan &pl, const Frames &a) {
+int launch_small(frt_ctx *h, const StftPlan &pl, const Frames &a) {
     constexpr int G = 32 / Q, WARPS = small_warps<Q>();
     const long long max_blocks = (long long)small_ctas_per_sm<Q>() * h->sm_count;
     long long blocks = ((a.total + G - 1) / G + WARPS - 1) / WARPS;
     if (blocks > max_blocks) blocks = max_blocks;
     const float2 *w2 = reinterpret_cast<const float2 *>(pl.win_dev.get());
-    with_mode(a.mode, [&](auto m) {
-        stft_small_kernel<Q, decltype(m)::value, TMA><<<(unsigned)blocks, WARPS * 32, small_smem<Q>(), a.st>>>(
-            a.x, a.x_stride, a.n_frames, a.hop, a.out, a.osc, a.osf, w2, pl.tw_dev.get(), pl.post_dev.get(),
-            a.total, a.vec_ok);
+    return with_mode(a.mode, [&](auto m) {
+        return frt_launch(h, stft_small_kernel<Q, decltype(m)::value, TMA>, (unsigned)blocks, WARPS * 32,
+                          small_smem<Q>(), a.st, a.x, a.x_stride, a.n_frames, a.hop, a.out, a.osc, a.osf, w2,
+                          pl.tw_dev.get(), pl.post_dev.get(), a.total, a.vec_ok);
     });
 }
 template <int R>
-void launch_large(const frt_ctx *h, const StftPlan &pl, const Frames &a) {
+int launch_large(frt_ctx *h, const StftPlan &pl, const Frames &a) {
     constexpr int NG = LARGE_WARPS / R;
     long long blocks = (a.total + NG - 1) / NG;
     if (blocks > h->sm_count) blocks = h->sm_count;
@@ -790,22 +745,22 @@ void launch_large(const frt_ctx *h, const StftPlan &pl, const Frames &a) {
         const double a = theta * 64.0 * R * n1;
         ha.v[n1] = make_float2((float)(0.5 * cos(a)), (float)(0.5 * sin(a)));
     }
-    with_mode(a.mode, [&](auto m) {
-        stft_large_kernel<R, decltype(m)::value><<<(unsigned)blocks, LARGE_WARPS * 32, large_smem<R>(), a.st>>>(
-            a.x, a.x_stride, a.n_frames, a.hop, a.out, a.osc, a.osf,
-            reinterpret_cast<const float2 *>(pl.win_dev.get()), pl.wlane_dev.get(), pl.tw_dev.get(),
-            pl.comb_dev.get(), pl.post_dev.get(), a.total, ha);
+    return with_mode(a.mode, [&](auto m) {
+        return frt_launch(h, stft_large_kernel<R, decltype(m)::value>, (unsigned)blocks, LARGE_WARPS * 32,
+                          large_smem<R>(), a.st, a.x, a.x_stride, a.n_frames, a.hop, a.out, a.osc, a.osf,
+                          reinterpret_cast<const float2 *>(pl.win_dev.get()), pl.wlane_dev.get(), pl.tw_dev.get(),
+                          pl.comb_dev.get(), pl.post_dev.get(), a.total, ha);
     });
 }
 template <int R>
-void launch_multi(const frt_ctx *h, const StftPlan &pl, const Frames &a) {
+int launch_multi(frt_ctx *h, const StftPlan &pl, const Frames &a) {
     long long blocks = (long long)h->sm_count * (R == 8 ? 2 : (R == 4 ? 4 : 8));
     if (blocks > a.total) blocks = a.total;
     const float2 *w2 = reinterpret_cast<const float2 *>(pl.win_dev.get());
-    with_mode(a.mode, [&](auto m) {
-        stft_multi_kernel<R, decltype(m)::value><<<(unsigned)blocks, 32 * R, multi_smem(R), a.st>>>(
-            a.x, a.x_stride, a.n_frames, a.hop, a.out, a.osc, a.osf, w2, pl.tw_dev.get(), pl.comb_dev.get(),
-            pl.post_dev.get(), a.total, a.vec_ok);
+    return with_mode(a.mode, [&](auto m) {
+        return frt_launch(h, stft_multi_kernel<R, decltype(m)::value>, (unsigned)blocks, 32 * R, multi_smem(R),
+                          a.st, a.x, a.x_stride, a.n_frames, a.hop, a.out, a.osc, a.osf, w2, pl.tw_dev.get(),
+                          pl.comb_dev.get(), pl.post_dev.get(), a.total, a.vec_ok);
     });
 }
 
@@ -890,8 +845,6 @@ extern "C" int frt_stft_plan(frt_handle h, int n_fft) {
             }
         FRT_CUDA(h, pl.wlane_dev.upload(wl));
     }
-    FRT_CUDA(h, set_smem_limits<FRT_STFT_POWER>());
-    FRT_CUDA(h, set_smem_limits<FRT_STFT_LOGPOWER>());
     pl.n_fft = n_fft;
     h->stft = &h->stft_cache.emplace(n_fft, std::move(pl)).first->second;
     return FRT_OK;
@@ -926,35 +879,33 @@ extern "C" int frt_stft_process(frt_handle h, const float *x_dev, int64_t x_stri
                    mode, align >= 1, (cudaStream_t)stream};
     if (N >= 64 && N <= 2048) {
         switch (N / 64) {
-            case 1: launch_small<1>(h, pl, a); break;
-            case 2: launch_small<2>(h, pl, a); break;
-            case 4: launch_small<4>(h, pl, a); break;
-            case 8: launch_small<8>(h, pl, a); break;
-            case 16: launch_small<16>(h, pl, a); break;
+            case 1: return launch_small<1>(h, pl, a);
+            case 2: return launch_small<2>(h, pl, a);
+            case 4: return launch_small<4>(h, pl, a);
+            case 8: return launch_small<8>(h, pl, a);
+            case 16: return launch_small<16>(h, pl, a);
             default:   // 16-byte aligned frames: the TMA engine stages them (cp.async.bulk)
-                if (align == 2) launch_small<32, true>(h, pl, a);
-                else launch_small<32>(h, pl, a);
+                if (align == 2) return launch_small<32, true>(h, pl, a);
+                return launch_small<32>(h, pl, a);
         }
-    } else if ((N == 4096 || N == 8192) && a.vec_ok) {
-        if (N == 4096) launch_large<2>(h, pl, a);
-        else launch_large<4>(h, pl, a);
-    } else if (N >= 4096) {
-        if (N == 4096) launch_multi<2>(h, pl, a);
-        else if (N == 8192) launch_multi<4>(h, pl, a);
-        else launch_multi<8>(h, pl, a);
-    } else {
-        FRT_CHECK_ARG(h, total <= 0x7fffffffLL, "too many frames for one launch");
-        const int M = N / 2;
-        int threads = M / 4;
-        if (threads < 32) threads = 32;
-        if (threads > 512) threads = 512;
-        stft_generic_kernel<<<(unsigned)total, threads, sizeof(float2) * 2 * M, a.st>>>(
-            x_dev, x_stride, n_frames, hop, out_dev, out_stride_c, out_stride_f, pl.win_dev.get(),
-            pl.tw_dev.get(), pl.post_dev.get(), mode, N, ilog2(M));
     }
-    h->launches++;
-    FRT_CUDA(h, cudaGetLastError());
-    return FRT_OK;
+    if ((N == 4096 || N == 8192) && a.vec_ok) {
+        if (N == 4096) return launch_large<2>(h, pl, a);
+        return launch_large<4>(h, pl, a);
+    }
+    if (N >= 4096) {
+        if (N == 4096) return launch_multi<2>(h, pl, a);
+        if (N == 8192) return launch_multi<4>(h, pl, a);
+        return launch_multi<8>(h, pl, a);
+    }
+    FRT_CHECK_ARG(h, total <= 0x7fffffffLL, "too many frames for one launch");
+    const int M = N / 2;
+    int threads = M / 4;
+    if (threads < 32) threads = 32;
+    if (threads > 512) threads = 512;
+    return frt_launch(h, stft_generic_kernel, (unsigned)total, threads, sizeof(float2) * 2 * M, a.st, x_dev,
+                      x_stride, n_frames, hop, out_dev, out_stride_c, out_stride_f, pl.win_dev.get(),
+                      pl.tw_dev.get(), pl.post_dev.get(), mode, N, ilog2(M));
 }
 
 extern "C" int frt_stft_process_host(frt_handle h, const float *x_host, int64_t x_stride,
