@@ -121,11 +121,13 @@ struct BankPlan;   // bank_internal.cuh
 struct DecPlan;    // bank.cu
 struct FirPlan;    // bank_fir.cu
 struct GccPlan;    // gcc_phat.cu
+struct GccLongPlan;   // gcc_long.cu
 struct PlanDelete {
     void operator()(BankPlan *p) const;
     void operator()(DecPlan *p) const;
     void operator()(FirPlan *p) const;
     void operator()(GccPlan *p) const;
+    void operator()(GccLongPlan *p) const;
 };
 template <class Plan>
 using PlanPtr = std::unique_ptr<Plan, PlanDelete>;
@@ -143,6 +145,8 @@ struct frt_ctx {
     PlanPtr<DecPlan> dec;
     PlanPtr<FirPlan> fir;
     PlanPtr<GccPlan> gcc;
+    PlanPtr<GccLongPlan> gcc_long;
+    DeviceArray<unsigned char> gcc_long_ws;   // frt_gcc_long_phat's workspace, grow-only
     StftStaging stft_host;
     CombStaging comb_host;
 };

@@ -15,6 +15,7 @@
 #include <cmath>
 
 #include "frt_internal.cuh"
+#include "fft_radix.cuh"
 
 namespace {
 
@@ -34,29 +35,6 @@ struct GccRadices {
     unsigned magic[GCC_MAX_PASSES];   // ceil(2^32 / n_next) of the pass: idx / n_next == umulhi(idx, magic)
 };
 
-__device__ __forceinline__ float2 cadd(float2 a, float2 b) { return make_float2(a.x + b.x, a.y + b.y); }
-__device__ __forceinline__ float2 csub(float2 a, float2 b) { return make_float2(a.x - b.x, a.y - b.y); }
-__device__ __forceinline__ float2 cmul(float2 a, float2 w) {
-    return make_float2(fmaf(a.x, w.x, -a.y * w.y), fmaf(a.x, w.y, a.y * w.x));
-}
-__device__ __forceinline__ float2 mul_mj(float2 a) { return make_float2(a.y, -a.x); }   // * (-j)
-__device__ __forceinline__ float2 cscale(float2 a, float s) { return make_float2(a.x * s, a.y * s); }
-
-template <int R> __device__ __forceinline__ void dft(float2 (&v)[R]);
-
-template <> __device__ __forceinline__ void dft<2>(float2 (&v)[2]) {
-    const float2 a = v[0], b = v[1];
-    v[0] = cadd(a, b);
-    v[1] = csub(a, b);
-}
-template <> __device__ __forceinline__ void dft<4>(float2 (&v)[4]) {
-    const float2 s02 = cadd(v[0], v[2]), d02 = csub(v[0], v[2]);
-    const float2 s13 = cadd(v[1], v[3]), d13 = mul_mj(csub(v[1], v[3]));
-    v[0] = cadd(s02, s13);
-    v[1] = cadd(d02, d13);
-    v[2] = csub(s02, s13);
-    v[3] = csub(d02, d13);
-}
 template <> __device__ __forceinline__ void dft<3>(float2 (&v)[3]) {
     const float s = 0.86602540378443864676f;
     const float2 t = cadd(v[1], v[2]);
@@ -195,36 +173,6 @@ static int digit_reverse(int k, int L, const GccRadices &rd) {
         k = kq;
     }
     return pos;
-}
-
-__device__ __forceinline__ float block_sum(float v, float *s_red) {
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
-    __syncthreads();
-    if (l == 0) s_red[w] = v;
-    __syncthreads();
-    float t = (threadIdx.x < (blockDim.x >> 5)) ? s_red[threadIdx.x] : 0.f;
-    if (w == 0) {
-        for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
-        if (l == 0) s_red[32] = t;
-    }
-    __syncthreads();
-    return s_red[32];
-}
-
-__device__ __forceinline__ float block_max(float v, float *s_red) {
-    for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-    const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
-    __syncthreads();
-    if (l == 0) s_red[w] = v;
-    __syncthreads();
-    float t = (threadIdx.x < (blockDim.x >> 5)) ? s_red[threadIdx.x] : -INFINITY;
-    if (w == 0) {
-        for (int o = 16; o > 0; o >>= 1) t = fmaxf(t, __shfl_xor_sync(0xffffffffu, t, o));
-        if (l == 0) s_red[32] = t;
-    }
-    __syncthreads();
-    return s_red[32];
 }
 
 struct GccArgs {
@@ -391,16 +339,12 @@ struct GccPlan {
 
 void PlanDelete::operator()(GccPlan *p) const { delete p; }
 
-extern "C" int frt_gcc_plan(frt_handle h, int length) {
-    if (!h) return FRT_EINVAL;
-    DeviceGuard g(h->device);
-    FRT_CHECK_ARG(h, length >= 4 && (length % 2) == 0, "length must be even and >= 4");
-    FRT_CHECK_ARG(h, (size_t)length * sizeof(float2) <= 220 * 1024,
-                  "length too large for the shared-memory FFT (max 28160)");
-    FRT_CHECK_ARG(h, (length / 2 + 1 + GCC_THREADS - 1) / GCC_THREADS <= GCC_MAX_PER_THREAD,
-                  "length too large");
-    if (h->gcc && h->gcc->L == length) return FRT_OK;
-    GccRadices rd;
+// The lengths this kernel takes, and their pass sequence: NULL when `length` is accepted, else why not.
+static const char *gcc_rule(int length, GccRadices &rd) {
+    if (!(length >= 4 && (length % 2) == 0)) return "length must be even and >= 4";
+    if (!((size_t)length * sizeof(float2) <= 220 * 1024))
+        return "length too large for the shared-memory FFT (max 28160)";
+    if (!((length / 2 + 1 + GCC_THREADS - 1) / GCC_THREADS <= GCC_MAX_PER_THREAD)) return "length too large";
     rd.n_passes = 0;
     int n = length;
     // large composite radices first (16 = 4x4, 25 = 5x5, 15 = 3x5 run in registers): every pass
@@ -412,8 +356,21 @@ extern "C" int frt_gcc_plan(frt_handle h, int length) {
     while (n % 15 == 0 && rd.n_passes < GCC_MAX_PASSES) { rd.radix[rd.n_passes++] = 15; n /= 15; }
     while (n % 5 == 0 && rd.n_passes < GCC_MAX_PASSES) { rd.radix[rd.n_passes++] = 5; n /= 5; }
     while (n % 3 == 0 && rd.n_passes < GCC_MAX_PASSES) { rd.radix[rd.n_passes++] = 3; n /= 3; }
-    if (n != 1)
-        return frt_fail(h, FRT_EINVAL, "length %d is not of the form 2^a 3^b 5^c", length);
+    if (n != 1) return "length is not of the form 2^a 3^b 5^c";
+    return nullptr;
+}
+
+extern "C" int frt_gcc_fits(int length) {
+    GccRadices rd;
+    return gcc_rule(length, rd) == nullptr;
+}
+
+extern "C" int frt_gcc_plan(frt_handle h, int length) {
+    if (!h) return FRT_EINVAL;
+    DeviceGuard g(h->device);
+    GccRadices rd;
+    if (const char *why = gcc_rule(length, rd)) return frt_fail(h, FRT_EINVAL, "length %d: %s", length, why);
+    if (h->gcc && h->gcc->L == length) return FRT_OK;
     {
         int nn = length;
         for (int i = 0; i < rd.n_passes; i++) {

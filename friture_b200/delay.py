@@ -11,7 +11,7 @@ import numpy as np
 from . import _lib, filter_data
 from ._lib import Handle
 from .audioproc import SAMPLING_RATE
-from .correlation import GccPhat
+from .correlation import gcc_phat_for
 from .stream import StreamFramer
 
 DEFAULT_DELAYRANGE = 1   # seconds, friture/delay_estimator.py:31
@@ -64,9 +64,14 @@ class DelayEstimator:
         self.needed = int(0.5 * self.length)                                 # :116-117
         self.dec0 = Decimator(n_pairs, self.Ndec, self.device)
         self.dec1 = Decimator(n_pairs, self.Ndec, self.device)
-        self.fr0 = StreamFramer(n_pairs, self.length, self.needed, self.device, pre_increment=True)
-        self.fr1 = StreamFramer(n_pairs, self.length, self.needed, self.device, pre_increment=True)
-        self.gcc = GccPhat(self.length, handle=self.dec0.handle, fs=self.subsampled_sampling_rate)
+        # a frame and its successor's hop, plus room for a few chunks; the framers grow when a
+        # longer chunk arrives (the default capacity, 4 L + 64 hops, is 3.5 GB per pair at 1000 s)
+        capacity = 2 * self.length + 4096
+        self.fr0 = StreamFramer(n_pairs, self.length, self.needed, self.device, capacity=capacity,
+                                pre_increment=True)
+        self.fr1 = StreamFramer(n_pairs, self.length, self.needed, self.device, capacity=capacity,
+                                pre_increment=True)
+        self.gcc = gcc_phat_for(self.length, handle=self.dec0.handle, fs=self.subsampled_sampling_rate)
         self.delay_ms = np.zeros(n_pairs)
         self.distance_m = np.zeros(n_pairs)
         self.correlation = np.zeros(n_pairs, dtype=int)

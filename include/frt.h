@@ -211,6 +211,22 @@ int frt_gcc_plan(frt_handle h, int length);
 int frt_gcc_phat(frt_handle h, const float *d0_dev, const float *d1_dev, int64_t stride,
                  int n_pairs, float *xcorr_dev, float *smoothed_dev, int have_prev, int *idx_dev,
                  float *val_dev, void *stream);
+/* 1 when frt_gcc_plan accepts `length`, else 0.  Pure host arithmetic (needs no GPU or handle).  */
+int frt_gcc_fits(int length);
+
+/* The same for every frame length the widget offers (0.1 .. 1000 s: L = 4 .. 24 000 000, odd or
+ * even), through Bluestein transforms over a power-of-two FFT of M = 2^m >= 2L-1 points in global
+ * memory.  For odd L the reference's irfft(W*G) returns L' = L-1 samples (the bin (L-1)/2 counts
+ * as Nyquist); for even L, L' = L.  The handle owns the plan (chirps and filter spectra, built in
+ * double precision: a few seconds on the host at the longest lengths) and a grow-only workspace;
+ * pairs run in groups whose workspace of about 8*M + 4*L' bytes per pair fits 2 GiB, one pair at
+ * least.  A call is asynchronous on `stream` unless the workspace has to grow.                  */
+int frt_gcc_long_plan(frt_handle h, int length);
+/* Arguments and results as frt_gcc_phat; xcorr_dev and smoothed_dev are [n_pairs][L'].  A pair's
+ * results are the same bits whatever n_pairs and run to run.                                     */
+int frt_gcc_long_phat(frt_handle h, const float *d0_dev, const float *d1_dev, int64_t stride,
+                      int n_pairs, float *xcorr_dev, float *smoothed_dev, int have_prev, int *idx_dev,
+                      float *val_dev, void *stream);
 
 /* ---------------------------------------------------------------- N-fold decimation
  * Stands behind `decimate_multiple(Ndec, bdec, adec, x, zis)` (friture/signal/decimate.py:45-71),
