@@ -20,32 +20,24 @@ def generalized_cross_correlation(d0, d1, handle=None):
     d1 = np.ascontiguousarray(d1, dtype=np.float32)
     if d0.ndim != 1 or d0.shape != d1.shape:
         raise ValueError("d0 and d1 must be 1-D arrays of the same length")
-    est = gcc_phat_for(d0.shape[0], handle=handle)
+    est = GccPhat(d0.shape[0], handle=handle)
     dev = torch.device("cuda", est.handle.device)
     _, _, x = est.estimate(torch.from_numpy(d0).to(dev)[None, :], torch.from_numpy(d1).to(dev)[None, :],
                            smooth=False, want_xcorr=True)
     return x[0].cpu().numpy().astype(np.float64)
 
 
-def gcc_phat_for(length, handle=None, fs=12000.0):
-    """The estimator for frames of ``length`` samples: ``GccPhat`` (the whole frame in shared
-    memory) when its kernel takes the length, ``LongGccPhat`` otherwise."""
-    if _lib.load_library().frt_gcc_fits(int(length)):
-        return GccPhat(length, handle=handle, fs=fs)
-    return LongGccPhat(length, handle=handle, fs=fs)
-
-
 class GccPhat:
-    """Batched GCC-PHAT over independent channel pairs.  ``estimate`` returns
+    """Batched GCC-PHAT over independent channel pairs, for every frame length the delay widget
+    offers (4 .. 24 000 000 samples, odd or even).  ``estimate`` returns
     (index of max |Xs|, Xs at that index, Xcorr or None); with ``smooth`` the handle keeps
-    ``Xs = 0.3*X + 0.7*Xs_prev`` per pair across calls like the widget's ``old_Xcorr``."""
-
-    _plan = "frt_gcc_plan"
-    _run = "frt_gcc_phat"
+    ``Xs = 0.3*X + 0.7*Xs_prev`` per pair across calls like the widget's ``old_Xcorr``.  For an odd
+    length Xcorr and the smoothed buffer hold ``length - 1`` samples, like the reference's
+    ``irfft``."""
 
     def __init__(self, length, handle=None, fs=12000.0):
         self.length = int(length)
-        self.out_length = self.length     # samples of Xcorr and of the smoothed buffer
+        self.out_length = self.length - (self.length & 1)   # samples of Xcorr and of the smoothed buffer
         self.fs = fs                      # 48 kHz / 2**Ndec, delay_estimator.py:53-54
         self._handle = handle
         self._smoothed = None
@@ -75,7 +67,7 @@ class GccPhat:
         self.handle.check_device(d1)
         d0 = d0.contiguous()
         d1 = d1.contiguous()
-        self.handle.call(self._plan, int(L))
+        self.handle.call("frt_gcc_plan", int(L))
         Lo = self.out_length
         idx = torch.empty(P, dtype=torch.int32, device=d0.device)
         val = torch.empty(P, dtype=torch.float32, device=d0.device)
@@ -91,7 +83,7 @@ class GccPhat:
             # frame (the kernel marks it), like old_Xcorr = None in the widget
             have_prev = 2 if self._have_prev else 0
         sp = _lib.current_stream_ptr(d0.device) if stream is None else c_void_p(int(stream))
-        self.handle.call(self._run, _lib._ptr(d0), _lib._ptr(d1), int(L), int(P),
+        self.handle.call("frt_gcc_phat", _lib._ptr(d0), _lib._ptr(d1), int(L), int(P),
                          _lib._ptr(xc), _lib._ptr(sm), have_prev, _lib._ptr(idx), _lib._ptr(val), sp)
         if smooth:
             self._have_prev = True
@@ -102,16 +94,3 @@ class GccPhat:
         d = 1e3 * idx.to("cpu").double().numpy() / self.fs
         span = 1e3 * self.length / self.fs
         return np.where(d > span / 2.0, d - span, d)
-
-
-class LongGccPhat(GccPhat):
-    """``GccPhat`` for every frame length the delay widget offers (4 .. 24 000 000 samples, odd or
-    even), through Bluestein transforms in global memory.  For an odd length Xcorr and the smoothed
-    buffer hold ``length - 1`` samples, like the reference's ``irfft``."""
-
-    _plan = "frt_gcc_long_plan"
-    _run = "frt_gcc_long_phat"
-
-    def __init__(self, length, handle=None, fs=12000.0):
-        super().__init__(length, handle=handle, fs=fs)
-        self.out_length = self.length - (self.length & 1)

@@ -132,6 +132,15 @@ struct PlanDelete {
 template <class Plan>
 using PlanPtr = std::unique_ptr<Plan, PlanDelete>;
 
+// GCC-PHAT: frt_gcc_plan / frt_gcc_phat (gcc_phat.cu) run lengths the shared-memory kernel cannot
+// hold on the Bluestein route of gcc_long.cu.  gcc_long_phat expects the arguments checked.
+std::vector<float> gcc_hanning(int length);   // numpy.hanning(length), evaluated in double
+int gcc_long_plan(frt_ctx *h, int length);
+int gcc_long_length(const frt_ctx *h);        // the planned L; needs h->gcc_long
+int gcc_long_phat(frt_ctx *h, const float *d0_dev, const float *d1_dev, int64_t stride, int n_pairs,
+                  float *xcorr_dev, float *smoothed_dev, int have_prev, int *idx_dev, float *val_dev,
+                  cudaStream_t st);
+
 // A plan call builds into a local PlanPtr and moves it into its slot only on success, so a call
 // that fails leaves the previous plan of that kind in place.
 struct frt_ctx {
@@ -144,9 +153,10 @@ struct frt_ctx {
     PlanPtr<BankPlan> bank;
     PlanPtr<DecPlan> dec;
     PlanPtr<FirPlan> fir;
-    PlanPtr<GccPlan> gcc;
-    PlanPtr<GccLongPlan> gcc_long;
-    DeviceArray<unsigned char> gcc_long_ws;   // frt_gcc_long_phat's workspace, grow-only
+    PlanPtr<GccPlan> gcc;             // frt_gcc_plan keeps one plan of each route, so that switching
+    PlanPtr<GccLongPlan> gcc_long;    // lengths back and forth rebuilds neither
+    bool gcc_long_route = false;      // the last accepted frt_gcc_plan length runs on gcc_long
+    DeviceArray<unsigned char> gcc_long_ws;   // the Bluestein route's workspace, grow-only
     StftStaging stft_host;
     CombStaging comb_host;
 };

@@ -1,8 +1,9 @@
-// GCC-PHAT for frames the shared-memory kernel of gcc_phat.cu cannot hold: every length
-// L = 4 .. 24 000 000, odd or even -- the delay widget's ranges 0.1 s .. 1000 s give
-// L = int(2 * range * 12000) (friture/delay_estimator.py:114-117,222-226).  Same numerics as
-// frt_gcc_phat (correlation.py:24-43, delay_estimator.py:129-142); for odd L numpy's irfft(W*G)
-// has L' = L-1 points, and everything after the forward transform is L' long.
+// The Bluestein route of frt_gcc_plan / frt_gcc_phat (gcc_phat.cu), for the frames its
+// shared-memory kernel cannot hold: any length L = 4 .. 24 000 000, odd or even -- the delay
+// widget's ranges 0.1 s .. 1000 s give L = int(2 * range * 12000)
+// (friture/delay_estimator.py:114-117,222-226).  Same numerics as gcc_phat_kernel
+// (correlation.py:24-43, delay_estimator.py:129-142); for odd L numpy's irfft(W*G) has L' = L-1
+// points, and everything after the forward transform is L' long.
 //
 //   u = (d0 - mean) hann + j (d1 - mean) hann      Z = DFT_L(u)          (one complex transform)
 //   D0/D1 from Z[k], conj Z[L-k];  G = conj(D0) D1, k = 0..L'/2;  Y = G / (1e-10 max|G| + |G|)
@@ -453,9 +454,7 @@ struct GccLongPlan {
 
 void PlanDelete::operator()(GccLongPlan *p) const { delete p; }
 
-extern "C" int frt_gcc_long_plan(frt_handle h, int length) {
-    if (!h) return FRT_EINVAL;
-    DeviceGuard g(h->device);
+int gcc_long_plan(frt_ctx *h, int length) {
     FRT_CHECK_ARG(h, length >= 4 && length <= GL_MAX_LENGTH, "length must be 4 .. 24000000");
     if (h->gcc_long && h->gcc_long->L == length) return FRT_OK;
     PlanPtr<GccLongPlan> pl(new (std::nothrow) GccLongPlan());
@@ -474,10 +473,7 @@ extern "C" int frt_gcc_long_plan(frt_handle h, int length) {
     try {
         const double PI = 3.14159265358979323846;
         const double M = std::ldexp(1.0, log_m);
-        std::vector<float> win(length);
-        for (int i = 0; i < length; i++)   // numpy.hanning(L)   (correlation.py:31)
-            win[i] = (float)(0.5 - 0.5 * cos(2.0 * PI * i / (double)(length - 1)));
-        FRT_CUDA(h, pl->window.upload(win));
+        FRT_CUDA(h, pl->window.upload(gcc_hanning(length)));
         std::vector<float2> t(size_t(1) << pl->log2);
         for (size_t i = 0; i < t.size(); i++) {
             const double ang = -2.0 * PI * (double)i / (double)t.size();
@@ -512,20 +508,12 @@ extern "C" int frt_gcc_long_plan(frt_handle h, int length) {
     return FRT_OK;
 }
 
-extern "C" int frt_gcc_long_phat(frt_handle h, const float *d0_dev, const float *d1_dev, int64_t stride,
-                                 int n_pairs, float *xcorr_dev, float *smoothed_dev, int have_prev,
-                                 int *idx_dev, float *val_dev, void *stream) {
-    if (!h) return FRT_EINVAL;
-    if (!h->gcc_long) return frt_fail(h, FRT_ESTATE, "frt_gcc_long_phat: call frt_gcc_long_plan first");
-    DeviceGuard g(h->device);
+int gcc_long_length(const frt_ctx *h) { return h->gcc_long->L; }
+
+int gcc_long_phat(frt_ctx *h, const float *d0_dev, const float *d1_dev, int64_t stride, int n_pairs,
+                  float *xcorr_dev, float *smoothed_dev, int have_prev, int *idx_dev, float *val_dev,
+                  cudaStream_t st) {
     const GccLongPlan *pl = h->gcc_long.get();
-    FRT_CHECK_ARG(h, n_pairs >= 0, "negative n_pairs");
-    if (n_pairs == 0) return FRT_OK;
-    FRT_CHECK_ARG(h, d0_dev && d1_dev && idx_dev && val_dev, "NULL buffer");
-    FRT_CHECK_ARG(h, stride >= pl->L, "stride smaller than the frame length");
-    FRT_CHECK_ARG(h, have_prev >= 0 && have_prev <= 2, "have_prev must be 0, 1 or 2");
-    FRT_CHECK_ARG(h, !have_prev || smoothed_dev, "have_prev needs the smoothed buffer");
-    const cudaStream_t st = (cudaStream_t)stream;
     const size_t M = size_t(1) << (pl->log1 + pl->log2), H = size_t(pl->Lp / 2 + 1);
     const int n_chunks = (pl->L + GL_STATS_CHUNK - 1) / GL_STATS_CHUNK;
     auto up = [](size_t b) { return (b + 255) & ~size_t(255); };

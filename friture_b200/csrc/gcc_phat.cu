@@ -365,11 +365,16 @@ extern "C" int frt_gcc_fits(int length) {
     return gcc_rule(length, rd) == nullptr;
 }
 
-extern "C" int frt_gcc_plan(frt_handle h, int length) {
-    if (!h) return FRT_EINVAL;
-    DeviceGuard g(h->device);
-    GccRadices rd;
-    if (const char *why = gcc_rule(length, rd)) return frt_fail(h, FRT_EINVAL, "length %d: %s", length, why);
+std::vector<float> gcc_hanning(int length) {
+    const double PI = 3.14159265358979323846;
+    std::vector<float> win(length);
+    for (int i = 0; i < length; i++)   // 0.5 - 0.5 cos(2 pi n / (L-1))   (correlation.py:31)
+        win[i] = (float)(0.5 - 0.5 * cos(2.0 * PI * i / (double)(length - 1)));
+    return win;
+}
+
+// The shared-memory route's plan for a length gcc_rule accepted, with its pass sequence rd.
+static int gcc_smem_plan(frt_ctx *h, int length, GccRadices rd) {
     if (h->gcc && h->gcc->L == length) return FRT_OK;
     {
         int nn = length;
@@ -384,36 +389,48 @@ extern "C" int frt_gcc_plan(frt_handle h, int length) {
     pl->L = length;
     pl->rd = rd;
     const double PI = 3.14159265358979323846;
-    std::vector<float> win(length);
     std::vector<float2> tw(length);
     for (int i = 0; i < length; i++) {
-        // numpy.hanning(L): 0.5 - 0.5 cos(2 pi n / (L-1))   (correlation.py:31)
-        win[i] = (float)(0.5 - 0.5 * cos(2.0 * PI * i / (double)(length - 1)));
         const double ang = -2.0 * PI * (double)i / (double)length;
         tw[i] = make_float2((float)cos(ang), (float)sin(ang));
     }
     std::vector<int> perm(length);
     for (int i = 0; i < length; i++) perm[i] = digit_reverse(i, length, rd);
-    FRT_CUDA(h, pl->window.upload(win));
+    FRT_CUDA(h, pl->window.upload(gcc_hanning(length)));
     FRT_CUDA(h, pl->perm.upload(perm));
     FRT_CUDA(h, pl->tw.upload(tw));
     h->gcc = std::move(pl);
     return FRT_OK;
 }
 
+extern "C" int frt_gcc_plan(frt_handle h, int length) {
+    if (!h) return FRT_EINVAL;
+    DeviceGuard g(h->device);
+    GccRadices rd;
+    const bool fits = gcc_rule(length, rd) == nullptr;
+    const int rc = fits ? gcc_smem_plan(h, length, rd) : gcc_long_plan(h, length);
+    if (rc == FRT_OK) h->gcc_long_route = !fits;
+    return rc;
+}
+
 extern "C" int frt_gcc_phat(frt_handle h, const float *d0_dev, const float *d1_dev, int64_t stride,
                             int n_pairs, float *xcorr_dev, float *smoothed_dev, int have_prev,
                             int *idx_dev, float *val_dev, void *stream) {
     if (!h) return FRT_EINVAL;
-    if (!h->gcc) return frt_fail(h, FRT_ESTATE, "frt_gcc_phat: call frt_gcc_plan first");
+    if (!(h->gcc_long_route ? (bool)h->gcc_long : (bool)h->gcc))
+        return frt_fail(h, FRT_ESTATE, "frt_gcc_phat: call frt_gcc_plan first");
     DeviceGuard g(h->device);
-    const GccPlan *pl = h->gcc.get();
+    const int L = h->gcc_long_route ? gcc_long_length(h) : h->gcc->L;
     FRT_CHECK_ARG(h, n_pairs >= 0, "negative n_pairs");
     if (n_pairs == 0) return FRT_OK;
     FRT_CHECK_ARG(h, d0_dev && d1_dev && idx_dev && val_dev, "NULL buffer");
-    FRT_CHECK_ARG(h, stride >= pl->L, "stride smaller than the frame length");
+    FRT_CHECK_ARG(h, stride >= L, "stride smaller than the frame length");
     FRT_CHECK_ARG(h, have_prev >= 0 && have_prev <= 2, "have_prev must be 0, 1 or 2");
     FRT_CHECK_ARG(h, !have_prev || smoothed_dev, "have_prev needs the smoothed buffer");
+    if (h->gcc_long_route)
+        return gcc_long_phat(h, d0_dev, d1_dev, stride, n_pairs, xcorr_dev, smoothed_dev, have_prev, idx_dev,
+                             val_dev, (cudaStream_t)stream);
+    const GccPlan *pl = h->gcc.get();
     GccArgs a;
     a.d0 = d0_dev;
     a.d1 = d1_dev;

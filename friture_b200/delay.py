@@ -11,7 +11,7 @@ import numpy as np
 from . import _lib, filter_data
 from ._lib import Handle
 from .audioproc import SAMPLING_RATE
-from .correlation import gcc_phat_for
+from .correlation import GccPhat
 from .stream import StreamFramer
 
 DEFAULT_DELAYRANGE = 1   # seconds, friture/delay_estimator.py:31
@@ -71,7 +71,7 @@ class DelayEstimator:
                                 pre_increment=True)
         self.fr1 = StreamFramer(n_pairs, self.length, self.needed, self.device, capacity=capacity,
                                 pre_increment=True)
-        self.gcc = gcc_phat_for(self.length, handle=self.dec0.handle, fs=self.subsampled_sampling_rate)
+        self.gcc = GccPhat(self.length, handle=self.dec0.handle, fs=self.subsampled_sampling_rate)
         self.delay_ms = np.zeros(n_pairs)
         self.distance_m = np.zeros(n_pairs)
         self.correlation = np.zeros(n_pairs, dtype=int)

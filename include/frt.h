@@ -195,13 +195,22 @@ int frt_peer_push(frt_handle h, const void *src, void *const *peer_dst, int n_pe
  * Stands behind `generalized_cross_correlation(d0, d1)` (friture/signal/correlation.py:24-43)
  * and the smoothing + peak pick around it (friture/delay_estimator.py:129-142).               */
 
-/* Plan for frames of `length` samples (even, 2^a 3^b 5^c, <= 28160; the widget's default is
- * 2 * delayrange_s * 12 kHz = 24000, delay_estimator.py:53-54,114-117).                       */
+/* Plan for frames of `length` samples, 4 .. 24 000 000 -- every delay range the widget offers
+ * (0.1 .. 1000 s, L = 2 * delayrange_s * 12 kHz, delay_estimator.py:53-54,114-117,222-226).
+ * Lengths frt_gcc_fits accepts (the default 24000 among them) run with the whole frame in shared
+ * memory.  All others run as Bluestein transforms over a power-of-two FFT of M = 2^m >= 2L-1
+ * points in global memory, whose plan (chirps and filter spectra, built in double precision)
+ * takes a few seconds of host time at the longest lengths, and whose calls use a grow-only
+ * workspace of about 8*M + 4*L' bytes per pair, in groups of pairs within 2 GiB (one pair at
+ * least); such a call is asynchronous on `stream` unless the workspace has to grow.  The handle
+ * keeps one plan of each kind; frt_gcc_phat runs the one the last accepted length chose.        */
 int frt_gcc_plan(frt_handle h, int length);
 /* n_pairs independent channel pairs: d0/d1[p*stride + n].  Inputs are not modified (the
- * reference subtracts the means in place, a side effect that is not reproduced).
- *   xcorr_dev     NULL or [n_pairs][length]: this frame's Xcorr (correlation.py:41)
- *   smoothed_dev  NULL or [n_pairs][length]: smoothed Xcorr (0.3*X + 0.7*old, delay_estimator.py:134-139),
+ * reference subtracts the means in place, a side effect that is not reproduced).  L' = L - 1 for
+ * odd L (the reference's irfft(W*G) returns L-1 samples; the bin (L-1)/2 counts as Nyquist), else
+ * L' = L.  A pair's results are the same bits whatever n_pairs and run to run.
+ *   xcorr_dev     NULL or [n_pairs][L']: this frame's Xcorr (correlation.py:41)
+ *   smoothed_dev  NULL or [n_pairs][L']: smoothed Xcorr (0.3*X + 0.7*old, delay_estimator.py:134-139),
  *                 written for every non-silent pair.  have_prev: 0 = first frame, nothing to blend
  *                 (a silent pair is marked "no previous" with a NaN in its slot 0); 1 = blend every
  *                 pair with the buffer; 2 = blend the pairs that have had a non-silent frame (no
@@ -211,22 +220,9 @@ int frt_gcc_plan(frt_handle h, int length);
 int frt_gcc_phat(frt_handle h, const float *d0_dev, const float *d1_dev, int64_t stride,
                  int n_pairs, float *xcorr_dev, float *smoothed_dev, int have_prev, int *idx_dev,
                  float *val_dev, void *stream);
-/* 1 when frt_gcc_plan accepts `length`, else 0.  Pure host arithmetic (needs no GPU or handle).  */
+/* 1 when frt_gcc_plan runs `length` on the shared-memory kernel (even, 2^a 3^b 5^c, <= 28160),
+ * else 0.  Pure host arithmetic (needs no GPU or handle).                                       */
 int frt_gcc_fits(int length);
-
-/* The same for every frame length the widget offers (0.1 .. 1000 s: L = 4 .. 24 000 000, odd or
- * even), through Bluestein transforms over a power-of-two FFT of M = 2^m >= 2L-1 points in global
- * memory.  For odd L the reference's irfft(W*G) returns L' = L-1 samples (the bin (L-1)/2 counts
- * as Nyquist); for even L, L' = L.  The handle owns the plan (chirps and filter spectra, built in
- * double precision: a few seconds on the host at the longest lengths) and a grow-only workspace;
- * pairs run in groups whose workspace of about 8*M + 4*L' bytes per pair fits 2 GiB, one pair at
- * least.  A call is asynchronous on `stream` unless the workspace has to grow.                  */
-int frt_gcc_long_plan(frt_handle h, int length);
-/* Arguments and results as frt_gcc_phat; xcorr_dev and smoothed_dev are [n_pairs][L'].  A pair's
- * results are the same bits whatever n_pairs and run to run.                                     */
-int frt_gcc_long_phat(frt_handle h, const float *d0_dev, const float *d1_dev, int64_t stride,
-                      int n_pairs, float *xcorr_dev, float *smoothed_dev, int have_prev, int *idx_dev,
-                      float *val_dev, void *stream);
 
 /* ---------------------------------------------------------------- N-fold decimation
  * Stands behind `decimate_multiple(Ndec, bdec, adec, x, zis)` (friture/signal/decimate.py:45-71),

@@ -60,7 +60,7 @@ def test_batch_vs_oracle(L):
     assert float(val[1]) < 0      # inverted polarity shows in the sign of the extremum
 
 
-def test_constant_input_and_inputs_untouched():
+def test_constant_input_inputs_untouched_and_short_frame_refused():
     import torch
     from friture_b200.correlation import GccPhat
     L = 4096
@@ -71,7 +71,7 @@ def test_constant_input_and_inputs_untouched():
     assert idx.tolist() == [0, 0] and val.tolist() == [0.0, 0.0]      # delay_estimator.py:164-167
     assert torch.equal(d1, d1c)
     with pytest.raises(ValueError):
-        GccPhat(7 * 1024).estimate(torch.zeros(1, 7 * 1024).cuda(), torch.zeros(1, 7 * 1024).cuda())
+        GccPhat(3).estimate(torch.zeros(1, 3).cuda(), torch.zeros(1, 3).cuda())
 
 
 def test_config4_sample_4096_pairs():

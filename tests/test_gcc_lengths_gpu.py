@@ -459,25 +459,58 @@ def test_decimator_channels_and_chunks(C, n_stages):
     assert max(rel) < DEC_REL_TOL, rel
 
 
-# --------------------------------------------------------------------------- GPU: rejected lengths
-@pytest.mark.gpu
-def test_rejected_lengths_leave_handle_usable():
-    """0.7 s and 1.1 s (factors 7 and 11), 28160 (fits the shared memory, factor 11), an odd and a
-    too short length raise ValueError; the handle's plan and results are unchanged afterwards."""
+# --------------------------------------------------------------------------- GPU: routes, rejected lengths
+SMEM_LAUNCHES = 1          # gcc_phat_kernel
+BLUESTEIN_LAUNCHES = 10    # the gl_* kernels of one workspace group
+
+
+def assert_route(est, launches):
+    """est's length runs on the route frt_gcc_plan picks for it: frt_gcc_fits says so, and one call
+    on one pair launches `launches` kernels."""
     import torch
+    from friture_b200 import _lib
+    assert _lib.load_library().frt_gcc_fits(est.length) == (launches == SMEM_LAUNCHES)
+    x = torch.randn((1, est.length), device="cuda")
+    n = est.handle.launch_count
+    est.estimate(x, x, smooth=False)
+    assert est.handle.launch_count - n == launches
+
+
+@pytest.mark.gpu
+def test_rejected_lengths_leave_both_routes_usable():
+    """0.7 s and 1.1 s (factors 7 and 11), 28160 (fits the shared memory, factor 11), an odd length
+    (Xcorr has L-1 samples) and 7168 (factor 7) run on the Bluestein route within the bound.  2, 3
+    and 24 000 001 raise ValueError; after each, a shared-memory and a Bluestein estimator on the
+    same handle give the same bits as their first call, each on its own route."""
+    import torch
+    import gcc_long_model as gm
     from friture_b200._lib import FrtValueError, Handle
     from friture_b200.correlation import GccPhat
     h = Handle(0)
-    L = 2400
-    d0, d1, _ = length_cases(L)
-    good = GccPhat(L, handle=h)
-    _, _, first = good.estimate(cuda(d0), cuda(d1), smooth=False, want_xcorr=True)
-    for p in range(8):
-        assert_within(first[p].cpu().numpy(), gcc_f64(d0[p], d1[p]), gcc_f32(d0[p], d1[p]),
-                      "L=%d %s" % (L, PAIR_KINDS[p]))
-    for bad in (16800, 26400, 28160, 2401, 2):
+    for L in (16800, 26400, 28160, 2401, 7168):
+        d0, d1, _ = length_cases(L)
+        est = GccPhat(L, handle=h)
+        idx, val, xc = est.estimate(cuda(d0), cuda(d1), smooth=False, want_xcorr=True)
+        assert xc.shape == (8, L - (L & 1))
+        idx, val, xc = idx.cpu().numpy(), val.cpu().numpy(), xc.cpu().numpy()
+        for p in range(8):
+            ref, f32 = gcc_f64(d0[p], d1[p]), gm.gcc_f32_any(d0[p], d1[p])
+            assert_within(xc[p], ref, f32, "L=%d %s" % (L, PAIR_KINDS[p]))
+            i, v, _ = fo.delay_peak(ref)
+            assert int(idx[p]) == i, (L, PAIR_KINDS[p], int(idx[p]), i)
+            assert abs(float(val[p]) - v) <= error_bound(ref, f32), (L, PAIR_KINDS[p])
+        assert_route(est, BLUESTEIN_LAUNCHES)
+    good = []
+    for L, launches in ((2400, SMEM_LAUNCHES), (55199, BLUESTEIN_LAUNCHES)):
+        d0, d1, _ = length_cases(L)
+        est, a, b = GccPhat(L, handle=h), cuda(d0), cuda(d1)
+        good.append((est, a, b, launches, est.estimate(a, b, smooth=False, want_xcorr=True)))
+    for bad in (3, 2, 24000001):
         z = torch.zeros((1, bad), device="cuda")
         with pytest.raises(FrtValueError):
             GccPhat(bad, handle=h).estimate(z, z + 1.0)
-        _, _, again = good.estimate(cuda(d0), cuda(d1), smooth=False, want_xcorr=True)
-        assert torch.equal(again, first), bad
+        for est, a, b, launches, first in good:
+            n = h.launch_count
+            again = est.estimate(a, b, smooth=False, want_xcorr=True)
+            assert h.launch_count - n == launches, (bad, est.length)
+            assert all(torch.equal(x, y) for x, y in zip(again, first)), (bad, est.length)

@@ -1,7 +1,8 @@
-"""The long GCC-PHAT path (friture_b200/csrc/gcc_long.cu, LongGccPhat) at the delay widget's
-lengths the shared-memory kernel rejects, odd lengths included (Xcorr then has L-1 samples, like
-the reference's irfft), against the float64 oracle with the bound of test_gcc_lengths_gpu: at most
-K = 20 times the error of the float32 restatement (gcc_long_model.gcc_f32_any), plus 1e-7."""
+"""GCC-PHAT's Bluestein route (friture_b200/csrc/gcc_long.cu), which GccPhat runs at the delay
+widget's lengths the shared-memory kernel rejects, odd lengths included (Xcorr then has L-1
+samples, like the reference's irfft), against the float64 oracle with the bound of
+test_gcc_lengths_gpu: at most K = 20 times the error of the float32 restatement
+(gcc_long_model.gcc_f32_any), plus 1e-7."""
 import os
 import sys
 
@@ -10,8 +11,9 @@ import pytest
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import gcc_long_model as gm  # noqa: E402
-from test_gcc_lengths_gpu import (ABS_FLOOR, K, PAIR_KINDS, DelayPipelineModel, assert_within,  # noqa: E402
-                                  error_bound, length_cases, shift_recoverable, smooth_f32, smooth_f64)
+from test_gcc_lengths_gpu import (ABS_FLOOR, BLUESTEIN_LAUNCHES, K, PAIR_KINDS, SMEM_LAUNCHES,  # noqa: E402
+                                  DelayPipelineModel, assert_route, assert_within, error_bound,
+                                  length_cases, shift_recoverable, smooth_f32, smooth_f64)
 
 from oracle import friture_oracle as fo  # noqa: E402
 
@@ -63,10 +65,10 @@ def check_frames(est, L, frames, label, pairs=range(8)):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("L", WIDGET + EXTRA)
-def test_length_vs_oracle(L):
-    from friture_b200.correlation import LongGccPhat, gcc_phat_for
-    est = gcc_phat_for(L)
-    assert isinstance(est, LongGccPhat)
+def test_long_length_vs_oracle(L):
+    from friture_b200.correlation import GccPhat
+    est = GccPhat(L)
+    assert_route(est, BLUESTEIN_LAUNCHES)
     if L < 1000000:
         check_frames(est, L, [length_cases(L, seed=s) for s in range(2)], "L=%d" % L)
     else:
@@ -76,25 +78,37 @@ def test_length_vs_oracle(L):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("L", [2400, 24000])
-def test_long_path_where_both_run(L):
-    """At lengths the shared-memory kernel also takes, the long path meets the same bound and
-    picks the same peaks as that kernel."""
-    from friture_b200.correlation import GccPhat, LongGccPhat
-    frames = [length_cases(L, seed=s) for s in range(3)]
-    check_frames(LongGccPhat(L), L, frames, "long L=%d" % L)
-    a, b, _ = frames[0]
-    i_short, _, _ = GccPhat(L).estimate(cuda(a), cuda(b), smooth=False)
-    i_long, _, _ = LongGccPhat(L).estimate(cuda(a), cuda(b), smooth=False)
-    assert np.array_equal(i_short.cpu().numpy(), i_long.cpu().numpy())
+def test_routes_alternate_on_one_handle():
+    """A shared-memory and a Bluestein estimator alternate on one handle for three rounds: each
+    call runs its own route and gives the same bits as on a fresh handle, so the handle follows
+    the route of the last plan call and keeps both plans."""
+    import torch
+    from friture_b200._lib import Handle
+    from friture_b200.correlation import GccPhat
+    cases = []
+    for L, launches in ((2400, SMEM_LAUNCHES), (16800, BLUESTEIN_LAUNCHES)):
+        d0, d1, _ = length_cases(L)
+        a, b = cuda(d0), cuda(d1)
+        fresh = Handle(0)
+        want = GccPhat(L, handle=fresh).estimate(a, b, smooth=False, want_xcorr=True)
+        fresh.close()
+        cases.append((L, launches, a, b, want))
+    h = Handle(0)
+    ests = {L: GccPhat(L, handle=h) for L, _, _, _, _ in cases}
+    for r in range(3):
+        for L, launches, a, b, want in cases:
+            n = h.launch_count
+            got = ests[L].estimate(a, b, smooth=False, want_xcorr=True)
+            assert h.launch_count - n == launches, (r, L)
+            assert all(torch.equal(x, y) for x, y in zip(got, want)), (r, L)
 
 
 @pytest.mark.gpu
-def test_same_bits_alone_in_groups_and_again():
+def test_long_same_bits_alone_in_groups_and_again():
     """One pair gives the same bits alone, as the first and the last of more pairs than one
     workspace group holds, and on a second call."""
     import torch
-    from friture_b200.correlation import LongGccPhat
+    from friture_b200.correlation import GccPhat
     L = 2400000
     P = group_size(L) + 2
     rng = np.random.default_rng(5)
@@ -104,7 +118,7 @@ def test_same_bits_alone_in_groups_and_again():
     d0 = torch.randn(P, L, device="cuda")
     d1 = torch.randn(P, L, device="cuda")
     d0[0], d1[0], d0[P - 1], d1[P - 1] = a, b, a, b
-    est = LongGccPhat(L)
+    est = GccPhat(L)
     i1, v1, x1 = est.estimate(a[None], b[None], smooth=False, want_xcorr=True)
     iP, vP, xP = est.estimate(d0, d1, smooth=False, want_xcorr=True)
     i2, v2, x2 = est.estimate(a[None], b[None], smooth=False, want_xcorr=True)
@@ -116,7 +130,7 @@ def test_same_bits_alone_in_groups_and_again():
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("L", [55199, 28800])
-def test_silence_and_previous_frame_modes(L):
+def test_long_silence_and_previous_frame_modes(L):
     """Six pairs, rows L+3 floats apart, four calls with silent pairs and have_prev = 0, 2, 2, 1,
     checked after each call against delay_estimator.py:129-142: raw Xcorr, smoothed buffer, index,
     value, and the "no previous frame" marker (NaN in slot 0)."""
@@ -129,7 +143,7 @@ def test_silence_and_previous_frame_modes(L):
              (1, {5: "const"})]
     rng = np.random.default_rng(L + 1)
     h = _lib.Handle(0)
-    h.call("frt_gcc_long_plan", L)
+    h.call("frt_gcc_plan", L)
     d0s = torch.full((P, stride), float("nan"), device="cuda")   # the padding must never be read
     d1s = torch.full((P, stride), float("nan"), device="cuda")
     xc = torch.empty((P, Lp), device="cuda")
@@ -152,7 +166,7 @@ def test_silence_and_previous_frame_modes(L):
         d0s[:, :L] = cuda(a)
         d1s[:, :L] = cuda(b)
         sm_before = sm.clone()
-        h.call("frt_gcc_long_phat", _lib._ptr(d0s), _lib._ptr(d1s), stride, P, _lib._ptr(xc),
+        h.call("frt_gcc_phat", _lib._ptr(d0s), _lib._ptr(d1s), stride, P, _lib._ptr(xc),
                _lib._ptr(sm), have_prev, _lib._ptr(idx), _lib._ptr(val), _lib.current_stream_ptr())
         torch.cuda.synchronize()
         g_xc, g_sm, g_idx, g_val = xc.cpu().numpy(), sm.cpu().numpy(), idx.cpu().numpy(), val.cpu().numpy()
@@ -178,17 +192,17 @@ def test_silence_and_previous_frame_modes(L):
 
 
 @pytest.mark.gpu
-def test_golden_from_reference():
+def test_long_golden_from_reference():
     """tests/golden/gcc_long.npz (oracle/make_golden_gcc_long.py): the unmodified reference's
     generalized_cross_correlation plus the widget's smoothing and peak pick over two frames at
     16800, 55199 (odd) and 240000, kept at every 61st index and around the peak."""
-    from friture_b200.correlation import LongGccPhat
+    from friture_b200.correlation import GccPhat
     from oracle.make_golden_gcc_long import golden_frames
     with np.load(os.path.join(GOLD, "gcc_long.npz")) as g:
         for L in (16800, 55199, 240000):
             (a0, a1), (b0, b1) = golden_frames(L)
             idx = g["index_%d" % L]
-            est = LongGccPhat(L)
+            est = GccPhat(L)
             ia, va, xa = est.estimate(cuda(a0[None]), cuda(a1[None]), smooth=True, want_xcorr=True)
             ib, vb, _ = est.estimate(cuda(b0[None]), cuda(b1[None]), smooth=True)
             assert xa.shape[1] == int(g["n_out_%d" % L])
@@ -200,24 +214,6 @@ def test_golden_from_reference():
             assert [int(ia[0]), int(ib[0])] == list(g["argmax_%d" % L])
             peak = int(np.searchsorted(idx, int(ib[0])))
             assert abs(float(vb[0]) - sm[peak]) <= error_bound(sm, s32[idx])
-
-
-@pytest.mark.gpu
-def test_rejected_lengths_leave_long_plan_usable():
-    import torch
-    from friture_b200._lib import FrtValueError, Handle
-    from friture_b200.correlation import LongGccPhat
-    h = Handle(0)
-    L = 55199
-    d0, d1, _ = length_cases(L)
-    good = LongGccPhat(L, handle=h)
-    _, _, first = good.estimate(cuda(d0), cuda(d1), smooth=False, want_xcorr=True)
-    for bad in (3, 2, 24000001):
-        z = torch.zeros((1, bad), device="cuda")
-        with pytest.raises(FrtValueError):
-            LongGccPhat(bad, handle=h).estimate(z, z + 1.0)
-        _, _, again = good.estimate(cuda(d0), cuda(d1), smooth=False, want_xcorr=True)
-        assert torch.equal(again, first), bad
 
 
 class OddAwarePipelineModel(DelayPipelineModel):
@@ -240,17 +236,17 @@ class OddAwarePipelineModel(DelayPipelineModel):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("delayrange_s, L", [(0.7, 16800), (1.1, 26400), (2.3, 55199), (10.0, 240000)])
-def test_delay_estimator_at_long_ranges(delayrange_s, L):
+def test_delay_estimator_on_long_route(delayrange_s, L):
     """Three pairs: x1 lagging x0, x1 leading x0 (the wrap of delay_estimator.py:150-151), and a
     lag near the edge of the range; chunks of about a sixteenth of a hop, then twice that."""
     import torch
-    from friture_b200.correlation import LongGccPhat
     from friture_b200.delay import DelayEstimator
     fs = 48000
     lags = [4 * round(f * delayrange_s * fs / 4) for f in (0.37, -0.23, 0.85)]
     model = OddAwarePipelineModel(3, delayrange_s)
     est = DelayEstimator(3, delayrange_s=delayrange_s)
-    assert est.length == model.L == L and isinstance(est.gcc, LongGccPhat)
+    assert est.length == model.L == L
+    assert_route(est.gcc, BLUESTEIN_LAUNCHES)
     hop48 = 4 * model.hop
     c1 = 512 * max(1, hop48 // (512 * 16))
     n1 = -(-5 * hop48 // c1)

@@ -13,7 +13,7 @@ T = 8192              # samples per channel
 HOP = 1024            # STFT hop and filterbank block
 N_OCT = 9
 STFT_SIZES = (4096, 2048)   # the second is current when the process calls run
-GCC_LENGTHS = (2400, 4800)  # planned, then re-planned
+GCC_LENGTHS = (2400, 16800)  # planned (shared-memory route), then re-planned and run (Bluestein route)
 GCC_PAIRS = 4
 DEC_STAGES = 2
 
@@ -98,17 +98,20 @@ def _cycle(b, tables3, tables6):
     h.call("frt_bank_process", _ptr(b["x"]), T, HOP, T // HOP, _ptr(b["energies"]), None, 0, 1, st)
     h.call("frt_firbank_process", _ptr(b["x"]), T, HOP, _ptr(b["y"]), b["y"].shape[1], st)
     h.call("frt_firbank_levels", _ptr(b["x"]), T, HOP, T // HOP, _ptr(b["levels"]), 1, st)
-    h.call("frt_gcc_phat", _ptr(b["d0"]), _ptr(b["d1"]), b["d0"].shape[1], GCC_PAIRS, _ptr(b["xcorr"]),
-           None, 0, _ptr(b["idx"]), _ptr(b["val"]), st)
+    gcc_phat = lambda: h.call("frt_gcc_phat", _ptr(b["d0"]), _ptr(b["d1"]), b["d0"].shape[1], GCC_PAIRS,
+                              _ptr(b["xcorr"]), None, 0, _ptr(b["idx"]), _ptr(b["val"]), st)
+    gcc_phat()
     h.call("frt_decimate_process", _ptr(b["x"]), T, T, _ptr(b["dec"]), T >> DEC_STAGES, st)
     torch.cuda.synchronize()
     h.call("frt_stft_process_host", _ptr(b["x_host"]), T, C, T, HOP, _ptr(b["spec_host"]), 1)
     h.call("frt_combined_process_host", _ptr(b["x_host"]), T, C, T, HOP, _ptr(b["comb_spec_host"]),
            _ptr(b["bands_host"]), N_OCT * 3, 1)
-    # re-plan at other sizes: the replaced plans are freed on the way
+    # re-plan at other sizes: the replaced plans are freed on the way; the second GCC length adds
+    # the Bluestein plan and its workspace next to the shared-memory plan
     _bank_plan(h, 6, tables6)
     _fir_plan(h, 6, tables6)
     h.call("frt_gcc_plan", GCC_LENGTHS[1])
+    gcc_phat()
     h.close()
     torch.cuda.synchronize()
 

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Rates of the long GCC-PHAT path (friture_b200/csrc/gcc_long.cu) with CUDA events after warm-up,
-at L = 16800, 26400, 55199, 240000, 2.4e6 and 24e6, and of both paths at L = 24000 on the same
-input.  Prints one JSON line per case plus the card's name and power limit read in the same run.
+"""Rates of GCC-PHAT's Bluestein route (friture_b200/csrc/gcc_long.cu) with CUDA events after
+warm-up, at L = 16800, 26400, 55199, 240000, 2.4e6 and 24e6, lengths GccPhat runs on that route.
+Prints one JSON line per case plus the card's name and power limit read in the same run.
 
 Two byte counts per case, each over 3.35 TB/s (H100 SXM HBM3): the algorithmic bytes (the 2L
 floats of input, plus L' floats of smoothed buffer read and written) and the traffic the passes
@@ -16,7 +16,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 import torch  # noqa: E402
 
-from friture_b200.correlation import GccPhat, LongGccPhat  # noqa: E402
+from friture_b200.correlation import GccPhat  # noqa: E402
 
 HBM = 3.35e12
 
@@ -79,20 +79,13 @@ def main():
         # enough pairs for about 2^28 workspace points (at least 8 column CTAs per SM), at most 4096
         P = max(2, min(4096, (1 << 28) // fft_points(L)))
         d0, d1 = inputs(P, L)
-        ms = time_calls(LongGccPhat(L), d0, d1, args.iters)
+        ms = time_calls(GccPhat(L), d0, d1, args.iters)
         lines.append({"path": "long", "L": L, "pairs": P, "ms_per_call": round(ms, 4),
                       "pairs_per_s": P / ms * 1e3,
                       "algorithmic_share_of_hbm": P * algorithmic(L) / (ms * 1e-3) / HBM,
                       "pass_traffic_share_of_hbm": P * traffic(L) / (ms * 1e-3) / HBM})
         del d0, d1
         torch.cuda.empty_cache()
-    L, P = 24000, 4096
-    d0, d1 = inputs(P, L, seed=1)
-    for name, est in (("shared-memory", GccPhat(L)), ("long", LongGccPhat(L)),
-                      ("shared-memory", GccPhat(L)), ("long", LongGccPhat(L))):
-        ms = time_calls(est, d0, d1, args.iters)
-        lines.append({"path": name, "L": L, "pairs": P, "ms_per_call": round(ms, 4), "pairs_per_s": P / ms * 1e3,
-                      "algorithmic_share_of_hbm": P * algorithmic(L) / (ms * 1e-3) / HBM})
     for ln in lines:
         print(json.dumps(ln))
     if args.out:
