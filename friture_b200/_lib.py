@@ -191,17 +191,23 @@ class Handle:
             pass
 
 
+def device_index(device=None) -> int:
+    """Index of the CUDA device named by None (the current one), an int or a torch.device."""
+    import torch
+    if not torch.cuda.is_available():
+        raise FrtError(FRT_ECUDA, "no CUDA device available; friture_b200 has no CPU fallback")
+    if isinstance(device, torch.device):
+        device = device.index
+    return torch.cuda.current_device() if device is None else int(device)
+
+
 _default_handles = {}
 
 
-def default_handle(device: int | None = None) -> Handle:
+def default_handle(device=None) -> Handle:
     """Process-wide handle per device (the drop-in classes share it, as the reference's widgets
     share one process)."""
-    if device is None:
-        import torch
-        if not torch.cuda.is_available():
-            raise FrtError(FRT_ECUDA, "no CUDA device available; friture_b200 has no CPU fallback")
-        device = torch.cuda.current_device()
+    device = device_index(device)
     h = _default_handles.get(device)
     if h is None:
         h = Handle(device)
@@ -209,6 +215,60 @@ def default_handle(device: int | None = None) -> Handle:
     return h
 
 
+def lazy_handle(make):
+    """A ``handle`` property that sets ``self._handle = make(self)`` on first use, so that an object
+    can be built and configured without a GPU."""
+    def get(self):
+        if self._handle is None:
+            self._handle = make(self)
+        return self._handle
+    return property(get)
+
+
+# the ``handle`` of the classes that share the process-wide handle of the current device
+shared_handle = lazy_handle(lambda self: default_handle())
+
+
 def current_stream_ptr(device=None):
     import torch
     return c_void_p(torch.cuda.current_stream(device).cuda_stream)
+
+
+def stream_ptr(device, stream=None):
+    """The stream a call runs on: the caller's ``stream`` (a CUDA stream handle as an int), else the
+    current torch stream of ``device``."""
+    return current_stream_ptr(device) if stream is None else c_void_p(int(stream))
+
+
+def _row_stride(shape, stride0):
+    # a length-1 axis may carry any stride: the library is told T for a one-row array
+    C, T = shape
+    return int(stride0) if C > 1 else int(T)
+
+
+def check_tensor(owner, x, name):
+    """Raise ValueError unless ``x`` is a CUDA float32 tensor on the GPU of ``owner.handle``.  The
+    handle is looked up last, so that a host array or CPU tensor is rejected without a GPU and
+    without creating a handle."""
+    import torch
+    if not isinstance(x, torch.Tensor) or x.dtype != torch.float32 or not x.is_cuda:
+        raise ValueError("%s must be a CUDA float32 tensor" % name)
+    owner.handle.check_device(x)
+
+
+def device_rows(owner, x, name):
+    """``x`` as [C, T] (a 1-D tensor is one row) and the row stride to pass for it, once it is
+    checked to be a CUDA float32 tensor on the GPU of ``owner.handle``, contiguous along time."""
+    check_tensor(owner, x, name)
+    if x.dim() == 1:
+        x = x[None, :]
+    if x.dim() != 2 or (x.shape[1] > 0 and x.stride(1) != 1):
+        raise ValueError("%s must be [C, T], contiguous along time" % name)
+    return x, _row_stride(x.shape, x.stride(0))
+
+
+def host_rows(x):
+    """Host twin of ``device_rows`` for a float32 NumPy array or CPU tensor [C, T] or [T]."""
+    if x.ndim == 1:
+        x = x[None, :]
+    return x, _row_stride(x.shape, x.stride(0) if hasattr(x, "data_ptr") else x.strides[0] // 4)

@@ -14,8 +14,6 @@ frame chunk on a side stream so that the link time hides behind the filterbank.
 """
 from __future__ import annotations
 
-from ctypes import c_void_p
-
 import numpy as np
 
 from . import _lib
@@ -28,9 +26,7 @@ class ChannelAnalyzer:
     def __init__(self, n_channels, fft_size=2048, hop=1024, bandsperoctave=3, n_octaves=10,
                  response_time=1.0, weighting=None, device=None):
         import torch
-        if device is None:
-            device = torch.cuda.current_device()
-        self.device = torch.device("cuda", int(device))
+        self.device = torch.device("cuda", _lib.device_index(device))
         self.handle = Handle(self.device.index)
         self.n_channels = int(n_channels)
         self.fft_size, self.hop = int(fft_size), int(hop)
@@ -94,17 +90,17 @@ class ChannelAnalyzer:
         return spec, bands
 
     def _bank(self, x, bands):
+        x, x_stride = _lib.device_rows(self, x, "x")
         self.bank._ensure_plan(x.shape[0])
         B = bands.shape[1]
-        self.handle.call("frt_bank_process_strided", _lib._ptr(x), int(x.stride(0)), int(self.hop), int(B),
-                         _lib._ptr(bands), int(bands.stride(0)), 1, _lib.current_stream_ptr(x.device))
+        self.handle.call("frt_bank_process_strided", _lib._ptr(x), x_stride, int(self.hop), int(B),
+                         _lib._ptr(bands), int(bands.stride(0)), 1, _lib.stream_ptr(x.device))
 
     # ------------------------------------------------------------------ host path
     def process_host(self, x_host, spec_host=None, bands_host=None):
         """x_host: CPU float32 tensor / array [C, n_samples] (pinned memory for full PCIe speed).
         Outputs are written into the given CPU tensors (allocated pinned when omitted)."""
         import torch
-        is_torch = hasattr(x_host, "data_ptr")
         C, T = x_host.shape
         F, B = self.frames(T), self.blocks(T)
         if spec_host is None:
@@ -113,8 +109,8 @@ class ChannelAnalyzer:
             bands_host = torch.empty((C, B, self.nbands), dtype=torch.float32, pin_memory=True)
         self.proc._ensure_plan()
         self.bank._ensure_plan(C)
-        stride = int(x_host.stride(0)) if is_torch else int(x_host.strides[0] // 4)
-        self.handle.call("frt_combined_process_host", _lib._ptr(x_host), stride, int(C), int(T),
+        _, x_stride = _lib.host_rows(x_host)
+        self.handle.call("frt_combined_process_host", _lib._ptr(x_host), x_stride, int(C), int(T),
                          int(self.hop), _lib._ptr(spec_host), _lib._ptr(bands_host), int(self.nbands), 1)
         return spec_host, bands_host
 
@@ -148,6 +144,7 @@ class ChannelAnalyzer:
         import torch
         import torch.distributed as dist
         C, T = x.shape
+        _, x_stride = _lib.device_rows(self, x, "x")
         F, B = self.frames(T), self.blocks(T)
         if F % n_chunks:
             raise ValueError("frames (%d) must divide into %d chunks" % (F, n_chunks))
@@ -179,9 +176,9 @@ class ChannelAnalyzer:
             dst = pg.local(i) if pg is not None else spec_chunks[i]
             with torch.cuda.stream(s_stft):
                 xi = x[:, i * fc * self.hop: (i * fc + fc - 1) * self.hop + self.fft_size]
-                self.handle.call("frt_stft_process", _lib._ptr(xi), int(x.stride(0)), int(C), int(fc),
+                self.handle.call("frt_stft_process", _lib._ptr(xi), x_stride, int(C), int(fc),
                                  int(self.hop), _lib._ptr(dst), int(fc * self.nbins),
-                                 int(self.nbins), _lib.STFT_LOGPOWER, _lib.current_stream_ptr(x.device))
+                                 int(self.nbins), _lib.STFT_LOGPOWER, _lib.stream_ptr(x.device))
             if pg is not None:
                 pg.push(i, s_stft)
             else:

@@ -12,12 +12,11 @@ shim returns float64 NumPy like the reference.
 from __future__ import annotations
 
 import logging
-from ctypes import c_void_p
 
 import numpy as np
 
 from . import _lib
-from ._lib import STFT_LOGPOWER, STFT_POWER, default_handle
+from ._lib import STFT_LOGPOWER, STFT_POWER
 from .weighting import abc_weighting
 
 SAMPLING_RATE = 48000      # friture/audiobackend.py:31
@@ -48,11 +47,7 @@ class audioproc():
         self.fft_size = 10
 
     # ------------------------------------------------------------------ plumbing
-    @property
-    def handle(self):
-        if self._handle is None:
-            self._handle = default_handle()
-        return self._handle
+    handle = _lib.shared_handle
 
     def _ensure_plan(self):
         self.handle.call("frt_stft_plan", int(self.fft_size))
@@ -122,12 +117,7 @@ class audioproc():
         ``10*log10(power+1e-30)`` (friture/spectrogram.py:119-125) when ``log``.
         """
         import torch
-        if x.dim() == 1:
-            x = x[None, :]
-        if x.dim() != 2 or x.dtype != torch.float32 or not x.is_cuda:
-            raise ValueError("x must be a CUDA float32 tensor [C, T]")
-        if x.shape[1] > 0 and x.stride(1) != 1:
-            raise ValueError("x must be contiguous along time")
+        x, x_stride = _lib.device_rows(self, x, "x")
         C, T = x.shape
         nf = frame_count(T, self.fft_size, hop)
         nb = self.fft_size // 2 + 1
@@ -137,13 +127,10 @@ class audioproc():
             raise ValueError("out must be a contiguous float32 tensor of shape %s" % ((C, nf, nb),))
         if C == 0 or nf == 0:
             return out
-        self.handle.check_device(x)
         self._ensure_plan()
-        sp = _lib.current_stream_ptr(x.device) if stream is None else c_void_p(int(stream))
-        self.handle.call("frt_stft_process", _lib._ptr(x), int(x.stride(0)) if C > 1 else int(T),
-                         int(C), int(nf),
+        self.handle.call("frt_stft_process", _lib._ptr(x), x_stride, int(C), int(nf),
                          int(hop), _lib._ptr(out), int(nf * nb), int(nb),
-                         STFT_LOGPOWER if log else STFT_POWER, sp)
+                         STFT_LOGPOWER if log else STFT_POWER, _lib.stream_ptr(x.device, stream))
         return out
 
     def stft_host(self, x, hop, log=True, out=None):
@@ -152,8 +139,7 @@ class audioproc():
         is_torch = hasattr(x, "data_ptr")
         if not is_torch:
             x = np.ascontiguousarray(x, dtype=np.float32)
-        if x.ndim == 1:
-            x = x[None, :]
+        x, x_stride = _lib.host_rows(x)
         C, T = x.shape
         nf = frame_count(T, self.fft_size, hop)
         nb = self.fft_size // 2 + 1
@@ -166,10 +152,7 @@ class audioproc():
         if C == 0 or nf == 0:
             return out
         self._ensure_plan()
-        stride = int(x.stride(0)) if is_torch else int(x.strides[0] // 4)
-        if C == 1:
-            stride = T      # a length-1 axis may carry any stride
-        self.handle.call("frt_stft_process_host", _lib._ptr(x), stride, int(C), int(T), int(hop),
+        self.handle.call("frt_stft_process_host", _lib._ptr(x), x_stride, int(C), int(T), int(hop),
                          _lib._ptr(out), STFT_LOGPOWER if log else STFT_POWER)
         return out
 

@@ -3,12 +3,9 @@
 pick of ``Delay_Estimator_Widget.handle_new_data`` (friture/delay_estimator.py:129-152)."""
 from __future__ import annotations
 
-from ctypes import c_void_p
-
 import numpy as np
 
 from . import _lib
-from ._lib import Handle, default_handle
 
 
 def generalized_cross_correlation(d0, d1, handle=None):
@@ -43,11 +40,7 @@ class GccPhat:
         self._smoothed = None
         self._have_prev = False
 
-    @property
-    def handle(self):
-        if self._handle is None:
-            self._handle = default_handle()
-        return self._handle
+    handle = _lib.shared_handle
 
     def reset(self):
         self._smoothed = None
@@ -55,18 +48,13 @@ class GccPhat:
 
     def estimate(self, d0, d1, smooth=True, want_xcorr=False, stream=None):
         import torch
-        if d0.dim() == 1:
-            d0, d1 = d0[None, :], d1[None, :]
-        if (d0.shape != d1.shape or d0.dtype != torch.float32 or d1.dtype != torch.float32
-                or not d0.is_cuda or not d1.is_cuda):
+        d0, _ = _lib.device_rows(self, d0.contiguous(), "d0")
+        d1, _ = _lib.device_rows(self, d1.contiguous(), "d1")
+        if d0.shape != d1.shape:
             raise ValueError("d0, d1 must be CUDA float32 tensors of the same shape [P, L]")
         P, L = d0.shape
         if L != self.length:
             raise ValueError("frame length %d != planned %d" % (L, self.length))
-        self.handle.check_device(d0)
-        self.handle.check_device(d1)
-        d0 = d0.contiguous()
-        d1 = d1.contiguous()
         self.handle.call("frt_gcc_plan", int(L))
         Lo = self.out_length
         idx = torch.empty(P, dtype=torch.int32, device=d0.device)
@@ -82,9 +70,9 @@ class GccPhat:
             # 2 = per pair: a pair whose frames have all been silent so far has no previous smoothed
             # frame (the kernel marks it), like old_Xcorr = None in the widget
             have_prev = 2 if self._have_prev else 0
-        sp = _lib.current_stream_ptr(d0.device) if stream is None else c_void_p(int(stream))
         self.handle.call("frt_gcc_phat", _lib._ptr(d0), _lib._ptr(d1), int(L), int(P),
-                         _lib._ptr(xc), _lib._ptr(sm), have_prev, _lib._ptr(idx), _lib._ptr(val), sp)
+                         _lib._ptr(xc), _lib._ptr(sm), have_prev, _lib._ptr(idx), _lib._ptr(val),
+                         _lib.stream_ptr(d0.device, stream))
         if smooth:
             self._have_prev = True
         return idx, val, xc

@@ -4,8 +4,6 @@ overlap and end-index semantics, GCC-PHAT, temporal smoothing, peak pick, delay 
 confidence."""
 from __future__ import annotations
 
-from ctypes import c_void_p
-
 import numpy as np
 
 from . import _lib, filter_data
@@ -22,9 +20,7 @@ class Decimator:
 
     def __init__(self, n_channels, n_stages=2, device=None):
         import torch
-        if device is None:
-            device = torch.cuda.current_device()
-        self.device = torch.device("cuda", device) if isinstance(device, int) else device
+        self.device = torch.device("cuda", _lib.device_index(device))
         self.n_channels = int(n_channels)
         self.n_stages = int(n_stages)
         self.handle = Handle(self.device.index)
@@ -33,18 +29,17 @@ class Decimator:
 
     def process(self, x, stream=None):
         import torch
-        if x.shape[0] != self.n_channels or x.dtype != torch.float32 or not x.is_cuda:
+        x, x_stride = _lib.device_rows(self, x.contiguous(), "x")
+        C, T = x.shape
+        if C != self.n_channels:
             raise ValueError("x must be a CUDA float32 tensor [%d, T]" % self.n_channels)
-        T = x.shape[1]
         if T == 0:
             return x
         if T % 256 != 0:
             raise ValueError("chunk length must be a multiple of 256")
-        x = x.contiguous()
         out = torch.empty((self.n_channels, T >> self.n_stages), dtype=torch.float32, device=x.device)
-        sp = _lib.current_stream_ptr(x.device) if stream is None else c_void_p(int(stream))
-        self.handle.call("frt_decimate_process", _lib._ptr(x), int(T), int(T), _lib._ptr(out),
-                         int(out.shape[1]), sp)
+        self.handle.call("frt_decimate_process", _lib._ptr(x), x_stride, int(T), _lib._ptr(out),
+                         int(out.shape[1]), _lib.stream_ptr(x.device, stream))
         return out
 
 
@@ -53,9 +48,7 @@ class DelayEstimator:
 
     def __init__(self, n_pairs, delayrange_s=DEFAULT_DELAYRANGE, device=None):
         import torch
-        if device is None:
-            device = torch.cuda.current_device()
-        self.device = torch.device("cuda", device) if isinstance(device, int) else device
+        self.device = torch.device("cuda", _lib.device_index(device))
         self.n_pairs = int(n_pairs)
         self.Ndec = 2                                                    # delay_estimator.py:52
         self.subsampled_sampling_rate = SAMPLING_RATE / 2 ** self.Ndec   # :53

@@ -9,13 +9,12 @@ per-pixel arithmetic runs in one CUDA kernel (``csrc/reduce.cu``)."""
 from __future__ import annotations
 
 import os
-from ctypes import c_float, c_void_p
+from ctypes import c_float
 from fractions import Fraction
 
 import numpy as np
 
 from . import _lib
-from ._lib import default_handle
 from .audioproc import SAMPLING_RATE, audioproc
 
 
@@ -141,11 +140,7 @@ class SpectrogramDisplay:
         self._tables = None
         self._old = None
 
-    @property
-    def handle(self):
-        if self._handle is None:
-            self._handle = default_handle()
-        return self._handle
+    handle = _lib.shared_handle
 
     def set_screen(self, height, width):
         if height != self.height:
@@ -176,8 +171,9 @@ class SpectrogramDisplay:
         import torch
         if db.dim() != 3 or db.shape[0] != self.n_channels or db.shape[2] != len(self.freq):
             raise ValueError("db must be [%d, F, %d]" % (self.n_channels, len(self.freq)))
-        if db.dtype != torch.float32 or not db.is_cuda or not db.is_contiguous():
+        if not db.is_contiguous():
             raise ValueError("db must be a contiguous CUDA float32 tensor")
+        _lib.check_tensor(self, db, "db")
         C, F, nb = db.shape
         self._ensure(db.device)
         cols, a = self.index.push(F)
@@ -188,10 +184,9 @@ class SpectrogramDisplay:
         cols_d = torch.from_numpy(cols).to(db.device) if n_out else None
         a_d = torch.from_numpy(a.astype(np.float32)).to(db.device) if n_out else None
         T = self._tables
-        sp = _lib.current_stream_ptr(db.device) if stream is None else c_void_p(int(stream))
         self.handle.call("frt_display_columns", _lib._ptr(db), int(F * nb), int(nb), int(C), int(F),
                          int(nb), _lib._ptr(T["w"]), c_float(self.spec_min), c_float(self.spec_max),
                          _lib._ptr(T["i0"]), _lib._ptr(T["t"]), int(self.height), _lib._ptr(cols_d),
                          _lib._ptr(a_d), int(n_out), _lib._ptr(self._old), _lib._ptr(T["lut"]),
-                         _lib._ptr(pixels) if n_out else None, sp)
+                         _lib._ptr(pixels) if n_out else None, _lib.stream_ptr(db.device, stream))
         return pixels

@@ -15,7 +15,7 @@ float32 second-order sections), so it matches the IIR bank to ~1e-6 and the live
 """
 from __future__ import annotations
 
-from ctypes import c_int64, c_void_p, byref
+from ctypes import c_int64, byref
 
 import numpy as np
 
@@ -72,7 +72,7 @@ class Octave_Filters():
         self.bdec, self.adec, self._sos_dec = filter_data.decimator()
         self.bdec = np.array(self.bdec)
         self.adec = np.array(self.adec)
-        self._device = device if handle is None else handle.device
+        self._device = device
         self._handle = handle      # share a handle (one GPU context) with other objects, or own one
         self._n_octaves = n_octaves
         self._response_time = response_time
@@ -98,7 +98,7 @@ class Octave_Filters():
         if x.shape[0] == 0:
             raise Exception("Filter input is too small")   # friture/signal/decimate.py:33-34
         import torch
-        dev = self._torch_device()
+        dev = torch.device("cuda", self.handle.device)
         if self._mode == "fft" and x.shape[0] > 4096:
             raise ValueError("fft mode: at most 4096 samples per call (the reference's live path is "
                              "valid up to 1024, friture/filter_design.py:400-401)")
@@ -156,21 +156,7 @@ class Octave_Filters():
         return labels[-len(self.fi):]
 
     # ------------------------------------------------------------------ plumbing
-    def _torch_device(self):
-        import torch
-        if self._device is None:
-            if not torch.cuda.is_available():
-                raise _lib.FrtError(_lib.FRT_ECUDA,
-                                    "no CUDA device available; friture_b200 has no CPU fallback")
-            self._device = torch.cuda.current_device()
-        return torch.device("cuda", int(self._device) if not hasattr(self._device, "index")
-                            else self._device.index)
-
-    @property
-    def handle(self):
-        if self._handle is None:
-            self._handle = Handle(self._torch_device().index)
-        return self._handle
+    handle = _lib.lazy_handle(lambda self: Handle(_lib.device_index(self._device)))
 
     def set_response_time(self, response_time):
         """Smoothing time constant of the fused exponential RMS (octavespectrum.py:140-156);
@@ -196,8 +182,9 @@ class Octave_Filters():
                          int(boct_fir.shape[1]), _lib._ptr(boct_fir), _lib._ptr(bdec_fir))
         self._fir_key = key
 
-    def _filter_batch_fir(self, x, block, stream=None):
-        """Live-path numerics: band outputs of x [C, n_blocks*block], block by block."""
+    def _filter_batch_fir(self, x, x_stride, block, stream=None):
+        """Live-path numerics: band outputs of x [C, n_blocks*block] (row stride ``x_stride``),
+        block by block."""
         import torch
         C, T = x.shape
         if block > 4096 or block % (1 << (self._n_octaves - 1)):
@@ -206,12 +193,12 @@ class Octave_Filters():
         self._ensure_fir_plan(C)
         offsets, lengths = ragged_layout(block, self.bandsperoctave, self._n_octaves)
         ystride = int(offsets[-1] + lengths[-1])
-        sp = _lib.current_stream_ptr(x.device) if stream is None else c_void_p(int(stream))
+        sp = _lib.stream_ptr(x.device, stream)
         parts = []
         for b in range(T // block):
             ybuf = torch.empty((C, ystride), dtype=torch.float32, device=x.device)
             xb = x[:, b * block:(b + 1) * block]
-            self.handle.call("frt_firbank_process", _lib._ptr(xb), int(x.stride(0)) if C > 1 else int(T),
+            self.handle.call("frt_firbank_process", _lib._ptr(xb), x_stride,
                              int(block), _lib._ptr(ybuf), ystride, sp)
             parts.append(ybuf)
         return [torch.cat([p[:, int(o):int(o) + int(n)] for p in parts], dim=1)
@@ -257,15 +244,10 @@ class Octave_Filters():
            in dB (10*log10(e+1e-30), octavespectrum.py:119-120) when ``db``.
         Filter and smoothing state carry over from call to call."""
         import torch
-        if x.dim() == 1:
-            x = x[None, :]
-        if x.dim() != 2 or x.dtype != torch.float32 or not x.is_cuda:
-            raise ValueError("x must be a CUDA float32 tensor [C, T]")
+        x, x_stride = _lib.device_rows(self, x, "x")
         C, T = x.shape
         if T == 0 or C == 0:
             raise Exception("Filter input is too small")
-        if x.stride(1) != 1:
-            raise ValueError("x must be contiguous along time")
         if block <= 0 or T % block != 0:
             raise ValueError("T must be a whole number of blocks")
         if block % 256 != 0 or (block >> (self._n_octaves - 1)) < 1:
@@ -274,12 +256,11 @@ class Octave_Filters():
         if energies and block > MAX_BLOCK:
             raise ValueError("block > %d: the reference's smoothing kernel is shorter than the "
                              "block (exp_smoothing.py:43-47)" % MAX_BLOCK)
-        self.handle.check_device(x)
         n_blocks = T // block
         if self._mode == "fft":
             if energies:
                 raise ValueError("fft mode gives the band outputs only (energies=False, want_y=True)")
-            return self._filter_batch_fir(x, block, stream), None
+            return self._filter_batch_fir(x, x_stride, block, stream), None
         self._ensure_plan(C)
         e = None
         if energies:
@@ -290,11 +271,9 @@ class Octave_Filters():
             offsets, lengths = ragged_layout(T, self.bandsperoctave, self._n_octaves)
             ystride = int(offsets[-1] + lengths[-1])
             ybuf = torch.empty((C, ystride), dtype=torch.float32, device=x.device)
-        sp = _lib.current_stream_ptr(x.device) if stream is None else c_void_p(int(stream))
-        self.handle.call("frt_bank_process", _lib._ptr(x), int(x.stride(0)) if C > 1 else int(T),
-                         int(block),
+        self.handle.call("frt_bank_process", _lib._ptr(x), x_stride, int(block),
                          int(n_blocks), _lib._ptr(e), _lib._ptr(ybuf), ystride,
-                         1 if db else 0, sp)
+                         1 if db else 0, _lib.stream_ptr(x.device, stream))
         y = None
         if want_y:
             y = [ybuf[:, int(o):int(o) + int(n)] for o, n in zip(offsets, lengths)]

@@ -6,8 +6,6 @@ of the call's blocks and writes one level vector per channel and block; the band
 leave the chip."""
 from __future__ import annotations
 
-from ctypes import c_void_p
-
 import numpy as np
 
 from . import _lib
@@ -86,12 +84,7 @@ class OctaveSpectrumAnalyzer:
         CUDA float32 tensor [C, n_blocks, nbands]: the widget's output after each block, in dB
         with the weighting when ``db``, else the smoothed linear band energies."""
         import torch
-        if not isinstance(x, torch.Tensor):
-            raise ValueError("x must be a torch tensor")
-        if x.dim() == 1:
-            x = x[None, :]
-        if x.dim() != 2 or x.dtype != torch.float32:
-            raise ValueError("x must be a float32 tensor [C, T]")
+        x, x_stride = _lib.device_rows(self.filters, x, "x")
         C, T = x.shape
         if C != self.n_channels:
             raise ValueError("expected %d channels, got %d" % (self.n_channels, C))
@@ -101,16 +94,11 @@ class OctaveSpectrumAnalyzer:
                              "keeps its even samples, friture/signal/decimate.py:41)" % (step, MAX_BLOCK))
         if T == 0 or T % block:
             raise ValueError("T must be a whole, non-zero number of blocks")
-        if x.stride(1) != 1 or (C > 1 and x.stride(0) < T):
-            raise ValueError("x must be contiguous along time, rows not overlapping")
-        if not x.is_cuda:
-            raise ValueError("x must be a CUDA tensor")
-        h = self.filters.handle
-        h.check_device(x)
+        if x_stride < T:
+            raise ValueError("x rows must not overlap")
         self._ensure_plan()
         n_blocks = T // block
         out = torch.empty((C, n_blocks, self.nbands), dtype=torch.float32, device=x.device)
-        sp = _lib.current_stream_ptr(x.device) if stream is None else c_void_p(int(stream))
-        h.call("frt_firbank_levels", _lib._ptr(x), int(x.stride(0)) if C > 1 else int(T), int(block),
-               int(n_blocks), _lib._ptr(out), 1 if db else 0, sp)
+        self.filters.handle.call("frt_firbank_levels", _lib._ptr(x), x_stride, int(block), int(n_blocks),
+                                 _lib._ptr(out), 1 if db else 0, _lib.stream_ptr(x.device, stream))
         return out

@@ -20,7 +20,6 @@ from functools import cached_property
 import numpy as np
 
 from . import _lib
-from ._lib import default_handle
 from .audioproc import SAMPLING_RATE
 from .display import Linear, Logarithmic, Mel
 
@@ -122,11 +121,7 @@ class _PlotState:
         self._last = None
         self.setspecrange(spec_min, spec_max)
 
-    @property
-    def handle(self):
-        if self._handle is None:
-            self._handle = default_handle()
-        return self._handle
+    handle = _lib.shared_handle
 
     def setspecrange(self, spec_min, spec_max):
         """New vertical range from the next call on; the peak state is kept."""
@@ -143,15 +138,15 @@ class _PlotState:
     def _run(self, y, peaks):
         """y: CUDA float32 [C, n_steps, K], contiguous along K.  Returns (y, z, peak, z_peak)."""
         import torch
-        if not isinstance(y, torch.Tensor) or y.dim() != 3 or y.dtype != torch.float32 or not y.is_cuda:
+        if not isinstance(y, torch.Tensor) or y.dim() != 3:
             raise ValueError("dB must be a CUDA float32 tensor [C, n_steps, K]")
         C, S, K = y.shape
         if C != self.n_channels or S == 0 or K == 0:
             raise ValueError("expected [%d, n_steps >= 1, K >= 1] dB, got %s" % (self.n_channels, tuple(y.shape)))
+        _lib.check_tensor(self, y, "dB")
         if K > 1 and y.stride(2) != 1:
             y = y.contiguous()
         h = self.handle
-        h.check_device(y)
         dev = y.device
         out = [torch.empty((C, K), dtype=torch.float32, device=dev) for _ in range(4 if peaks else 2)]
         state = (self.peak, self.peak_int, self.peak_decay)
@@ -161,7 +156,7 @@ class _PlotState:
             # new size that the next call would read without the reset
             state = tuple(torch.empty((C, K), dtype=torch.float64, device=dev) for _ in range(3))
         st = [_lib._ptr(t) if peaks else None for t in state]
-        sp = _lib.current_stream_ptr(dev)
+        sp = _lib.stream_ptr(dev)
         h.call("frt_plot_curves", _lib._ptr(y), int(y.stride(0)), int(y.stride(1)), int(C), int(S),
                int(K), c_double(self.spec_min), c_double(self.spec_max), c_double(PEAK_DECAY),
                1 if peaks else 0, 1 if reset else 0, *st, *[_lib._ptr(t) for t in out],

@@ -9,7 +9,7 @@ each channel is a (reference, measurement) pair and the output is the transfer f
 the two."""
 from __future__ import annotations
 
-from ctypes import c_float, c_void_p
+from ctypes import c_float
 
 import numpy as np
 
@@ -96,11 +96,10 @@ class SpectrumAnalyzer:
         db = torch.empty((C, nb), dtype=torch.float32, device=x.device)
         imax = torch.empty(C, dtype=torch.int32, device=x.device)
         ipitch = torch.empty(C, dtype=torch.int32, device=x.device)
-        sp = _lib.current_stream_ptr(x.device) if stream is None else c_void_p(int(stream))
         self.proc.handle.call("frt_spectrum_reduce", _lib._ptr(power), int(nf * nb), int(nb), int(C),
                               int(nf), int(nb), c_float(self.alpha), _lib._ptr(self._disp),
                               _lib._ptr(self._w_dev) if self.weighting else None, _lib._ptr(db),
-                              _lib._ptr(imax), _lib._ptr(ipitch), sp)
+                              _lib._ptr(imax), _lib._ptr(ipitch), _lib.stream_ptr(x.device, stream))
         if self._disp2 is not None and nf > 0:
             # the widget smooths an all-zero second column on every tick it does not fill
             # (spectrum.py:142,158-159): dispbuffers2 * (1-alpha)^frames, on the kernel's stream
@@ -129,12 +128,12 @@ class SpectrumAnalyzer:
         db = torch.empty((C, nb), dtype=torch.float32, device=x.device)
         imax = torch.empty(C, dtype=torch.int32, device=x.device)
         ipitch = torch.empty(C, dtype=torch.int32, device=x.device)
-        sp = _lib.current_stream_ptr(x.device) if stream is None else c_void_p(int(stream))
         # power [2C, nf, nb]: pair c's reference at row 2c, its measurement at row 2c + 1
         p1 = power.data_ptr() if nf else 0
         p2 = p1 + 4 * nf * nb if nf else 0
         self.proc.handle.call("frt_spectrum_reduce_dual", _lib._ptr(p1), _lib._ptr(p2),
                               int(2 * nf * nb), int(nb), int(C), int(nf), int(nb),
                               c_float(self.alpha), _lib._ptr(self._disp), _lib._ptr(self._disp2),
-                              _lib._ptr(db), _lib._ptr(imax), _lib._ptr(ipitch), sp)
+                              _lib._ptr(db), _lib._ptr(imax), _lib._ptr(ipitch),
+                              _lib.stream_ptr(x.device, stream))
         return self._indices_to_hz(db, imax, ipitch)

@@ -61,6 +61,38 @@ def test_combined_device_and_host_paths_match_oracle():
     assert rel_err(torch.cat([b_a, b_b], 1).cpu().numpy(), ref_bands) < TOL
 
 
+def one_row(T=9 * 1024):
+    return (np.random.default_rng(5).standard_normal(T) * 0.1).astype(np.float32)
+
+
+def test_one_row_view_with_unit_row_stride():
+    """A one-row view may carry any stride along its length-1 axis: torch.empty(T, 1).t() has
+    strides (1, 1).  Both halves of the analysis give the bits of the same row laid out as usual,
+    each from a fresh analyzer."""
+    import torch
+    from friture_b200.analyzer import ChannelAnalyzer
+    x = one_row()
+    view = torch.from_numpy(x).cuda()[:, None].t()
+    row = torch.from_numpy(x)[None, :].cuda()
+    assert view.stride() == (1, 1) and row.stride() == (len(x), 1)
+    spec, bands = ChannelAnalyzer(1).process(view)
+    ref_spec, ref_bands = ChannelAnalyzer(1).process(row)
+    assert torch.equal(spec, ref_spec) and torch.equal(bands, ref_bands)
+
+
+def test_one_row_host_view_with_any_row_stride():
+    """The host path on np.empty((T, 1)).T, whose strides are (4, 4)."""
+    import torch
+    from friture_b200.analyzer import ChannelAnalyzer
+    x = one_row()
+    col = np.empty((len(x), 1), np.float32)
+    col[:, 0] = x
+    assert col.T.strides == (4, 4)
+    spec, bands = ChannelAnalyzer(1).process_host(col.T)
+    ref_spec, ref_bands = ChannelAnalyzer(1).process_host(x[None, :])
+    assert torch.equal(spec, ref_spec) and torch.equal(bands, ref_bands)
+
+
 def test_combined_long_host_stream_and_weighting():
     import torch
     from friture_b200.analyzer import ChannelAnalyzer
