@@ -1,6 +1,7 @@
 """ctypes binding of ``libfrt_b200.so`` (the C ABI declared in ``include/frt.h``)."""
 from __future__ import annotations
 
+import contextlib
 import ctypes
 import os
 import threading
@@ -234,10 +235,19 @@ def current_stream_ptr(device=None):
     return c_void_p(torch.cuda.current_stream(device).cuda_stream)
 
 
-def stream_ptr(device, stream=None):
+@contextlib.contextmanager
+def call_stream(device, stream=None):
     """The stream a call runs on: the caller's ``stream`` (a CUDA stream handle as an int), else the
-    current torch stream of ``device``."""
-    return current_stream_ptr(device) if stream is None else c_void_p(int(stream))
+    current torch stream of ``device``.  It is the current stream for the body, so that the
+    wrapper's own torch work -- allocations, fills, uploads, copies and host reads -- is ordered
+    with the library's kernels on it, and the temporaries it frees go back to that stream's pool.
+    Yields the handle to pass to the library."""
+    if stream is None:
+        yield current_stream_ptr(device)
+        return
+    import torch
+    with torch.cuda.stream(torch.cuda.ExternalStream(int(stream), device=device)):
+        yield c_void_p(int(stream))
 
 
 def _row_stride(shape, stride0):

@@ -93,8 +93,9 @@ class ChannelAnalyzer:
         x, x_stride = _lib.device_rows(self, x, "x")
         self.bank._ensure_plan(x.shape[0])
         B = bands.shape[1]
-        self.handle.call("frt_bank_process_strided", _lib._ptr(x), x_stride, int(self.hop), int(B),
-                         _lib._ptr(bands), int(bands.stride(0)), 1, _lib.stream_ptr(x.device))
+        with _lib.call_stream(x.device) as sp:
+            self.handle.call("frt_bank_process_strided", _lib._ptr(x), x_stride, int(self.hop), int(B),
+                             _lib._ptr(bands), int(bands.stride(0)), 1, sp)
 
     # ------------------------------------------------------------------ host path
     def process_host(self, x_host, spec_host=None, bands_host=None):
@@ -174,11 +175,11 @@ class ChannelAnalyzer:
             raise ValueError("transport must be 'peer' or 'nccl'")
         for i in range(n_chunks):
             dst = pg.local(i) if pg is not None else spec_chunks[i]
-            with torch.cuda.stream(s_stft):
+            with torch.cuda.stream(s_stft), _lib.call_stream(x.device) as sp:
                 xi = x[:, i * fc * self.hop: (i * fc + fc - 1) * self.hop + self.fft_size]
                 self.handle.call("frt_stft_process", _lib._ptr(xi), x_stride, int(C), int(fc),
                                  int(self.hop), _lib._ptr(dst), int(fc * self.nbins),
-                                 int(self.nbins), _lib.STFT_LOGPOWER, _lib.stream_ptr(x.device))
+                                 int(self.nbins), _lib.STFT_LOGPOWER, sp)
             if pg is not None:
                 pg.push(i, s_stft)
             else:

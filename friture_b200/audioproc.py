@@ -121,16 +121,18 @@ class audioproc():
         C, T = x.shape
         nf = frame_count(T, self.fft_size, hop)
         nb = self.fft_size // 2 + 1
-        if out is None:
-            out = torch.empty((C, nf, nb), dtype=torch.float32, device=x.device)
-        elif tuple(out.shape) != (C, nf, nb) or out.dtype != torch.float32 or not out.is_contiguous():
+        if out is not None and (tuple(out.shape) != (C, nf, nb) or out.dtype != torch.float32
+                                or not out.is_contiguous()):
             raise ValueError("out must be a contiguous float32 tensor of shape %s" % ((C, nf, nb),))
-        if C == 0 or nf == 0:
-            return out
-        self._ensure_plan()
-        self.handle.call("frt_stft_process", _lib._ptr(x), x_stride, int(C), int(nf),
-                         int(hop), _lib._ptr(out), int(nf * nb), int(nb),
-                         STFT_LOGPOWER if log else STFT_POWER, _lib.stream_ptr(x.device, stream))
+        with _lib.call_stream(x.device, stream) as sp:
+            if out is None:
+                out = torch.empty((C, nf, nb), dtype=torch.float32, device=x.device)
+            if C == 0 or nf == 0:
+                return out
+            self._ensure_plan()
+            self.handle.call("frt_stft_process", _lib._ptr(x), x_stride, int(C), int(nf),
+                             int(hop), _lib._ptr(out), int(nf * nb), int(nb),
+                             STFT_LOGPOWER if log else STFT_POWER, sp)
         return out
 
     def stft_host(self, x, hop, log=True, out=None):

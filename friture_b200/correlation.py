@@ -48,31 +48,32 @@ class GccPhat:
 
     def estimate(self, d0, d1, smooth=True, want_xcorr=False, stream=None):
         import torch
-        d0, _ = _lib.device_rows(self, d0.contiguous(), "d0")
-        d1, _ = _lib.device_rows(self, d1.contiguous(), "d1")
-        if d0.shape != d1.shape:
-            raise ValueError("d0, d1 must be CUDA float32 tensors of the same shape [P, L]")
-        P, L = d0.shape
-        if L != self.length:
-            raise ValueError("frame length %d != planned %d" % (L, self.length))
-        self.handle.call("frt_gcc_plan", int(L))
-        Lo = self.out_length
-        idx = torch.empty(P, dtype=torch.int32, device=d0.device)
-        val = torch.empty(P, dtype=torch.float32, device=d0.device)
-        xc = torch.empty((P, Lo), dtype=torch.float32, device=d0.device) if want_xcorr else None
-        sm = None
-        have_prev = 0
-        if smooth:
-            if self._smoothed is None or tuple(self._smoothed.shape) != (P, Lo):
-                self._smoothed = torch.zeros((P, Lo), dtype=torch.float32, device=d0.device)
-                self._have_prev = False
-            sm = self._smoothed
-            # 2 = per pair: a pair whose frames have all been silent so far has no previous smoothed
-            # frame (the kernel marks it), like old_Xcorr = None in the widget
-            have_prev = 2 if self._have_prev else 0
-        self.handle.call("frt_gcc_phat", _lib._ptr(d0), _lib._ptr(d1), int(L), int(P),
-                         _lib._ptr(xc), _lib._ptr(sm), have_prev, _lib._ptr(idx), _lib._ptr(val),
-                         _lib.stream_ptr(d0.device, stream))
+        _lib.check_tensor(self, d0, "d0")
+        with _lib.call_stream(d0.device, stream) as sp:
+            d0, _ = _lib.device_rows(self, d0.contiguous(), "d0")
+            d1, _ = _lib.device_rows(self, d1.contiguous(), "d1")
+            if d0.shape != d1.shape:
+                raise ValueError("d0, d1 must be CUDA float32 tensors of the same shape [P, L]")
+            P, L = d0.shape
+            if L != self.length:
+                raise ValueError("frame length %d != planned %d" % (L, self.length))
+            self.handle.call("frt_gcc_plan", int(L))
+            Lo = self.out_length
+            idx = torch.empty(P, dtype=torch.int32, device=d0.device)
+            val = torch.empty(P, dtype=torch.float32, device=d0.device)
+            xc = torch.empty((P, Lo), dtype=torch.float32, device=d0.device) if want_xcorr else None
+            sm = None
+            have_prev = 0
+            if smooth:
+                if self._smoothed is None or tuple(self._smoothed.shape) != (P, Lo):
+                    self._smoothed = torch.zeros((P, Lo), dtype=torch.float32, device=d0.device)
+                    self._have_prev = False
+                sm = self._smoothed
+                # 2 = per pair: a pair whose frames have all been silent so far has no previous smoothed
+                # frame (the kernel marks it), like old_Xcorr = None in the widget
+                have_prev = 2 if self._have_prev else 0
+            self.handle.call("frt_gcc_phat", _lib._ptr(d0), _lib._ptr(d1), int(L), int(P),
+                             _lib._ptr(xc), _lib._ptr(sm), have_prev, _lib._ptr(idx), _lib._ptr(val), sp)
         if smooth:
             self._have_prev = True
         return idx, val, xc

@@ -595,10 +595,8 @@ extern "C" int frt_bank_plan(frt_handle h, int n_channels, int bands_per_octave,
     pl->ne = (size_t)n_octaves * bands_per_octave;
     FRT_CUDA(h, pl->zstate.alloc(pl->nz * n_channels));
     FRT_CUDA(h, pl->ema.alloc(pl->ne * n_channels));
-    FRT_CUDA(h, cudaMemset(pl->zstate.get(), 0, sizeof(float) * pl->nz * n_channels));
-    FRT_CUDA(h, cudaMemset(pl->ema.get(), 0, sizeof(float) * pl->ne * n_channels));
-    // the memsets run on the legacy stream; callers process on their own (possibly non-blocking) streams
-    FRT_CUDA(h, cudaDeviceSynchronize());
+    FRT_CUDA(h, frt_sync_zero(pl->zstate.get(), sizeof(float) * pl->nz * n_channels));
+    FRT_CUDA(h, frt_sync_zero(pl->ema.get(), sizeof(float) * pl->ne * n_channels));
     h->bank = std::move(pl);
     return FRT_OK;
 }
@@ -608,9 +606,8 @@ extern "C" int frt_bank_reset(frt_handle h) {
     if (!h->bank) return frt_fail(h, FRT_ESTATE, "frt_bank_reset: no plan");
     DeviceGuard g(h->device);
     BankPlan *pl = h->bank.get();
-    FRT_CUDA(h, cudaMemset(pl->zstate.get(), 0, sizeof(float) * pl->nz * pl->n_channels));
-    FRT_CUDA(h, cudaMemset(pl->ema.get(), 0, sizeof(float) * pl->ne * pl->n_channels));
-    FRT_CUDA(h, cudaDeviceSynchronize());
+    FRT_CUDA(h, frt_sync_zero(pl->zstate.get(), sizeof(float) * pl->nz * pl->n_channels));
+    FRT_CUDA(h, frt_sync_zero(pl->ema.get(), sizeof(float) * pl->ne * pl->n_channels));
     return FRT_OK;
 }
 
@@ -626,7 +623,7 @@ extern "C" int frt_bank_set_weighting(frt_handle h, const float *weight_db_host)
         return FRT_OK;
     }
     if (!pl->weight.get()) FRT_CUDA(h, pl->weight.alloc(nb));
-    FRT_CUDA(h, cudaMemcpy(pl->weight.get(), weight_db_host, sizeof(float) * nb, cudaMemcpyHostToDevice));
+    FRT_CUDA(h, frt_sync_copy(pl->weight.get(), weight_db_host, sizeof(float) * nb, cudaMemcpyHostToDevice));
     return FRT_OK;
 }
 
@@ -654,13 +651,12 @@ extern "C" int frt_bank_get_state(frt_handle h, float *z_host, float *ema_host) 
     if (!h->bank) return frt_fail(h, FRT_ESTATE, "frt_bank_get_state: no plan");
     DeviceGuard g(h->device);
     BankPlan *pl = h->bank.get();
-    FRT_CUDA(h, cudaDeviceSynchronize());
     if (z_host)
-        FRT_CUDA(h, cudaMemcpy(z_host, pl->zstate.get(), sizeof(float) * pl->nz * pl->n_channels,
-                               cudaMemcpyDeviceToHost));
+        FRT_CUDA(h, frt_sync_copy(z_host, pl->zstate.get(), sizeof(float) * pl->nz * pl->n_channels,
+                                  cudaMemcpyDeviceToHost));
     if (ema_host)
-        FRT_CUDA(h, cudaMemcpy(ema_host, pl->ema.get(), sizeof(float) * pl->ne * pl->n_channels,
-                               cudaMemcpyDeviceToHost));
+        FRT_CUDA(h, frt_sync_copy(ema_host, pl->ema.get(), sizeof(float) * pl->ne * pl->n_channels,
+                                  cudaMemcpyDeviceToHost));
     return FRT_OK;
 }
 
@@ -669,13 +665,12 @@ extern "C" int frt_bank_set_state(frt_handle h, const float *z_host, const float
     if (!h->bank) return frt_fail(h, FRT_ESTATE, "frt_bank_set_state: no plan");
     DeviceGuard g(h->device);
     BankPlan *pl = h->bank.get();
-    FRT_CUDA(h, cudaDeviceSynchronize());
     if (z_host)
-        FRT_CUDA(h, cudaMemcpy(pl->zstate.get(), z_host, sizeof(float) * pl->nz * pl->n_channels,
-                               cudaMemcpyHostToDevice));
+        FRT_CUDA(h, frt_sync_copy(pl->zstate.get(), z_host, sizeof(float) * pl->nz * pl->n_channels,
+                                  cudaMemcpyHostToDevice));
     if (ema_host)
-        FRT_CUDA(h, cudaMemcpy(pl->ema.get(), ema_host, sizeof(float) * pl->ne * pl->n_channels,
-                               cudaMemcpyHostToDevice));
+        FRT_CUDA(h, frt_sync_copy(pl->ema.get(), ema_host, sizeof(float) * pl->ne * pl->n_channels,
+                                  cudaMemcpyHostToDevice));
     return FRT_OK;
 }
 
@@ -830,8 +825,7 @@ extern "C" int frt_decimate_plan(frt_handle h, int n_channels, int n_stages, con
     pl->n_stages = n_stages;
     const size_t nz = (size_t)n_stages * 6 * 2 * n_channels;
     FRT_CUDA(h, pl->zstate.alloc(nz));
-    FRT_CUDA(h, cudaMemset(pl->zstate.get(), 0, sizeof(float) * nz));
-    FRT_CUDA(h, cudaDeviceSynchronize());
+    FRT_CUDA(h, frt_sync_zero(pl->zstate.get(), sizeof(float) * nz));
     h->dec = std::move(pl);
     return FRT_OK;
 }

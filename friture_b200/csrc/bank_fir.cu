@@ -291,13 +291,12 @@ extern "C" int frt_firbank_plan(frt_handle h, int n_channels, int bands_per_octa
     FRT_CUDA(h, pl->alpha.alloc(n_octaves));
     FRT_CUDA(h, pl->decay.alloc((size_t)n_octaves * FIR_DECAY_STRIDE));
     FRT_CUDA(h, pl->weight_db.alloc(nb));
-    FRT_CUDA(h, cudaMemcpy(pl->taps.get(), fir_band, sizeof(double) * (size_t)bands_per_octave * n_taps,
-                           cudaMemcpyHostToDevice));
-    FRT_CUDA(h, cudaMemcpy(pl->taps.get() + (size_t)bands_per_octave * n_taps, fir_dec, sizeof(double) * n_taps,
-                           cudaMemcpyHostToDevice));
-    FRT_CUDA(h, cudaMemset(pl->hist.get(), 0, sizeof(float) * nh));
-    FRT_CUDA(h, cudaMemset(pl->sp.get(), 0, sizeof(double) * n_channels * nb));
-    FRT_CUDA(h, cudaDeviceSynchronize());
+    FRT_CUDA(h, frt_sync_copy(pl->taps.get(), fir_band, sizeof(double) * (size_t)bands_per_octave * n_taps,
+                              cudaMemcpyHostToDevice));
+    FRT_CUDA(h, frt_sync_copy(pl->taps.get() + (size_t)bands_per_octave * n_taps, fir_dec, sizeof(double) * n_taps,
+                              cudaMemcpyHostToDevice));
+    FRT_CUDA(h, frt_sync_zero(pl->hist.get(), sizeof(float) * nh));
+    FRT_CUDA(h, frt_sync_zero(pl->sp.get(), sizeof(double) * n_channels * nb));
     h->fir = std::move(pl);
     return FRT_OK;
 }
@@ -307,9 +306,8 @@ extern "C" int frt_firbank_reset(frt_handle h) {
     FirPlan *pl = h->fir.get();
     if (!pl) return frt_fail(h, FRT_ESTATE, "frt_firbank_reset: no plan");
     DeviceGuard g(h->device);
-    FRT_CUDA(h, cudaMemset(pl->hist.get(), 0, sizeof(float) * (size_t)pl->n_channels * pl->n_oct * (pl->L - 1)));
-    FRT_CUDA(h, cudaMemset(pl->sp.get(), 0, sizeof(double) * (size_t)pl->n_channels * pl->n_oct * pl->bpo));
-    FRT_CUDA(h, cudaDeviceSynchronize());
+    FRT_CUDA(h, frt_sync_zero(pl->hist.get(), sizeof(float) * (size_t)pl->n_channels * pl->n_oct * (pl->L - 1)));
+    FRT_CUDA(h, frt_sync_zero(pl->sp.get(), sizeof(double) * (size_t)pl->n_channels * pl->n_oct * pl->bpo));
     return FRT_OK;
 }
 
@@ -325,11 +323,11 @@ extern "C" int frt_firbank_set_smoothing(frt_handle h, const double *alphas, con
     for (int j = 0; j < pl->n_oct; j++)
         for (int m = 0; m < FIR_DECAY_STRIDE; m++)
             decay[(size_t)j * FIR_DECAY_STRIDE + m] = std::pow(1.0 - alphas[j], (double)m);
-    FRT_CUDA(h, cudaMemcpy(pl->alpha.get(), alphas, sizeof(double) * pl->n_oct, cudaMemcpyHostToDevice));
-    FRT_CUDA(h, cudaMemcpy(pl->decay.get(), decay.data(), sizeof(double) * decay.size(), cudaMemcpyHostToDevice));
+    FRT_CUDA(h, frt_sync_copy(pl->alpha.get(), alphas, sizeof(double) * pl->n_oct, cudaMemcpyHostToDevice));
+    FRT_CUDA(h, frt_sync_copy(pl->decay.get(), decay.data(), sizeof(double) * decay.size(), cudaMemcpyHostToDevice));
     if (weight_db)
-        FRT_CUDA(h, cudaMemcpy(pl->weight_db.get(), weight_db, sizeof(float) * (size_t)pl->n_oct * pl->bpo,
-                               cudaMemcpyHostToDevice));
+        FRT_CUDA(h, frt_sync_copy(pl->weight_db.get(), weight_db, sizeof(float) * (size_t)pl->n_oct * pl->bpo,
+                                  cudaMemcpyHostToDevice));
     pl->weighted = weight_db != nullptr;
     pl->smoothing = true;
     return FRT_OK;

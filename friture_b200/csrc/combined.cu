@@ -23,6 +23,9 @@ extern "C" int frt_combined_process_host(frt_handle h, const float *x_host, int6
     const int64_t B = n_samples / hop;                                   // filterbank blocks
     const int64_t F = n_samples >= N ? (n_samples - N) / hop + 1 : 0;    // spectrogram columns
     if (B == 0) return FRT_OK;
+    // the staging streams are non-blocking and wait for nothing: a device call on this handle that is
+    // still queued on any stream (it reads and writes the filterbank state) must finish first
+    FRT_CUDA(h, cudaDeviceSynchronize());
     CombStaging &p = h->comb_host;
     FRT_CUDA(h, p.create());
     FRT_CUDA(h, p.d_x.grow((size_t)n_channels * n_samples));

@@ -25,6 +25,25 @@ struct EventDestroy {
     void operator()(cudaEvent_t e) const { cudaEventDestroy(e); }
 };
 
+// Every host-side write to or read of device memory that is not ordered on a caller's stream (plans,
+// setters, resets, state checkpoints) goes through these two.  A kernel of this handle may still be
+// queued on any stream, blocking or not, and must run with what it saw when it was queued, so the
+// device is drained first.  The device is drained again afterwards: a pageable host-to-device
+// cudaMemcpy may return before the data has landed, and a kernel launched next on a non-blocking
+// stream would not wait for it.
+inline cudaError_t frt_sync_copy(void *dst, const void *src, size_t bytes, cudaMemcpyKind kind) {
+    cudaError_t e = cudaDeviceSynchronize();
+    if (e == cudaSuccess) e = cudaMemcpy(dst, src, bytes, kind);
+    if (e == cudaSuccess) e = cudaDeviceSynchronize();
+    return e;
+}
+inline cudaError_t frt_sync_zero(void *dst, size_t bytes) {
+    cudaError_t e = cudaDeviceSynchronize();
+    if (e == cudaSuccess) e = cudaMemset(dst, 0, bytes);
+    if (e == cudaSuccess) e = cudaDeviceSynchronize();
+    return e;
+}
+
 // One cudaMalloc allocation of n elements of T, or none.  Move-only.
 template <class T>
 struct DeviceArray {
@@ -45,7 +64,7 @@ struct DeviceArray {
     cudaError_t upload(const std::vector<T> &host) {
         cudaError_t e = alloc(host.size());
         if (e != cudaSuccess) return e;
-        return cudaMemcpy(get(), host.data(), sizeof(T) * host.size(), cudaMemcpyHostToDevice);
+        return frt_sync_copy(get(), host.data(), sizeof(T) * host.size(), cudaMemcpyHostToDevice);
     }
     // staging: reallocates only when a call needs more than it holds, so steady-state calls do not
     cudaError_t grow(size_t count) { return count <= n ? cudaSuccess : alloc(count); }

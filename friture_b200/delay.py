@@ -29,17 +29,19 @@ class Decimator:
 
     def process(self, x, stream=None):
         import torch
-        x, x_stride = _lib.device_rows(self, x.contiguous(), "x")
-        C, T = x.shape
-        if C != self.n_channels:
-            raise ValueError("x must be a CUDA float32 tensor [%d, T]" % self.n_channels)
-        if T == 0:
-            return x
-        if T % 256 != 0:
-            raise ValueError("chunk length must be a multiple of 256")
-        out = torch.empty((self.n_channels, T >> self.n_stages), dtype=torch.float32, device=x.device)
-        self.handle.call("frt_decimate_process", _lib._ptr(x), x_stride, int(T), _lib._ptr(out),
-                         int(out.shape[1]), _lib.stream_ptr(x.device, stream))
+        _lib.check_tensor(self, x, "x")
+        with _lib.call_stream(x.device, stream) as sp:
+            x, x_stride = _lib.device_rows(self, x.contiguous(), "x")
+            C, T = x.shape
+            if C != self.n_channels:
+                raise ValueError("x must be a CUDA float32 tensor [%d, T]" % self.n_channels)
+            if T == 0:
+                return x
+            if T % 256 != 0:
+                raise ValueError("chunk length must be a multiple of 256")
+            out = torch.empty((self.n_channels, T >> self.n_stages), dtype=torch.float32, device=x.device)
+            self.handle.call("frt_decimate_process", _lib._ptr(x), x_stride, int(T), _lib._ptr(out),
+                             int(out.shape[1]), sp)
         return out
 
 

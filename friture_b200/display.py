@@ -175,18 +175,19 @@ class SpectrogramDisplay:
             raise ValueError("db must be a contiguous CUDA float32 tensor")
         _lib.check_tensor(self, db, "db")
         C, F, nb = db.shape
-        self._ensure(db.device)
-        cols, a = self.index.push(F)
-        n_out = len(cols)
-        pixels = torch.empty((C, self.height, n_out), dtype=torch.int32, device=db.device)
-        if F == 0:
-            return pixels
-        cols_d = torch.from_numpy(cols).to(db.device) if n_out else None
-        a_d = torch.from_numpy(a.astype(np.float32)).to(db.device) if n_out else None
-        T = self._tables
-        self.handle.call("frt_display_columns", _lib._ptr(db), int(F * nb), int(nb), int(C), int(F),
-                         int(nb), _lib._ptr(T["w"]), c_float(self.spec_min), c_float(self.spec_max),
-                         _lib._ptr(T["i0"]), _lib._ptr(T["t"]), int(self.height), _lib._ptr(cols_d),
-                         _lib._ptr(a_d), int(n_out), _lib._ptr(self._old), _lib._ptr(T["lut"]),
-                         _lib._ptr(pixels) if n_out else None, _lib.stream_ptr(db.device, stream))
+        with _lib.call_stream(db.device, stream) as sp:
+            self._ensure(db.device)
+            cols, a = self.index.push(F)
+            n_out = len(cols)
+            pixels = torch.empty((C, self.height, n_out), dtype=torch.int32, device=db.device)
+            if F == 0:
+                return pixels
+            cols_d = torch.from_numpy(cols).to(db.device) if n_out else None
+            a_d = torch.from_numpy(a.astype(np.float32)).to(db.device) if n_out else None
+            T = self._tables
+            self.handle.call("frt_display_columns", _lib._ptr(db), int(F * nb), int(nb), int(C), int(F),
+                             int(nb), _lib._ptr(T["w"]), c_float(self.spec_min), c_float(self.spec_max),
+                             _lib._ptr(T["i0"]), _lib._ptr(T["t"]), int(self.height), _lib._ptr(cols_d),
+                             _lib._ptr(a_d), int(n_out), _lib._ptr(self._old), _lib._ptr(T["lut"]),
+                             _lib._ptr(pixels) if n_out else None, sp)
         return pixels

@@ -182,9 +182,9 @@ class Octave_Filters():
                          int(boct_fir.shape[1]), _lib._ptr(boct_fir), _lib._ptr(bdec_fir))
         self._fir_key = key
 
-    def _filter_batch_fir(self, x, x_stride, block, stream=None):
+    def _filter_batch_fir(self, x, x_stride, block, sp):
         """Live-path numerics: band outputs of x [C, n_blocks*block] (row stride ``x_stride``),
-        block by block."""
+        block by block, on the stream ``sp``, which is current."""
         import torch
         C, T = x.shape
         if block > 4096 or block % (1 << (self._n_octaves - 1)):
@@ -193,7 +193,6 @@ class Octave_Filters():
         self._ensure_fir_plan(C)
         offsets, lengths = ragged_layout(block, self.bandsperoctave, self._n_octaves)
         ystride = int(offsets[-1] + lengths[-1])
-        sp = _lib.stream_ptr(x.device, stream)
         parts = []
         for b in range(T // block):
             ybuf = torch.empty((C, ystride), dtype=torch.float32, device=x.device)
@@ -257,26 +256,26 @@ class Octave_Filters():
             raise ValueError("block > %d: the reference's smoothing kernel is shorter than the "
                              "block (exp_smoothing.py:43-47)" % MAX_BLOCK)
         n_blocks = T // block
-        if self._mode == "fft":
+        if self._mode == "fft" and energies:
+            raise ValueError("fft mode gives the band outputs only (energies=False, want_y=True)")
+        with _lib.call_stream(x.device, stream) as sp:
+            if self._mode == "fft":
+                return self._filter_batch_fir(x, x_stride, block, sp), None
+            self._ensure_plan(C)
+            e = None
             if energies:
-                raise ValueError("fft mode gives the band outputs only (energies=False, want_y=True)")
-            return self._filter_batch_fir(x, x_stride, block, stream), None
-        self._ensure_plan(C)
-        e = None
-        if energies:
-            e = torch.empty((C, n_blocks, self.nbands), dtype=torch.float32, device=x.device)
-        ybuf = None
-        ystride = 0
-        if want_y:
-            offsets, lengths = ragged_layout(T, self.bandsperoctave, self._n_octaves)
-            ystride = int(offsets[-1] + lengths[-1])
-            ybuf = torch.empty((C, ystride), dtype=torch.float32, device=x.device)
-        self.handle.call("frt_bank_process", _lib._ptr(x), x_stride, int(block),
-                         int(n_blocks), _lib._ptr(e), _lib._ptr(ybuf), ystride,
-                         1 if db else 0, _lib.stream_ptr(x.device, stream))
-        y = None
-        if want_y:
-            y = [ybuf[:, int(o):int(o) + int(n)] for o, n in zip(offsets, lengths)]
+                e = torch.empty((C, n_blocks, self.nbands), dtype=torch.float32, device=x.device)
+            ybuf = None
+            ystride = 0
+            if want_y:
+                offsets, lengths = ragged_layout(T, self.bandsperoctave, self._n_octaves)
+                ystride = int(offsets[-1] + lengths[-1])
+                ybuf = torch.empty((C, ystride), dtype=torch.float32, device=x.device)
+            self.handle.call("frt_bank_process", _lib._ptr(x), x_stride, int(block),
+                             int(n_blocks), _lib._ptr(e), _lib._ptr(ybuf), ystride, 1 if db else 0, sp)
+            y = None
+            if want_y:
+                y = [ybuf[:, int(o):int(o) + int(n)] for o, n in zip(offsets, lengths)]
         return y, e
 
     def energies_batch(self, x, block, db=False):

@@ -98,7 +98,8 @@ class OctaveSpectrumAnalyzer:
             raise ValueError("x rows must not overlap")
         self._ensure_plan()
         n_blocks = T // block
-        out = torch.empty((C, n_blocks, self.nbands), dtype=torch.float32, device=x.device)
-        self.filters.handle.call("frt_firbank_levels", _lib._ptr(x), x_stride, int(block), int(n_blocks),
-                                 _lib._ptr(out), 1 if db else 0, _lib.stream_ptr(x.device, stream))
+        with _lib.call_stream(x.device, stream) as sp:
+            out = torch.empty((C, n_blocks, self.nbands), dtype=torch.float32, device=x.device)
+            self.filters.handle.call("frt_firbank_levels", _lib._ptr(x), x_stride, int(block), int(n_blocks),
+                                     _lib._ptr(out), 1 if db else 0, sp)
         return out

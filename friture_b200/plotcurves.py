@@ -148,19 +148,19 @@ class _PlotState:
             y = y.contiguous()
         h = self.handle
         dev = y.device
-        out = [torch.empty((C, K), dtype=torch.float32, device=dev) for _ in range(4 if peaks else 2)]
-        state = (self.peak, self.peak_int, self.peak_decay)
-        reset = peaks and (self.peak is None or self.peak.shape[1] != K)
-        if reset:
-            # kept aside until the call is accepted: a rejected call must not leave a state of the
-            # new size that the next call would read without the reset
-            state = tuple(torch.empty((C, K), dtype=torch.float64, device=dev) for _ in range(3))
-        st = [_lib._ptr(t) if peaks else None for t in state]
-        sp = _lib.stream_ptr(dev)
-        h.call("frt_plot_curves", _lib._ptr(y), int(y.stride(0)), int(y.stride(1)), int(C), int(S),
-               int(K), c_double(self.spec_min), c_double(self.spec_max), c_double(PEAK_DECAY),
-               1 if peaks else 0, 1 if reset else 0, *st, *[_lib._ptr(t) for t in out],
-               *([None, None] if not peaks else []), sp)
+        with _lib.call_stream(dev) as sp:
+            out = [torch.empty((C, K), dtype=torch.float32, device=dev) for _ in range(4 if peaks else 2)]
+            state = (self.peak, self.peak_int, self.peak_decay)
+            reset = peaks and (self.peak is None or self.peak.shape[1] != K)
+            if reset:
+                # kept aside until the call is accepted: a rejected call must not leave a state of the
+                # new size that the next call would read without the reset
+                state = tuple(torch.empty((C, K), dtype=torch.float64, device=dev) for _ in range(3))
+            st = [_lib._ptr(t) if peaks else None for t in state]
+            h.call("frt_plot_curves", _lib._ptr(y), int(y.stride(0)), int(y.stride(1)), int(C), int(S),
+                   int(K), c_double(self.spec_min), c_double(self.spec_max), c_double(PEAK_DECAY),
+                   1 if peaks else 0, 1 if reset else 0, *st, *[_lib._ptr(t) for t in out],
+                   *([None, None] if not peaks else []), sp)
         if reset:
             self.peak, self.peak_int, self.peak_decay = state
         return out + [None] * (4 - len(out))

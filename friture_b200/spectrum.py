@@ -88,28 +88,27 @@ class SpectrumAnalyzer:
             x = x[:, 0]
         nb = self.fft_size // 2 + 1
         nf = frame_count(x.shape[1], self.fft_size, self.hop)
-        power = self.proc.stft(x, hop=self.hop, log=False, stream=stream)
-        if self._disp is None:
-            self._disp = torch.zeros((C, nb), dtype=torch.float32, device=x.device)
-        if self._w_dev is None:
-            self._w_dev = torch.from_numpy(np.ascontiguousarray(self.w, dtype=np.float32)).to(x.device)
-        db = torch.empty((C, nb), dtype=torch.float32, device=x.device)
-        imax = torch.empty(C, dtype=torch.int32, device=x.device)
-        ipitch = torch.empty(C, dtype=torch.int32, device=x.device)
-        self.proc.handle.call("frt_spectrum_reduce", _lib._ptr(power), int(nf * nb), int(nb), int(C),
-                              int(nf), int(nb), c_float(self.alpha), _lib._ptr(self._disp),
-                              _lib._ptr(self._w_dev) if self.weighting else None, _lib._ptr(db),
-                              _lib._ptr(imax), _lib._ptr(ipitch), _lib.stream_ptr(x.device, stream))
-        if self._disp2 is not None and nf > 0:
-            # the widget smooths an all-zero second column on every tick it does not fill
-            # (spectrum.py:142,158-159): dispbuffers2 * (1-alpha)^frames, on the kernel's stream
-            ts = torch.cuda.current_stream(x.device) if stream is None else \
-                torch.cuda.ExternalStream(int(stream), device=x.device)
-            with torch.cuda.stream(ts):
+        with _lib.call_stream(x.device, stream) as sp:
+            power = self.proc.stft(x, hop=self.hop, log=False, stream=stream)
+            if self._disp is None:
+                self._disp = torch.zeros((C, nb), dtype=torch.float32, device=x.device)
+            if self._w_dev is None:
+                self._w_dev = torch.from_numpy(np.ascontiguousarray(self.w, dtype=np.float32)).to(x.device)
+            db = torch.empty((C, nb), dtype=torch.float32, device=x.device)
+            imax = torch.empty(C, dtype=torch.int32, device=x.device)
+            ipitch = torch.empty(C, dtype=torch.int32, device=x.device)
+            self.proc.handle.call("frt_spectrum_reduce", _lib._ptr(power), int(nf * nb), int(nb), int(C),
+                                  int(nf), int(nb), c_float(self.alpha), _lib._ptr(self._disp),
+                                  _lib._ptr(self._w_dev) if self.weighting else None, _lib._ptr(db),
+                                  _lib._ptr(imax), _lib._ptr(ipitch), sp)
+            if self._disp2 is not None and nf > 0:
+                # the widget smooths an all-zero second column on every tick it does not fill
+                # (spectrum.py:142,158-159): dispbuffers2 * (1-alpha)^frames
                 self._disp2.mul_((1. - self.alpha) ** nf)
-        return self._indices_to_hz(db, imax, ipitch)
+            return self._indices_to_hz(db, imax, ipitch)
 
     def _indices_to_hz(self, db, imax, ipitch):
+        # on the call's stream, which is current: the reads wait for the kernel that writes them
         fmax = self.freq[imax.cpu().numpy()]
         fpitch = np.maximum(self.freq[ipitch.cpu().numpy()], 1e-20)     # spectrum.py:181
         return db, fmax, fpitch
@@ -120,20 +119,20 @@ class SpectrumAnalyzer:
         C, _, T = x.shape
         nb = self.fft_size // 2 + 1
         nf = frame_count(T, self.fft_size, self.hop)
-        power = self.proc.stft(x.view(2 * C, T), hop=self.hop, log=False, stream=stream)
-        if self._disp is None:
-            self._disp = torch.zeros((C, nb), dtype=torch.float32, device=x.device)
-        if self._disp2 is None:
-            self._disp2 = torch.zeros((C, nb), dtype=torch.float32, device=x.device)
-        db = torch.empty((C, nb), dtype=torch.float32, device=x.device)
-        imax = torch.empty(C, dtype=torch.int32, device=x.device)
-        ipitch = torch.empty(C, dtype=torch.int32, device=x.device)
-        # power [2C, nf, nb]: pair c's reference at row 2c, its measurement at row 2c + 1
-        p1 = power.data_ptr() if nf else 0
-        p2 = p1 + 4 * nf * nb if nf else 0
-        self.proc.handle.call("frt_spectrum_reduce_dual", _lib._ptr(p1), _lib._ptr(p2),
-                              int(2 * nf * nb), int(nb), int(C), int(nf), int(nb),
-                              c_float(self.alpha), _lib._ptr(self._disp), _lib._ptr(self._disp2),
-                              _lib._ptr(db), _lib._ptr(imax), _lib._ptr(ipitch),
-                              _lib.stream_ptr(x.device, stream))
-        return self._indices_to_hz(db, imax, ipitch)
+        with _lib.call_stream(x.device, stream) as sp:
+            power = self.proc.stft(x.view(2 * C, T), hop=self.hop, log=False, stream=stream)
+            if self._disp is None:
+                self._disp = torch.zeros((C, nb), dtype=torch.float32, device=x.device)
+            if self._disp2 is None:
+                self._disp2 = torch.zeros((C, nb), dtype=torch.float32, device=x.device)
+            db = torch.empty((C, nb), dtype=torch.float32, device=x.device)
+            imax = torch.empty(C, dtype=torch.int32, device=x.device)
+            ipitch = torch.empty(C, dtype=torch.int32, device=x.device)
+            # power [2C, nf, nb]: pair c's reference at row 2c, its measurement at row 2c + 1
+            p1 = power.data_ptr() if nf else 0
+            p2 = p1 + 4 * nf * nb if nf else 0
+            self.proc.handle.call("frt_spectrum_reduce_dual", _lib._ptr(p1), _lib._ptr(p2),
+                                  int(2 * nf * nb), int(nb), int(C), int(nf), int(nb),
+                                  c_float(self.alpha), _lib._ptr(self._disp), _lib._ptr(self._disp2),
+                                  _lib._ptr(db), _lib._ptr(imax), _lib._ptr(ipitch), sp)
+            return self._indices_to_hz(db, imax, ipitch)

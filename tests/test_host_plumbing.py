@@ -15,6 +15,7 @@ PKG = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), 
 ONLY_IN_LIB = [
     "current_stream_ptr(",
     "c_void_p(int(stream))",
+    "torch.cuda.ExternalStream(",   # call_stream makes the caller's stream current
     "torch.cuda.current_device()",
     "default_handle()",
     "check_device(",

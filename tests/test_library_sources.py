@@ -1,7 +1,9 @@
 """CPU: the CUDA sources keep one copy of the launch path and of the device primitives the kernel
 files share.  Every kernel launch goes through frt_launch (friture_b200/csrc/frt_internal.cuh), which
 sets the dynamic shared-memory limit, checks the launch and counts it; the fast log2 and the cp.async
-wrappers are defined there once."""
+wrappers are defined there once.  So are frt_sync_copy and frt_sync_zero, the only synchronous copies
+and fills: they drain the device before and after, so that no kernel queued on any stream sees a plan,
+setter or reset that came after it, and no kernel launched next misses one that came before."""
 import os
 
 import pytest
@@ -18,6 +20,8 @@ ONLY_IN_HOME = [
     "cp.async.cg",              # cp_async16
     "commit_group",             # cp_async_commit
     "wait_group",               # cp_async_wait<N>
+    "cudaMemcpy(",              # frt_sync_copy
+    "cudaMemset(",              # frt_sync_zero
 ]
 
 
