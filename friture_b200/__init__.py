@@ -9,9 +9,9 @@ device raises.
 from ._lib import FrtError, Handle, lib_path, load_library  # noqa: F401
 from .audioproc import audioproc, AudioProc, SAMPLING_RATE, FRAMES_PER_BUFFER  # noqa: F401
 from .octavefilters import Octave_Filters, OctaveFilters  # noqa: F401
-from .correlation import generalized_cross_correlation, GccPhat  # noqa: F401
+from .correlation import generalized_cross_correlation, GccPhat, PairGccPhat  # noqa: F401
 from .analyzer import ChannelAnalyzer  # noqa: F401
 
 __all__ = ["FrtError", "Handle", "lib_path", "load_library", "audioproc", "AudioProc",
-           "Octave_Filters", "OctaveFilters", "generalized_cross_correlation", "GccPhat",
+           "Octave_Filters", "OctaveFilters", "generalized_cross_correlation", "GccPhat", "PairGccPhat",
            "ChannelAnalyzer", "SAMPLING_RATE", "FRAMES_PER_BUFFER"]

@@ -47,7 +47,6 @@ class GccPhat:
         self._have_prev = False
 
     def estimate(self, d0, d1, smooth=True, want_xcorr=False, stream=None):
-        import torch
         _lib.check_tensor(self, d0, "d0")
         with _lib.call_stream(d0.device, stream) as sp:
             d0, _ = _lib.device_rows(self, d0.contiguous(), "d0")
@@ -58,28 +57,87 @@ class GccPhat:
             if L != self.length:
                 raise ValueError("frame length %d != planned %d" % (L, self.length))
             self.handle.call("frt_gcc_plan", int(L))
-            Lo = self.out_length
-            idx = torch.empty(P, dtype=torch.int32, device=d0.device)
-            val = torch.empty(P, dtype=torch.float32, device=d0.device)
-            xc = torch.empty((P, Lo), dtype=torch.float32, device=d0.device) if want_xcorr else None
-            sm = None
-            have_prev = 0
-            if smooth:
-                if self._smoothed is None or tuple(self._smoothed.shape) != (P, Lo):
-                    self._smoothed = torch.zeros((P, Lo), dtype=torch.float32, device=d0.device)
-                    self._have_prev = False
-                sm = self._smoothed
-                # 2 = per pair: a pair whose frames have all been silent so far has no previous smoothed
-                # frame (the kernel marks it), like old_Xcorr = None in the widget
-                have_prev = 2 if self._have_prev else 0
+            idx, val, xc, sm, have_prev = self._outputs(P, d0.device, smooth, want_xcorr)
             self.handle.call("frt_gcc_phat", _lib._ptr(d0), _lib._ptr(d1), int(L), int(P),
                              _lib._ptr(xc), _lib._ptr(sm), have_prev, _lib._ptr(idx), _lib._ptr(val), sp)
         if smooth:
             self._have_prev = True
         return idx, val, xc
 
+    def _outputs(self, P, device, smooth, want_xcorr):
+        """The output tensors of a call on P pairs, and the smoothed buffer and ``have_prev`` to pass."""
+        import torch
+        Lo = self.out_length
+        idx = torch.empty(P, dtype=torch.int32, device=device)
+        val = torch.empty(P, dtype=torch.float32, device=device)
+        xc = torch.empty((P, Lo), dtype=torch.float32, device=device) if want_xcorr else None
+        sm = None
+        have_prev = 0
+        if smooth:
+            if self._smoothed is None or tuple(self._smoothed.shape) != (P, Lo):
+                self._smoothed = torch.zeros((P, Lo), dtype=torch.float32, device=device)
+                self._have_prev = False
+            sm = self._smoothed
+            # 2 = per pair: a pair whose frames have all been silent so far has no previous smoothed
+            # frame (the kernel marks it), like old_Xcorr = None in the widget
+            have_prev = 2 if self._have_prev else 0
+        return idx, val, xc, sm, have_prev
+
     def delay_ms(self, idx):
         """Index -> delay in ms, wrapped to +-L/2 (delay_estimator.py:147-152)."""
         d = 1e3 * idx.to("cpu").double().numpy() / self.fs
         span = 1e3 * self.length / self.fs
         return np.where(d > span / 2.0, d - span, d)
+
+
+class PairGccPhat(GccPhat):
+    """GCC-PHAT between channels of one multichannel frame: ``estimate(x)`` takes x [C, L] and
+    correlates, for every entry (i, j) of ``pairs``, channel i (the widget's channel 0) with
+    channel j.  Each channel is transformed once however many pairs it is in.  Outputs, smoothing
+    state, ``reset`` and ``delay_ms`` are those of ``GccPhat``, indexed by pair.  With the pairs
+    (0, 1), (2, 3), ... the results are the same bits as ``GccPhat.estimate(x[0::2], x[1::2])``."""
+
+    def __init__(self, length, n_channels, pairs, handle=None, fs=12000.0):
+        super().__init__(length, handle=handle, fs=fs)
+        self.n_channels = int(n_channels)
+        if self.n_channels < 1:
+            raise ValueError("n_channels must be >= 1")
+        p = np.asarray(pairs)
+        if p.size == 0:
+            p = np.zeros((0, 2), dtype=np.int32)
+        if p.ndim != 2 or p.shape[1] != 2 or not np.issubdtype(p.dtype, np.integer):
+            raise ValueError("pairs must be integer (i, j) pairs, shape [P, 2]")
+        if p.size and (p.min() < 0 or p.max() >= self.n_channels):
+            raise ValueError("pair channels must lie in 0 .. %d" % (self.n_channels - 1))
+        self.pairs = np.ascontiguousarray(p, dtype=np.int32)
+        self.n_pairs = self.pairs.shape[0]
+        self._table = object()   # identifies this object's table on the handle
+
+    def _sync_table(self):
+        """Give the handle this object's pair table unless it already holds it: another object on
+        the same handle may have set its own since."""
+        h = self.handle
+        if getattr(h, "_gcc_pairs_table", None) is not self._table:
+            h.call("frt_gcc_set_pairs", self.n_channels, _lib._ptr(self.pairs), self.n_pairs)
+            h._gcc_pairs_table = self._table
+
+    def estimate(self, x, smooth=True, want_xcorr=False, stream=None):
+        """x: CUDA float32 [C, L], any row stride.  Returns (idx [P], val [P], xcorr [P, L'] or None)."""
+        _lib.check_tensor(self, x, "x")
+        with _lib.call_stream(x.device, stream) as sp:
+            if x.dim() == 2 and x.shape[1] > 0 and x.stride(1) != 1:
+                x = x.contiguous()
+            x, x_stride = _lib.device_rows(self, x, "x")
+            C, L = x.shape
+            if C != self.n_channels:
+                raise ValueError("x has %d channels, the pair table %d" % (C, self.n_channels))
+            if L != self.length:
+                raise ValueError("frame length %d != planned %d" % (L, self.length))
+            self.handle.call("frt_gcc_plan", int(L))
+            self._sync_table()
+            idx, val, xc, sm, have_prev = self._outputs(self.n_pairs, x.device, smooth, want_xcorr)
+            self.handle.call("frt_gcc_phat_pairs", _lib._ptr(x), x_stride, _lib._ptr(xc), _lib._ptr(sm),
+                             have_prev, _lib._ptr(idx), _lib._ptr(val), sp)
+        if smooth:
+            self._have_prev = True
+        return idx, val, xc

@@ -15,6 +15,17 @@ __device__ __forceinline__ float2 cmul(float2 a, float2 w) {
 __device__ __forceinline__ float2 mul_mj(float2 a) { return make_float2(a.y, -a.x); }   // * (-j)
 __device__ __forceinline__ float2 cscale(float2 a, float s) { return make_float2(a.x * s, a.y * s); }
 
+// The two real sequences packed as u + j v share one complex transform Z; zk = Z[k], zm = Z[L-k]
+// (Z[0] for k = 0) give their spectra D0 = (Zk + conj Zm)/2 and D1 = (Zk - conj Zm)/(2j).
+__device__ __forceinline__ void split_packed(float2 zk, float2 zm, float2 &D0, float2 &D1) {
+    D0 = make_float2(0.5f * (zk.x + zm.x), 0.5f * (zk.y - zm.y));
+    D1 = make_float2(0.5f * (zk.y + zm.y), -0.5f * (zk.x - zm.x));
+}
+// The cross-spectrum G = conj(D0) D1 of GCC (correlation.py:34).
+__device__ __forceinline__ float2 cross_spectrum(float2 D0, float2 D1) {
+    return make_float2(D0.x * D1.x + D0.y * D1.y, D0.x * D1.y - D0.y * D1.x);
+}
+
 // In-register forward DFT of R points, outputs in natural order.
 template <int R> __device__ __forceinline__ void dft(float2 (&v)[R]);
 

@@ -159,6 +159,15 @@ int gcc_long_length(const frt_ctx *h);        // the planned L; needs h->gcc_lon
 int gcc_long_phat(frt_ctx *h, const float *d0_dev, const float *d1_dev, int64_t stride, int n_pairs,
                   float *xcorr_dev, float *smoothed_dev, int have_prev, int *idx_dev, float *val_dev,
                   cudaStream_t st);
+// frt_gcc_phat_pairs: the spectra of the table's n_channels channels, D_c[k] for k = 0..L'/2, whether
+// each channel is constant, and a zero row of L floats when n_channels is odd (else NULL).
+struct GccSpectra {
+    float2 *spec;
+    int *quiet;
+    float *zero;
+};
+int gcc_long_phat_pairs(frt_ctx *h, const float *x_dev, int64_t stride, const GccSpectra &w, float *xcorr_dev,
+                        float *smoothed_dev, int have_prev, int *idx_dev, float *val_dev, cudaStream_t st);
 
 // A plan call builds into a local PlanPtr and moves it into its slot only on success, so a call
 // that fails leaves the previous plan of that kind in place.
@@ -176,6 +185,10 @@ struct frt_ctx {
     PlanPtr<GccLongPlan> gcc_long;    // lengths back and forth rebuilds neither
     bool gcc_long_route = false;      // the last accepted frt_gcc_plan length runs on gcc_long
     DeviceArray<unsigned char> gcc_long_ws;   // the Bluestein route's workspace, grow-only
+    DeviceArray<int2> gcc_pairs;      // frt_gcc_set_pairs: the pair table (i, j) on the device
+    int gcc_pairs_n = -1;             // its entries; -1 before the first accepted table
+    int gcc_pairs_channels = 0;       // the channels of the input it indexes
+    DeviceArray<unsigned char> gcc_spec_ws;   // frt_gcc_phat_pairs' per-channel spectra, grow-only
     StftStaging stft_host;
     CombStaging comb_host;
 };

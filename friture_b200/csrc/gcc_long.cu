@@ -58,7 +58,7 @@ struct PairState {
     float m0, m1;
     int silent, prev;
     unsigned gmax;             // max|G| as float bits: non-negative floats order like their bits
-    unsigned pad;
+    unsigned quiet;            // bit 0: d0 is constant, bit 1: d1 is constant
     unsigned long long best;   // bits of |Xs| << 32 | (0xffffffff - index): the max is the first maximum
 };
 
@@ -84,10 +84,23 @@ struct GlArgs {
     int have_prev;
     int *idx;
     float *val;
+    // frt_gcc_phat_pairs.  Phase 1 (a group of packed channel pairs d0 = channel ch0 + 2p, d1 = the next
+    // one): per_channel = 1, so that a pair is skipped only when both channels are constant, and the
+    // spectra and flags of channels < n_ch land in spec / quiet.  Phase 2 (a group of table entries):
+    // pair p correlates channels pairs[p].
+    int per_channel, ch0, n_ch;
+    float2 *spec;              // [n_ch][L'/2+1]
+    int *quiet;                // [n_ch]
+    const int2 *pairs;
 };
 
 __device__ __forceinline__ float2 conj2(float2 a) { return make_float2(a.x, -a.y); }
 __device__ __forceinline__ int brev(int k, int bits) { return (int)(__brev((unsigned)k) >> (32 - bits)); }
+// Whether the pair blends with its smoothed row.  have_prev: 1 = every pair; 2 = the pairs without the
+// "no previous" NaN in slot 0.  Read before the last pass rewrites slot 0.
+__device__ __forceinline__ int gl_prev(const GlArgs &a, int pair) {
+    return a.have_prev == 1 || (a.have_prev == 2 && !isnan(a.smoothed[(size_t)pair * a.Lp]));
+}
 __device__ __forceinline__ float2 tw_m(const GlArgs &a, unsigned e) {
     return cmul(__ldg(a.tw_hi + (e >> a.tw_shift)), __ldg(a.tw_lo + (e & ((1u << a.tw_shift) - 1u))));
 }
@@ -209,13 +222,10 @@ __global__ void __launch_bounds__(256) gl_stats_finish(const GlArgs a) {
         st.m0 = s0 / (float)a.L;
         st.m1 = s1 / (float)a.L;
         // constant inputs (std == 0) are skipped by the reference (delay_estimator.py:129-131)
-        st.silent = !(span0 > 0.f) || !(span1 > 0.f);
-        // have_prev: 1 = every pair blends; 2 = the pairs without the "no previous" NaN in slot 0.
-        // Read here, before the last pass rewrites slot 0.
-        st.prev = a.have_prev == 1 ||
-                  (a.have_prev == 2 && !isnan(a.smoothed[(size_t)pair * a.Lp]));
+        st.quiet = (span0 > 0.f ? 0u : 1u) | (span1 > 0.f ? 0u : 2u);
+        st.silent = a.per_channel ? st.quiet == 3u : st.quiet != 0u;
+        st.prev = gl_prev(a, pair);
         st.gmax = 0u;
-        st.pad = 0u;
         st.best = 0ull;
         a.st[pair] = st;
     }
@@ -359,12 +369,65 @@ __global__ void __launch_bounds__(GL_THREADS) gl_split(const GlArgs a) {
     const int k = blockIdx.x * blockDim.x + threadIdx.x;
     float ag = 0.f;
     if (k <= a.Lp / 2) {
-        const float2 zk = z[k], zm = z[k == 0 ? 0 : a.L - k];
-        // D0 = (Zk + conj Zm)/2 ; D1 = (Zk - conj Zm)/(2j)
-        const float2 D0 = make_float2(0.5f * (zk.x + zm.x), 0.5f * (zk.y - zm.y));
-        const float2 D1 = make_float2(0.5f * (zk.y + zm.y), -0.5f * (zk.x - zm.x));
-        const float2 G = make_float2(D0.x * D1.x + D0.y * D1.y, D0.x * D1.y - D0.y * D1.x);
+        float2 D0, D1;
+        split_packed(z[k], z[k == 0 ? 0 : a.L - k], D0, D1);
+        const float2 G = cross_spectrum(D0, D1);
         a.g[(size_t)pair * (a.Lp / 2 + 1) + k] = G;
+        ag = hypotf(G.x, G.y);
+    }
+    const float m = block_max(ag, s_red);
+    if (threadIdx.x == 0) atomicMax(&a.st[pair].gmax, __float_as_uint(m));
+}
+
+// ---- frt_gcc_phat_pairs, phase 1: the Hermitian split of a packed channel pair's Z into the two
+// channels' spectra, and the channels' constant flags
+__global__ void __launch_bounds__(GL_THREADS) gl_split_spec(const GlArgs a) {
+    const int pair = blockIdx.y, c0 = a.ch0 + 2 * pair, c1 = c0 + 1;
+    const PairState st = a.st[pair];
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+        a.quiet[c0] = st.quiet & 1u;
+        if (c1 < a.n_ch) a.quiet[c1] = (st.quiet >> 1) & 1u;
+    }
+    if (st.silent) return;
+    const float2 *z = a.buf + ((size_t)pair << (a.log1 + a.log2));
+    const int k = blockIdx.x * blockDim.x + threadIdx.x;
+    const size_t H = (size_t)(a.Lp / 2 + 1);
+    if (k < (int)H) {
+        float2 D0, D1;
+        split_packed(z[k], z[k == 0 ? 0 : a.L - k], D0, D1);
+        a.spec[(size_t)c0 * H + k] = D0;
+        if (c1 < a.n_ch) a.spec[(size_t)c1 * H + k] = D1;
+    }
+}
+
+// ---- phase 2, per table entry (i, j): the state gl_stats_finish gives a pair; silent when a channel
+// is constant
+__global__ void __launch_bounds__(256) gl_pair_state(const GlArgs a, int n_pairs) {
+    const int pair = blockIdx.x * blockDim.x + threadIdx.x;
+    if (pair >= n_pairs) return;
+    const int2 ij = a.pairs[pair];
+    PairState st;
+    st.m0 = st.m1 = 0.f;
+    st.quiet = (a.quiet[ij.x] ? 1u : 0u) | (a.quiet[ij.y] ? 2u : 0u);
+    st.silent = st.quiet != 0u;
+    st.prev = gl_prev(a, pair);
+    st.gmax = 0u;
+    st.best = 0ull;
+    a.st[pair] = st;
+}
+
+// ---- phase 2: G = conj(D_i) D_j for k = 0..L'/2 from the stored spectra, and max|G| (as gl_split)
+__global__ void __launch_bounds__(GL_THREADS) gl_cross(const GlArgs a) {
+    __shared__ float s_red[33];
+    const int pair = blockIdx.y;
+    if (a.st[pair].silent) return;
+    const int2 ij = a.pairs[pair];
+    const size_t H = (size_t)(a.Lp / 2 + 1);
+    const int k = blockIdx.x * blockDim.x + threadIdx.x;
+    float ag = 0.f;
+    if (k < (int)H) {
+        const float2 G = cross_spectrum(a.spec[(size_t)ij.x * H + k], a.spec[(size_t)ij.y * H + k]);
+        a.g[(size_t)pair * H + k] = G;
         ag = hypotf(G.x, G.y);
     }
     const float m = block_max(ag, s_red);
@@ -510,24 +573,25 @@ int gcc_long_plan(frt_ctx *h, int length) {
 
 int gcc_long_length(const frt_ctx *h) { return h->gcc_long->L; }
 
-int gcc_long_phat(frt_ctx *h, const float *d0_dev, const float *d1_dev, int64_t stride, int n_pairs,
-                  float *xcorr_dev, float *smoothed_dev, int have_prev, int *idx_dev, float *val_dev,
-                  cudaStream_t st) {
-    const GccLongPlan *pl = h->gcc_long.get();
+// The arguments every pass of a call shares, and its workspace: groups of pairs whose buffers fit
+// GL_WORKSPACE_BUDGET, at most n_pairs.  Returns the group size through `group`.
+static int gl_setup(frt_ctx *h, const GccLongPlan *pl, int n_pairs, int64_t stride, int have_prev, GlArgs &a,
+                    int &group) {
     const size_t M = size_t(1) << (pl->log1 + pl->log2), H = size_t(pl->Lp / 2 + 1);
     const int n_chunks = (pl->L + GL_STATS_CHUNK - 1) / GL_STATS_CHUNK;
     auto up = [](size_t b) { return (b + 255) & ~size_t(255); };
     const size_t per_pair = up(M * sizeof(float2)) + up(H * sizeof(float2)) + up(n_chunks * 6 * sizeof(float)) +
                             up(sizeof(PairState));
-    size_t group = GL_WORKSPACE_BUDGET / per_pair;
-    group = group < 1 ? 1 : group > (size_t)GL_MAX_GROUP ? (size_t)GL_MAX_GROUP : group;
-    group = group > (size_t)n_pairs ? (size_t)n_pairs : group;
-    const size_t o_g = up(group * M * sizeof(float2)), o_part = o_g + up(group * H * sizeof(float2)),
-                 o_st = o_part + up(group * n_chunks * 6 * sizeof(float)), bytes = o_st + group * sizeof(PairState);
+    size_t gr = GL_WORKSPACE_BUDGET / per_pair;
+    gr = gr < 1 ? 1 : gr > (size_t)GL_MAX_GROUP ? (size_t)GL_MAX_GROUP : gr;
+    gr = gr > (size_t)n_pairs ? (size_t)n_pairs : gr;
+    const size_t o_g = up(gr * M * sizeof(float2)), o_part = o_g + up(gr * H * sizeof(float2)),
+                 o_st = o_part + up(gr * n_chunks * 6 * sizeof(float)), bytes = o_st + gr * sizeof(PairState);
     FRT_CUDA(h, h->gcc_long_ws.grow(bytes));
     unsigned char *ws = h->gcc_long_ws.get();
+    group = (int)gr;
 
-    GlArgs a;
+    a = GlArgs{};
     a.stride = stride;
     a.L = pl->L;
     a.Lp = pl->Lp;
@@ -546,41 +610,114 @@ int gcc_long_phat(frt_ctx *h, const float *d0_dev, const float *d1_dev, int64_t 
     a.part = (float *)(ws + o_part);
     a.st = (PairState *)(ws + o_st);
     a.have_prev = have_prev;
+    return FRT_OK;
+}
+
+// The forward transform of np packed pairs d0 + j d1 (means, silence, the three passes), leaving Z in
+// the pairs' buffers.
+static int gl_forward(frt_ctx *h, const GccLongPlan *pl, GlArgs &a, int np, cudaStream_t st) {
     const int M1 = 1 << pl->log1, M2 = 1 << pl->log2;
     const size_t smem_cols = sizeof(float2) * (size_t)(M1 + 1) << pl->lgc;
     const size_t smem_rows = sizeof(float2) * (size_t)M2 << pl->lgr;
-    const double inv_m = 1.0 / (double)M;
-    for (int p0 = 0; p0 < n_pairs; p0 += (int)group) {
-        const int np = n_pairs - p0 < (int)group ? n_pairs - p0 : (int)group;
+    const dim3 g_cols(M2 >> pl->lgc, np), g_rows(M1 >> pl->lgr, np);
+    a.chirp = pl->chirp.get();
+    a.bt = pl->bt.get();
+    a.scale = (float)(1.0 / std::ldexp(1.0, pl->log1 + pl->log2));
+    int rc = frt_launch(h, gl_stats, dim3(a.n_chunks, np), 256, 0, st, a);
+    if (rc == FRT_OK) rc = frt_launch(h, gl_stats_finish, np, 256, 0, st, a);
+    if (rc == FRT_OK) rc = frt_launch(h, gl_cols_fwd<false>, g_cols, GL_THREADS, smem_cols, st, a);
+    if (rc == FRT_OK) rc = frt_launch(h, gl_rows, g_rows, GL_THREADS, smem_rows, st, a);
+    if (rc == FRT_OK) rc = frt_launch(h, gl_cols_inv<false>, g_cols, GL_THREADS, smem_cols, st, a);
+    return rc;
+}
+
+// From G and max|G| of np pairs: the inverse real transform of length L' through a forward transform of
+// the conjugate, the smoothing and the peak pick.
+static int gl_inverse(frt_ctx *h, const GccLongPlan *pl, GlArgs &a, int np, cudaStream_t st) {
+    const int M1 = 1 << pl->log1, M2 = 1 << pl->log2;
+    const size_t smem_cols = sizeof(float2) * (size_t)(M1 + 1) << pl->lgc;
+    const size_t smem_rows = sizeof(float2) * (size_t)M2 << pl->lgr;
+    const dim3 g_cols(M2 >> pl->lgc, np), g_rows(M1 >> pl->lgr, np);
+    a.chirp = pl->Lp != pl->L ? pl->chirp_p.get() : pl->chirp.get();
+    a.bt = pl->Lp != pl->L ? pl->bt_p.get() : pl->bt.get();
+    a.scale = (float)(1.0 / std::ldexp(1.0, pl->log1 + pl->log2) / (double)pl->Lp);
+    int rc = frt_launch(h, gl_cols_fwd<true>, g_cols, GL_THREADS, smem_cols, st, a);
+    if (rc == FRT_OK) rc = frt_launch(h, gl_rows, g_rows, GL_THREADS, smem_rows, st, a);
+    if (rc == FRT_OK) rc = frt_launch(h, gl_cols_inv<true>, g_cols, GL_THREADS, smem_cols, st, a);
+    if (rc == FRT_OK) rc = frt_launch(h, gl_finish, (np + 255) / 256, 256, 0, st, a, np);
+    return rc;
+}
+
+// The outputs of the group starting at pair p0.
+static void gl_outputs(const GccLongPlan *pl, GlArgs &a, int p0, float *xcorr_dev, float *smoothed_dev,
+                       int *idx_dev, float *val_dev) {
+    a.xcorr = xcorr_dev ? xcorr_dev + (size_t)p0 * pl->Lp : nullptr;
+    a.smoothed = smoothed_dev ? smoothed_dev + (size_t)p0 * pl->Lp : nullptr;
+    a.idx = idx_dev + p0;
+    a.val = val_dev + p0;
+}
+
+int gcc_long_phat(frt_ctx *h, const float *d0_dev, const float *d1_dev, int64_t stride, int n_pairs,
+                  float *xcorr_dev, float *smoothed_dev, int have_prev, int *idx_dev, float *val_dev,
+                  cudaStream_t st) {
+    const GccLongPlan *pl = h->gcc_long.get();
+    GlArgs a;
+    int group = 0;
+    int rc = gl_setup(h, pl, n_pairs, stride, have_prev, a, group);
+    const unsigned split_blocks = (unsigned)((pl->Lp / 2 + 1 + GL_THREADS - 1) / GL_THREADS);
+    for (int p0 = 0; p0 < n_pairs && rc == FRT_OK; p0 += group) {
+        const int np = n_pairs - p0 < group ? n_pairs - p0 : group;
         a.d0 = d0_dev + (size_t)p0 * stride;
         a.d1 = d1_dev + (size_t)p0 * stride;
-        a.xcorr = xcorr_dev ? xcorr_dev + (size_t)p0 * pl->Lp : nullptr;
-        a.smoothed = smoothed_dev ? smoothed_dev + (size_t)p0 * pl->Lp : nullptr;
-        a.idx = idx_dev + p0;
-        a.val = val_dev + p0;
-        const dim3 g_cols(M2 >> pl->lgc, np), g_rows(M1 >> pl->lgr, np);
-        int rc = frt_launch(h, gl_stats, dim3(n_chunks, np), 256, 0, st, a);
-        if (rc == FRT_OK) rc = frt_launch(h, gl_stats_finish, np, 256, 0, st, a);
-        // forward transform of length L
-        a.chirp = pl->chirp.get();
-        a.bt = pl->bt.get();
-        a.scale = (float)inv_m;
-        if (rc == FRT_OK) rc = frt_launch(h, gl_cols_fwd<false>, g_cols, GL_THREADS, smem_cols, st, a);
-        if (rc == FRT_OK) rc = frt_launch(h, gl_rows, g_rows, GL_THREADS, smem_rows, st, a);
-        if (rc == FRT_OK) rc = frt_launch(h, gl_cols_inv<false>, g_cols, GL_THREADS, smem_cols, st, a);
-        if (rc == FRT_OK)
-            rc = frt_launch(h, gl_split, dim3((unsigned)((H + GL_THREADS - 1) / GL_THREADS), np), GL_THREADS, 0, st, a);
-        // inverse real transform of length L' through a forward transform of the conjugate
-        if (pl->Lp != pl->L) {
-            a.chirp = pl->chirp_p.get();
-            a.bt = pl->bt_p.get();
-        }
-        a.scale = (float)(inv_m / (double)pl->Lp);
-        if (rc == FRT_OK) rc = frt_launch(h, gl_cols_fwd<true>, g_cols, GL_THREADS, smem_cols, st, a);
-        if (rc == FRT_OK) rc = frt_launch(h, gl_rows, g_rows, GL_THREADS, smem_rows, st, a);
-        if (rc == FRT_OK) rc = frt_launch(h, gl_cols_inv<true>, g_cols, GL_THREADS, smem_cols, st, a);
-        if (rc == FRT_OK) rc = frt_launch(h, gl_finish, (np + 255) / 256, 256, 0, st, a, np);
-        if (rc != FRT_OK) return rc;
+        gl_outputs(pl, a, p0, xcorr_dev, smoothed_dev, idx_dev, val_dev);
+        rc = gl_forward(h, pl, a, np, st);
+        if (rc == FRT_OK) rc = frt_launch(h, gl_split, dim3(split_blocks, np), GL_THREADS, 0, st, a);
+        if (rc == FRT_OK) rc = gl_inverse(h, pl, a, np, st);
     }
-    return FRT_OK;
+    return rc;
+}
+
+int gcc_long_phat_pairs(frt_ctx *h, const float *x_dev, int64_t stride, const GccSpectra &w, float *xcorr_dev,
+                        float *smoothed_dev, int have_prev, int *idx_dev, float *val_dev, cudaStream_t st) {
+    const GccLongPlan *pl = h->gcc_long.get();
+    const int C = h->gcc_pairs_channels, n_pairs = h->gcc_pairs_n;
+    const int packs = (C + 1) / 2;
+    const unsigned split_blocks = (unsigned)((pl->Lp / 2 + 1 + GL_THREADS - 1) / GL_THREADS);
+    GlArgs a;
+    int group = 0;
+    int rc = gl_setup(h, pl, packs > n_pairs ? packs : n_pairs, 2 * stride, 0, a, group);
+    a.spec = w.spec;
+    a.quiet = w.quiet;
+    a.n_ch = C;
+    // phase 1: channels 2q and 2q+1 packed as d0 + j d1 (row stride 2 * stride); an odd last channel is
+    // packed with the zero row, in a group of its own
+    a.per_channel = 1;
+    for (int q0 = 0; q0 < packs && rc == FRT_OK; q0 += group) {
+        int np = packs - q0 < group ? packs - q0 : group;
+        const bool odd_last = (C & 1) && q0 + np == packs;
+        if (odd_last) np--;
+        for (int part = 0; part < 2 && rc == FRT_OK; part++) {
+            if (part == 1 && !odd_last) break;
+            const int qa = part == 0 ? q0 : packs - 1, nq = part == 0 ? np : 1;
+            if (nq == 0) continue;
+            a.ch0 = 2 * qa;
+            a.d0 = x_dev + (size_t)a.ch0 * stride;
+            a.d1 = part == 0 ? a.d0 + stride : w.zero;
+            rc = gl_forward(h, pl, a, nq, st);
+            if (rc == FRT_OK) rc = frt_launch(h, gl_split_spec, dim3(split_blocks, nq), GL_THREADS, 0, st, a);
+        }
+    }
+    // phase 2: the table's entries in groups; d0 / d1 are not read
+    a.per_channel = 0;
+    a.have_prev = have_prev;
+    a.d0 = a.d1 = x_dev;
+    for (int p0 = 0; p0 < n_pairs && rc == FRT_OK; p0 += group) {
+        const int np = n_pairs - p0 < group ? n_pairs - p0 : group;
+        a.pairs = h->gcc_pairs.get() + p0;
+        gl_outputs(pl, a, p0, xcorr_dev, smoothed_dev, idx_dev, val_dev);
+        rc = frt_launch(h, gl_pair_state, (np + 255) / 256, 256, 0, st, a, np);
+        if (rc == FRT_OK) rc = frt_launch(h, gl_cross, dim3(split_blocks, np), GL_THREADS, 0, st, a);
+        if (rc == FRT_OK) rc = gl_inverse(h, pl, a, np, st);
+    }
+    return rc;
 }

@@ -190,6 +190,138 @@ struct GccArgs {
     GccRadices rd;
 };
 
+// The device steps of one pair, shared by gcc_phat_kernel (rows d0, d1 of independent pairs) and
+// the two phases of frt_gcc_phat_pairs (gcc_spectra_kernel, gcc_pairs_kernel).
+
+// Loads two rows into z as d0 + j d1 and returns their means and spans (max - min); a span that is
+// not > 0 marks a constant row, which the reference skips (delay_estimator.py:129-131).
+__device__ __forceinline__ void gcc_load(float2 *z, const float *d0, const float *d1, int L, float *s_red,
+                                         float &m0, float &m1, float &span0, float &span1) {
+    const int tid = threadIdx.x, nt = blockDim.x;
+    float s0 = 0.f, s1 = 0.f, mn0 = INFINITY, mx0 = -INFINITY, mn1 = INFINITY, mx1 = -INFINITY;
+    for (int n = tid; n < L; n += nt) {
+        const float u = __ldg(d0 + n), v = __ldg(d1 + n);
+        z[n] = make_float2(u, v);
+        s0 += u;
+        s1 += v;
+        mn0 = fminf(mn0, u); mx0 = fmaxf(mx0, u);
+        mn1 = fminf(mn1, v); mx1 = fmaxf(mx1, v);
+    }
+    m0 = block_sum(s0, s_red) / (float)L;
+    m1 = block_sum(s1, s_red) / (float)L;
+    span0 = block_max(mx0, s_red) + block_max(-mn0, s_red);
+    span1 = block_max(mx1, s_red) + block_max(-mn1, s_red);
+}
+
+// Outputs of a pair with a constant input: (0, 0), a zero Xcorr, the smoothed row left alone.
+__device__ __forceinline__ void gcc_silent(int pair, int L, float *xcorr, float *smoothed, int have_prev,
+                                           int *idx, float *val) {
+    const int tid = threadIdx.x, nt = blockDim.x;
+    if (tid == 0) {
+        idx[pair] = 0;
+        val[pair] = 0.f;
+    }
+    if (xcorr)
+        for (int n = tid; n < L; n += nt) xcorr[(size_t)pair * L + n] = 0.f;
+    // the reference leaves old_Xcorr alone on a silent frame (delay_estimator.py:129-131,162-165);
+    // on the very first call there is none yet: mark the pair "no previous" (NaN in slot 0)
+    if (smoothed && have_prev == 0 && tid == 0) smoothed[(size_t)pair * L] = nanf("");
+    __syncthreads();
+}
+
+// From this thread's slice g of G[k], k = tid + i * blockDim.x <= L/2, and its max |G|: the PHAT
+// weighting and the inverse transform, x[n] = Re(FFT(conj Yfull))[n] / L at z[perm[n]].
+__device__ __forceinline__ void gcc_inverse(float2 *z, const float2 (&g)[GCC_MAX_PER_THREAD], float gmax,
+                                            int L, float *s_red, const GccRadices &rd,
+                                            const float2 *__restrict__ tw) {
+    const int tid = threadIdx.x, nt = blockDim.x, half = L / 2;
+    const float m = block_max(gmax, s_red);   // also orders the reads of z before the writes below
+    const float floor_ = 1e-10f * m;
+#pragma unroll
+    for (int i = 0; i < GCC_MAX_PER_THREAD; i++) {
+        const int k = tid + i * nt;
+        if (k <= half) {
+            const float ag = sqrtf(g[i].x * g[i].x + g[i].y * g[i].y);
+            const float w = 1.0f / (floor_ + ag);
+            float2 y = make_float2(g[i].x * w, g[i].y * w);
+            if (k == 0 || k == half) y.y = 0.f;          // irfft ignores these imaginary parts
+            // second FFT runs on conj(Y): x = Re(FFT(conj Y)) / L
+            z[k] = make_float2(y.x, -y.y);
+            if (k != 0 && k != half) z[L - k] = y;        // Y[L-k] = conj(Y[k])
+        }
+    }
+    __syncthreads();
+    fft_inplace(z, L, rd, tw, nullptr, 0.f, 0.f);
+}
+
+// Smoothing (delay_estimator.py:134-139) and arg-max of |Xs| (first maximum wins) of the inverse
+// transform in z; writes the pair's Xcorr, smoothed row, idx and val.
+__device__ __forceinline__ void gcc_finish(const float2 *z, int L, const int *__restrict__ perm, int pair,
+                                           float *xcorr, float *smoothed, int have_prev, int *idx,
+                                           float *val, float *s_red, int *s_idx) {
+    const int tid = threadIdx.x, nt = blockDim.x;
+    const float inv = 1.0f / (float)L;
+    float best = -1.f;
+    int besti = 0x7fffffff;
+    float *sm = smoothed ? smoothed + (size_t)pair * L : nullptr;
+    float *xc = xcorr ? xcorr + (size_t)pair * L : nullptr;
+    // have_prev: 1 = every pair has a previous smoothed frame; 2 = per pair, a NaN in slot 0
+    // marks a pair that has had only silent frames so far (old_Xcorr is None there)
+    bool prev = have_prev == 1;
+    if (sm && have_prev == 2) prev = !isnan(sm[0]);
+    __syncthreads();     // everyone has read the marker before slot 0 is rewritten
+    for (int n = tid; n < L; n += nt) {
+        float v = z[__ldg(perm + n)].x * inv;
+        if (xc) xc[n] = v;
+        if (sm) {
+            if (prev) v = 0.3f * v + 0.7f * sm[n];
+            sm[n] = v;
+        }
+        const float av = fabsf(v);
+        if (av > best) {
+            best = av;
+            besti = n;
+        }
+    }
+    // block arg-max
+    for (int o = 16; o > 0; o >>= 1) {
+        const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+        const int oi = __shfl_xor_sync(0xffffffffu, besti, o);
+        if (ob > best || (ob == best && oi < besti)) {
+            best = ob;
+            besti = oi;
+        }
+    }
+    __syncthreads();
+    if ((tid & 31) == 0) {
+        s_red[tid >> 5] = best;
+        s_idx[tid >> 5] = besti;
+    }
+    __syncthreads();
+    if (tid < 32) {
+        best = (tid < (nt >> 5)) ? s_red[tid] : -1.f;
+        besti = (tid < (nt >> 5)) ? s_idx[tid] : 0x7fffffff;
+        for (int o = 16; o > 0; o >>= 1) {
+            const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+            const int oi = __shfl_xor_sync(0xffffffffu, besti, o);
+            if (ob > best || (ob == best && oi < besti)) {
+                best = ob;
+                besti = oi;
+            }
+        }
+        if (tid == 0) s_idx[32] = besti;
+    }
+    __syncthreads();
+    if (tid == 0) {
+        const int bi = s_idx[32];
+        float v = z[__ldg(perm + bi)].x * inv;
+        if (sm) v = sm[bi];
+        idx[pair] = bi;
+        val[pair] = v;
+    }
+    __syncthreads();
+}
+
 __global__ void __launch_bounds__(GCC_THREADS, 1) gcc_phat_kernel(const GccArgs a) {
     extern __shared__ float2 z[];
     __shared__ float s_red[40];
@@ -197,33 +329,11 @@ __global__ void __launch_bounds__(GCC_THREADS, 1) gcc_phat_kernel(const GccArgs 
     const int L = a.L, half = L / 2;
     const int tid = threadIdx.x, nt = blockDim.x;
     for (int pair = blockIdx.x; pair < a.n_pairs; pair += gridDim.x) {
-        const float *d0 = a.d0 + (size_t)pair * a.stride;
-        const float *d1 = a.d1 + (size_t)pair * a.stride;
-        // means; constant inputs (std == 0) are skipped by the reference (delay_estimator.py:129-131)
-        float s0 = 0.f, s1 = 0.f, mn0 = INFINITY, mx0 = -INFINITY, mn1 = INFINITY, mx1 = -INFINITY;
-        for (int n = tid; n < L; n += nt) {
-            const float u = __ldg(d0 + n), v = __ldg(d1 + n);
-            z[n] = make_float2(u, v);
-            s0 += u;
-            s1 += v;
-            mn0 = fminf(mn0, u); mx0 = fmaxf(mx0, u);
-            mn1 = fminf(mn1, v); mx1 = fmaxf(mx1, v);
-        }
-        const float m0 = block_sum(s0, s_red) / (float)L;
-        const float m1 = block_sum(s1, s_red) / (float)L;
-        const float span0 = block_max(mx0, s_red) + block_max(-mn0, s_red);
-        const float span1 = block_max(mx1, s_red) + block_max(-mn1, s_red);
+        float m0, m1, span0, span1;
+        gcc_load(z, a.d0 + (size_t)pair * a.stride, a.d1 + (size_t)pair * a.stride, L, s_red, m0, m1, span0,
+                 span1);
         if (!(span0 > 0.f) || !(span1 > 0.f)) {
-            if (tid == 0) {
-                a.idx[pair] = 0;
-                a.val[pair] = 0.f;
-            }
-            if (a.xcorr)
-                for (int n = tid; n < L; n += nt) a.xcorr[(size_t)pair * L + n] = 0.f;
-            // the reference leaves old_Xcorr alone on a silent frame (delay_estimator.py:129-131,162-165);
-            // on the very first call there is none yet: mark the pair "no previous" (NaN in slot 0)
-            if (a.smoothed && a.have_prev == 0 && tid == 0) a.smoothed[(size_t)pair * L] = nanf("");
-            __syncthreads();
+            gcc_silent(pair, L, a.xcorr, a.smoothed, a.have_prev, a.idx, a.val);
             continue;
         }
         fft_inplace(z, L, a.rd, a.tw, a.window, m0, m1);   // mean removal + window fused in
@@ -236,94 +346,103 @@ __global__ void __launch_bounds__(GCC_THREADS, 1) gcc_phat_kernel(const GccArgs 
             const int k = tid + i * nt;
             g[i] = make_float2(0.f, 0.f);
             if (k <= half) {
-                const float2 zk = z[__ldg(a.perm + k)];
-                const float2 zm = z[__ldg(a.perm + (k == 0 ? 0 : L - k))];
-                // D0 = (Zk + conj Zm)/2 ; D1 = (Zk - conj Zm)/(2j)
-                const float2 D0 = make_float2(0.5f * (zk.x + zm.x), 0.5f * (zk.y - zm.y));
-                const float2 D1 = make_float2(0.5f * (zk.y + zm.y), -0.5f * (zk.x - zm.x));
-                g[i] = make_float2(D0.x * D1.x + D0.y * D1.y, D0.x * D1.y - D0.y * D1.x);
+                float2 D0, D1;
+                split_packed(z[__ldg(a.perm + k)], z[__ldg(a.perm + (k == 0 ? 0 : L - k))], D0, D1);
+                g[i] = cross_spectrum(D0, D1);
                 gmax = fmaxf(gmax, sqrtf(g[i].x * g[i].x + g[i].y * g[i].y));
             }
         }
-        const float m = block_max(gmax, s_red);   // also orders the reads above before the writes below
-        const float floor_ = 1e-10f * m;
+        gcc_inverse(z, g, gmax, L, s_red, a.rd, a.tw);
+        gcc_finish(z, L, a.perm, pair, a.xcorr, a.smoothed, a.have_prev, a.idx, a.val, s_red, s_idx);
+    }
+}
+
+// ---- frt_gcc_phat_pairs on the shared-memory route.  Phase 1: one CTA per two channels (2q, 2q+1;
+// an odd last channel is packed with a zero row) transforms them with one complex FFT, exactly as
+// gcc_phat_kernel transforms a pair, and stores both spectra D_c[k], k = 0..L/2, and whether each
+// channel is constant.  Phase 2: one CTA per table entry (i, j) forms G = conj(D_i) D_j and runs
+// gcc_phat_kernel's PHAT weighting, inverse transform, smoothing and peak pick.
+struct GccSpecArgs {
+    const float *x;            // channel c at x[c*stride + n]
+    long long stride;
+    int n_channels, L;
+    const float *zero;         // [L] zeros: the partner of an odd last channel
+    const float *window;
+    const float2 *tw;
+    const int *perm;
+    float2 *spec;              // [n_channels][L/2+1] D_c
+    int *quiet;                // [n_channels] 1 = constant channel
+    GccRadices rd;
+};
+
+__global__ void __launch_bounds__(GCC_THREADS, 1) gcc_spectra_kernel(const GccSpecArgs a) {
+    extern __shared__ float2 z[];
+    __shared__ float s_red[40];
+    const int L = a.L, H = L / 2 + 1;
+    const int tid = threadIdx.x, nt = blockDim.x;
+    for (int q = blockIdx.x; 2 * q < a.n_channels; q += gridDim.x) {
+        const int c0 = 2 * q, c1 = 2 * q + 1;
+        const bool has1 = c1 < a.n_channels;
+        float m0, m1, span0, span1;
+        gcc_load(z, a.x + (size_t)c0 * a.stride, has1 ? a.x + (size_t)c1 * a.stride : a.zero, L, s_red, m0, m1,
+                 span0, span1);
+        const bool quiet0 = !(span0 > 0.f), quiet1 = !(span1 > 0.f);
+        if (tid == 0) {
+            a.quiet[c0] = quiet0;
+            if (has1) a.quiet[c1] = quiet1;
+        }
+        if (quiet0 && quiet1) continue;   // gcc_load's reductions ordered every read of z
+        fft_inplace(z, L, a.rd, a.tw, a.window, m0, m1);
+        for (int k = tid; k < H; k += nt) {
+            float2 D0, D1;
+            split_packed(z[__ldg(a.perm + k)], z[__ldg(a.perm + (k == 0 ? 0 : L - k))], D0, D1);
+            a.spec[(size_t)c0 * H + k] = D0;
+            if (has1) a.spec[(size_t)c1 * H + k] = D1;
+        }
+        __syncthreads();
+    }
+}
+
+struct GccPairArgs {
+    const int2 *pairs;         // [n_pairs] (i, j): G = conj(D_i) D_j
+    int n_pairs, L;
+    const float2 *spec;
+    const int *quiet;
+    const float2 *tw;
+    const int *perm;
+    float *xcorr, *smoothed;
+    int have_prev;
+    int *idx;
+    float *val;
+    GccRadices rd;
+};
+
+__global__ void __launch_bounds__(GCC_THREADS, 1) gcc_pairs_kernel(const GccPairArgs a) {
+    extern __shared__ float2 z[];
+    __shared__ float s_red[40];
+    __shared__ int s_idx[33];
+    const int L = a.L, half = L / 2, H = half + 1;
+    const int tid = threadIdx.x, nt = blockDim.x;
+    for (int pair = blockIdx.x; pair < a.n_pairs; pair += gridDim.x) {
+        const int2 ij = __ldg(a.pairs + pair);
+        if (__ldg(a.quiet + ij.x) || __ldg(a.quiet + ij.y)) {
+            gcc_silent(pair, L, a.xcorr, a.smoothed, a.have_prev, a.idx, a.val);
+            continue;
+        }
+        const float2 *Di = a.spec + (size_t)ij.x * H, *Dj = a.spec + (size_t)ij.y * H;
+        float2 g[GCC_MAX_PER_THREAD];
+        float gmax = 0.f;
 #pragma unroll
         for (int i = 0; i < GCC_MAX_PER_THREAD; i++) {
             const int k = tid + i * nt;
+            g[i] = make_float2(0.f, 0.f);
             if (k <= half) {
-                const float ag = sqrtf(g[i].x * g[i].x + g[i].y * g[i].y);
-                const float w = 1.0f / (floor_ + ag);
-                float2 y = make_float2(g[i].x * w, g[i].y * w);
-                if (k == 0 || k == half) y.y = 0.f;          // irfft ignores these imaginary parts
-                // second FFT runs on conj(Y): x = Re(FFT(conj Y)) / L
-                z[k] = make_float2(y.x, -y.y);
-                if (k != 0 && k != half) z[L - k] = y;        // Y[L-k] = conj(Y[k])
+                g[i] = cross_spectrum(Di[k], Dj[k]);
+                gmax = fmaxf(gmax, sqrtf(g[i].x * g[i].x + g[i].y * g[i].y));
             }
         }
-        __syncthreads();
-        fft_inplace(z, L, a.rd, a.tw, nullptr, 0.f, 0.f);
-
-        // smoothing (delay_estimator.py:134-139) and arg-max of |Xs| (first maximum wins)
-        const float inv = 1.0f / (float)L;
-        float best = -1.f;
-        int besti = 0x7fffffff;
-        float *sm = a.smoothed ? a.smoothed + (size_t)pair * L : nullptr;
-        float *xc = a.xcorr ? a.xcorr + (size_t)pair * L : nullptr;
-        // have_prev: 1 = every pair has a previous smoothed frame; 2 = per pair, a NaN in slot 0
-        // marks a pair that has had only silent frames so far (old_Xcorr is None there)
-        bool prev = a.have_prev == 1;
-        if (sm && a.have_prev == 2) prev = !isnan(sm[0]);
-        __syncthreads();     // everyone has read the marker before slot 0 is rewritten
-        for (int n = tid; n < L; n += nt) {
-            float v = z[__ldg(a.perm + n)].x * inv;
-            if (xc) xc[n] = v;
-            if (sm) {
-                if (prev) v = 0.3f * v + 0.7f * sm[n];
-                sm[n] = v;
-            }
-            const float av = fabsf(v);
-            if (av > best) {
-                best = av;
-                besti = n;
-            }
-        }
-        // block arg-max
-        for (int o = 16; o > 0; o >>= 1) {
-            const float ob = __shfl_xor_sync(0xffffffffu, best, o);
-            const int oi = __shfl_xor_sync(0xffffffffu, besti, o);
-            if (ob > best || (ob == best && oi < besti)) {
-                best = ob;
-                besti = oi;
-            }
-        }
-        __syncthreads();
-        if ((tid & 31) == 0) {
-            s_red[tid >> 5] = best;
-            s_idx[tid >> 5] = besti;
-        }
-        __syncthreads();
-        if (tid < 32) {
-            best = (tid < (nt >> 5)) ? s_red[tid] : -1.f;
-            besti = (tid < (nt >> 5)) ? s_idx[tid] : 0x7fffffff;
-            for (int o = 16; o > 0; o >>= 1) {
-                const float ob = __shfl_xor_sync(0xffffffffu, best, o);
-                const int oi = __shfl_xor_sync(0xffffffffu, besti, o);
-                if (ob > best || (ob == best && oi < besti)) {
-                    best = ob;
-                    besti = oi;
-                }
-            }
-            if (tid == 0) s_idx[32] = besti;
-        }
-        __syncthreads();
-        if (tid == 0) {
-            const int bi = s_idx[32];
-            float v = z[__ldg(a.perm + bi)].x * inv;
-            if (sm) v = sm[bi];
-            a.idx[pair] = bi;
-            a.val[pair] = v;
-        }
-        __syncthreads();
+        gcc_inverse(z, g, gmax, L, s_red, a.rd, a.tw);
+        gcc_finish(z, L, a.perm, pair, a.xcorr, a.smoothed, a.have_prev, a.idx, a.val, s_red, s_idx);
     }
 }
 
@@ -448,4 +567,107 @@ extern "C" int frt_gcc_phat(frt_handle h, const float *d0_dev, const float *d1_d
     a.rd = pl->rd;
     int blocks = n_pairs < h->sm_count ? n_pairs : h->sm_count;
     return frt_launch(h, gcc_phat_kernel, blocks, GCC_THREADS, sizeof(float2) * pl->L, (cudaStream_t)stream, a);
+}
+
+extern "C" int frt_gcc_set_pairs(frt_handle h, int n_channels, const int *pairs_host, int n_pairs) {
+    if (!h) return FRT_EINVAL;
+    FRT_CHECK_ARG(h, n_channels >= 1, "n_channels must be >= 1");
+    FRT_CHECK_ARG(h, n_pairs >= 0, "negative n_pairs");
+    FRT_CHECK_ARG(h, n_pairs == 0 || pairs_host, "NULL pair table");
+    for (int p = 0; p < 2 * n_pairs; p++)
+        if (pairs_host[p] < 0 || pairs_host[p] >= n_channels)
+            return frt_fail(h, FRT_EINVAL, "pair %d: channel %d outside 0 .. %d", p / 2, pairs_host[p],
+                            n_channels - 1);
+    DeviceGuard g(h->device);
+    DeviceArray<int2> table;
+    if (n_pairs > 0) {
+        std::vector<int2> t(n_pairs);
+        for (int p = 0; p < n_pairs; p++) t[p] = make_int2(pairs_host[2 * p], pairs_host[2 * p + 1]);
+        FRT_CUDA(h, table.upload(t));
+    } else {
+        FRT_CUDA(h, cudaDeviceSynchronize());   // no queued call still reads the table freed below
+    }
+    h->gcc_pairs = std::move(table);
+    h->gcc_pairs_n = n_pairs;
+    h->gcc_pairs_channels = n_channels;
+    return FRT_OK;
+}
+
+// The spectrum workspace of frt_gcc_phat_pairs: [C][H] float2 spectra, [C] int flags, and an L-float
+// zero row when C is odd.  Grow-only; a failed allocation is FRT_ENOMEM and leaves the handle usable.
+static int gcc_spectra_workspace(frt_ctx *h, int L, int H, GccSpectra &w) {
+    const size_t C = (size_t)h->gcc_pairs_channels;
+    auto up = [](size_t b) { return (b + 255) & ~size_t(255); };
+    const size_t o_quiet = up(C * H * sizeof(float2)), o_zero = o_quiet + up(C * sizeof(int));
+    const size_t bytes = o_zero + ((C & 1) ? (size_t)L * sizeof(float) : 0);
+    const cudaError_t e = h->gcc_spec_ws.grow(bytes);
+    if (e == cudaErrorMemoryAllocation) {
+        cudaGetLastError();
+        return frt_fail(h, FRT_ENOMEM, "the spectra of %zu channels (%zu bytes) do not fit", C, bytes);
+    }
+    FRT_CUDA(h, e);
+    unsigned char *ws = h->gcc_spec_ws.get();
+    w.spec = (float2 *)ws;
+    w.quiet = (int *)(ws + o_quiet);
+    w.zero = (C & 1) ? (float *)(ws + o_zero) : nullptr;
+    return FRT_OK;
+}
+
+extern "C" int frt_gcc_phat_pairs(frt_handle h, const float *x_dev, int64_t stride, float *xcorr_dev,
+                                  float *smoothed_dev, int have_prev, int *idx_dev, float *val_dev,
+                                  void *stream) {
+    if (!h) return FRT_EINVAL;
+    if (h->gcc_pairs_n < 0) return frt_fail(h, FRT_ESTATE, "frt_gcc_phat_pairs: call frt_gcc_set_pairs first");
+    if (!(h->gcc_long_route ? (bool)h->gcc_long : (bool)h->gcc))
+        return frt_fail(h, FRT_ESTATE, "frt_gcc_phat_pairs: call frt_gcc_plan first");
+    DeviceGuard g(h->device);
+    const int L = h->gcc_long_route ? gcc_long_length(h) : h->gcc->L;
+    FRT_CHECK_ARG(h, stride >= L, "stride smaller than the frame length");
+    const int n_pairs = h->gcc_pairs_n;
+    if (n_pairs == 0) return FRT_OK;
+    FRT_CHECK_ARG(h, x_dev && idx_dev && val_dev, "NULL buffer");
+    FRT_CHECK_ARG(h, have_prev >= 0 && have_prev <= 2, "have_prev must be 0, 1 or 2");
+    FRT_CHECK_ARG(h, !have_prev || smoothed_dev, "have_prev needs the smoothed buffer");
+    const cudaStream_t st = (cudaStream_t)stream;
+    const int Lp = L - (L & 1);
+    GccSpectra w;
+    int rc = gcc_spectra_workspace(h, L, Lp / 2 + 1, w);
+    if (rc != FRT_OK) return rc;
+    if (w.zero) FRT_CUDA(h, cudaMemsetAsync(w.zero, 0, sizeof(float) * L, st));
+    if (h->gcc_long_route)
+        return gcc_long_phat_pairs(h, x_dev, stride, w, xcorr_dev, smoothed_dev, have_prev, idx_dev, val_dev, st);
+    const GccPlan *pl = h->gcc.get();
+    const int C = h->gcc_pairs_channels;
+    GccSpecArgs s;
+    s.x = x_dev;
+    s.stride = stride;
+    s.n_channels = C;
+    s.L = L;
+    s.zero = w.zero;
+    s.window = pl->window.get();
+    s.tw = pl->tw.get();
+    s.perm = pl->perm.get();
+    s.spec = w.spec;
+    s.quiet = w.quiet;
+    s.rd = pl->rd;
+    const int packs = (C + 1) / 2;
+    rc = frt_launch(h, gcc_spectra_kernel, packs < h->sm_count ? packs : h->sm_count, GCC_THREADS,
+                    sizeof(float2) * L, st, s);
+    if (rc != FRT_OK) return rc;
+    GccPairArgs a;
+    a.pairs = h->gcc_pairs.get();
+    a.n_pairs = n_pairs;
+    a.L = L;
+    a.spec = w.spec;
+    a.quiet = w.quiet;
+    a.tw = pl->tw.get();
+    a.perm = pl->perm.get();
+    a.xcorr = xcorr_dev;
+    a.smoothed = smoothed_dev;
+    a.have_prev = have_prev;
+    a.idx = idx_dev;
+    a.val = val_dev;
+    a.rd = pl->rd;
+    return frt_launch(h, gcc_pairs_kernel, n_pairs < h->sm_count ? n_pairs : h->sm_count, GCC_THREADS,
+                      sizeof(float2) * L, st, a);
 }

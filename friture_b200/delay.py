@@ -9,7 +9,7 @@ import numpy as np
 from . import _lib, filter_data
 from ._lib import Handle
 from .audioproc import SAMPLING_RATE
-from .correlation import GccPhat
+from .correlation import GccPhat, PairGccPhat
 from .stream import StreamFramer
 
 DEFAULT_DELAYRANGE = 1   # seconds, friture/delay_estimator.py:31
@@ -45,47 +45,27 @@ class Decimator:
         return out
 
 
-class DelayEstimator:
-    """Per pair (channel 0 vs channel 1 of each stream): push 48 kHz chunks, get the delay."""
+class _DelayWidget:
+    """What the widget's numeric part shares between the pair and the channel-array estimators: the
+    frame geometry of a delay range and the published values."""
 
-    def __init__(self, n_pairs, delayrange_s=DEFAULT_DELAYRANGE, device=None):
+    def _setup_range(self, delayrange_s, device):
         import torch
         self.device = torch.device("cuda", _lib.device_index(device))
-        self.n_pairs = int(n_pairs)
         self.Ndec = 2                                                    # delay_estimator.py:52
         self.subsampled_sampling_rate = SAMPLING_RATE / 2 ** self.Ndec   # :53
         self.delayrange_s = delayrange_s
         self.length = int(2 * delayrange_s * self.subsampled_sampling_rate)   # :114-115
         self.needed = int(0.5 * self.length)                                 # :116-117
-        self.dec0 = Decimator(n_pairs, self.Ndec, self.device)
-        self.dec1 = Decimator(n_pairs, self.Ndec, self.device)
         # a frame and its successor's hop, plus room for a few chunks; the framers grow when a
         # longer chunk arrives (the default capacity, 4 L + 64 hops, is 3.5 GB per pair at 1000 s)
-        capacity = 2 * self.length + 4096
-        self.fr0 = StreamFramer(n_pairs, self.length, self.needed, self.device, capacity=capacity,
-                                pre_increment=True)
-        self.fr1 = StreamFramer(n_pairs, self.length, self.needed, self.device, capacity=capacity,
-                                pre_increment=True)
-        self.gcc = GccPhat(self.length, handle=self.dec0.handle, fs=self.subsampled_sampling_rate)
+        self.capacity = 2 * self.length + 4096
+
+    def _setup_outputs(self, n_pairs):
         self.delay_ms = np.zeros(n_pairs)
         self.distance_m = np.zeros(n_pairs)
         self.correlation = np.zeros(n_pairs, dtype=int)
         self.Xcorr_extremum = np.zeros(n_pairs)
-
-    def handle_new_data(self, x0, x1):
-        """x0, x1: CUDA float32 [n_pairs, n] chunks of the two channels at 48 kHz."""
-        d0 = self.dec0.process(x0)
-        d1 = self.dec1.process(x1)
-        self.fr0.push(d0)
-        self.fr1.push(d1)
-        v0, r = self.fr0.take()
-        v1, _ = self.fr1.take()
-        for i in range(r):
-            a = v0[:, i * self.needed:i * self.needed + self.length]
-            b = v1[:, i * self.needed:i * self.needed + self.length]
-            idx, val, xc = self.gcc.estimate(a, b, smooth=True, want_xcorr=False)
-            self._publish(idx, val)
-        return r
 
     def _publish(self, idx, val):
         import torch
@@ -104,3 +84,61 @@ class DelayEstimator:
         x = (norm > 1.) * (norm - 1.)                                      # :173-176
         x = (0.12 * x) ** 3
         self.correlation = ((x / (1. + x)) * 100).astype(int)
+
+
+class DelayEstimator(_DelayWidget):
+    """Per pair (channel 0 vs channel 1 of each stream): push 48 kHz chunks, get the delay."""
+
+    def __init__(self, n_pairs, delayrange_s=DEFAULT_DELAYRANGE, device=None):
+        self._setup_range(delayrange_s, device)
+        self.n_pairs = int(n_pairs)
+        self.dec0 = Decimator(n_pairs, self.Ndec, self.device)
+        self.dec1 = Decimator(n_pairs, self.Ndec, self.device)
+        self.fr0 = StreamFramer(n_pairs, self.length, self.needed, self.device, capacity=self.capacity,
+                                pre_increment=True)
+        self.fr1 = StreamFramer(n_pairs, self.length, self.needed, self.device, capacity=self.capacity,
+                                pre_increment=True)
+        self.gcc = GccPhat(self.length, handle=self.dec0.handle, fs=self.subsampled_sampling_rate)
+        self._setup_outputs(n_pairs)
+
+    def handle_new_data(self, x0, x1):
+        """x0, x1: CUDA float32 [n_pairs, n] chunks of the two channels at 48 kHz."""
+        d0 = self.dec0.process(x0)
+        d1 = self.dec1.process(x1)
+        self.fr0.push(d0)
+        self.fr1.push(d1)
+        v0, r = self.fr0.take()
+        v1, _ = self.fr1.take()
+        for i in range(r):
+            a = v0[:, i * self.needed:i * self.needed + self.length]
+            b = v1[:, i * self.needed:i * self.needed + self.length]
+            idx, val, xc = self.gcc.estimate(a, b, smooth=True, want_xcorr=False)
+            self._publish(idx, val)
+        return r
+
+
+class ArrayDelayEstimator(_DelayWidget):
+    """Delays between channels of one multichannel stream: for every entry (i, j) of ``pairs``,
+    channel i is the widget's channel 0 and channel j its channel 1.  Push [C, n] chunks at 48 kHz;
+    each channel is decimated, framed and transformed once.  ``delay_ms``, ``distance_m``,
+    ``correlation`` and ``Xcorr_extremum`` are indexed by pair, as ``DelayEstimator``'s are."""
+
+    def __init__(self, n_channels, pairs, delayrange_s=DEFAULT_DELAYRANGE, device=None):
+        self._setup_range(delayrange_s, device)
+        self.n_channels = int(n_channels)
+        self.dec = Decimator(self.n_channels, self.Ndec, self.device)
+        self.fr = StreamFramer(self.n_channels, self.length, self.needed, self.device, capacity=self.capacity,
+                               pre_increment=True)
+        self.gcc = PairGccPhat(self.length, self.n_channels, pairs, handle=self.dec.handle,
+                               fs=self.subsampled_sampling_rate)
+        self.n_pairs = self.gcc.n_pairs
+        self._setup_outputs(self.n_pairs)
+
+    def handle_new_data(self, x):
+        """x: CUDA float32 [n_channels, n] chunk at 48 kHz.  Returns the number of frames run."""
+        self.fr.push(self.dec.process(x))
+        v, r = self.fr.take()
+        for i in range(r):
+            idx, val, _ = self.gcc.estimate(v[:, i * self.needed:i * self.needed + self.length], smooth=True)
+            self._publish(idx, val)
+        return r

@@ -223,6 +223,21 @@ int frt_gcc_phat(frt_handle h, const float *d0_dev, const float *d1_dev, int64_t
 /* 1 when frt_gcc_plan runs `length` on the shared-memory kernel (even, 2^a 3^b 5^c, <= 28160),
  * else 0.  Pure host arithmetic (needs no GPU or handle).                                       */
 int frt_gcc_fits(int length);
+/* Pair table for frt_gcc_phat_pairs: pair p correlates channel pairs_host[2p] (the widget's
+ * channel 0, d0) with channel pairs_host[2p+1] (d1) of an n_channels-row input.  Indices are
+ * checked here (0 <= i, j < n_channels; i == j and repeated pairs are allowed); a refused call
+ * keeps the previous table.  Written between device-wide synchronisations like the other setters. */
+int frt_gcc_set_pairs(frt_handle h, int n_channels, const int *pairs_host, int n_pairs);
+/* GCC-PHAT, smoothing and peak pick of every pair in the table, on x[c*stride + n], c < n_channels,
+ * n < L (the current frt_gcc_plan length).  Outputs, have_prev, silent-pair rules and L' exactly as
+ * frt_gcc_phat, indexed by pair.  Each channel is mean-removed, windowed and transformed once:
+ * channels 2k and 2k+1 share one complex transform (an odd last channel is packed with zeros), so
+ * with the table (0,1), (2,3), ... the outputs are the same bits as frt_gcc_phat(x[0::2], x[1::2]).
+ * The per-channel spectra take a grow-only workspace of about 8 * n_channels * (L'/2+1) bytes;
+ * the Bluestein route also uses frt_gcc_phat's workspace for the transforms.  FRT_ESTATE without a
+ * table or a plan; FRT_ENOMEM when the spectra do not fit on the device (the handle stays usable). */
+int frt_gcc_phat_pairs(frt_handle h, const float *x_dev, int64_t stride, float *xcorr_dev,
+                       float *smoothed_dev, int have_prev, int *idx_dev, float *val_dev, void *stream);
 
 /* ---------------------------------------------------------------- N-fold decimation
  * Stands behind `decimate_multiple(Ndec, bdec, adec, x, zis)` (friture/signal/decimate.py:45-71),
