@@ -56,17 +56,17 @@ class GccPhat:
             P, L = d0.shape
             if L != self.length:
                 raise ValueError("frame length %d != planned %d" % (L, self.length))
-            self.handle.call("frt_gcc_plan", int(L))
-            idx, val, xc, sm, have_prev = self._outputs(P, d0.device, smooth, want_xcorr)
-            self.handle.call("frt_gcc_phat", _lib._ptr(d0), _lib._ptr(d1), int(L), int(P),
-                             _lib._ptr(xc), _lib._ptr(sm), have_prev, _lib._ptr(idx), _lib._ptr(val), sp)
-        if smooth:
-            self._have_prev = True
-        return idx, val, xc
+            return self._call("frt_gcc_phat", P, d0.device, smooth, want_xcorr, sp,
+                              _lib._ptr(d0), _lib._ptr(d1), int(L), int(P))
 
-    def _outputs(self, P, device, smooth, want_xcorr):
-        """The output tensors of a call on P pairs, and the smoothed buffer and ``have_prev`` to pass."""
+    def _call(self, symbol, P, device, smooth, want_xcorr, sp, *inputs, after_plan=None):
+        """Plans the length, runs ``after_plan()`` if given, makes the outputs of P pairs and calls
+        ``symbol(*inputs, xcorr, smoothed, have_prev, idx, val, stream)``; returns (idx, val, xcorr or
+        None)."""
         import torch
+        self.handle.call("frt_gcc_plan", self.length)
+        if after_plan is not None:
+            after_plan()
         Lo = self.out_length
         idx = torch.empty(P, dtype=torch.int32, device=device)
         val = torch.empty(P, dtype=torch.float32, device=device)
@@ -81,7 +81,11 @@ class GccPhat:
             # 2 = per pair: a pair whose frames have all been silent so far has no previous smoothed
             # frame (the kernel marks it), like old_Xcorr = None in the widget
             have_prev = 2 if self._have_prev else 0
-        return idx, val, xc, sm, have_prev
+        self.handle.call(symbol, *inputs, _lib._ptr(xc), _lib._ptr(sm), have_prev, _lib._ptr(idx), _lib._ptr(val),
+                         sp)
+        if smooth:
+            self._have_prev = True
+        return idx, val, xc
 
     def delay_ms(self, idx):
         """Index -> delay in ms, wrapped to +-L/2 (delay_estimator.py:147-152)."""
@@ -133,11 +137,5 @@ class PairGccPhat(GccPhat):
                 raise ValueError("x has %d channels, the pair table %d" % (C, self.n_channels))
             if L != self.length:
                 raise ValueError("frame length %d != planned %d" % (L, self.length))
-            self.handle.call("frt_gcc_plan", int(L))
-            self._sync_table()
-            idx, val, xc, sm, have_prev = self._outputs(self.n_pairs, x.device, smooth, want_xcorr)
-            self.handle.call("frt_gcc_phat_pairs", _lib._ptr(x), x_stride, _lib._ptr(xc), _lib._ptr(sm),
-                             have_prev, _lib._ptr(idx), _lib._ptr(val), sp)
-        if smooth:
-            self._have_prev = True
-        return idx, val, xc
+            return self._call("frt_gcc_phat_pairs", self.n_pairs, x.device, smooth, want_xcorr, sp,
+                              _lib._ptr(x), x_stride, after_plan=self._sync_table)

@@ -155,16 +155,14 @@ using PlanPtr = std::unique_ptr<Plan, PlanDelete>;
 // hold on the Bluestein route of gcc_long.cu.  gcc_long_phat expects the arguments checked.
 std::vector<float> gcc_hanning(int length);   // numpy.hanning(length), evaluated in double
 int gcc_long_plan(frt_ctx *h, int length);
-int gcc_long_length(const frt_ctx *h);        // the planned L; needs h->gcc_long
 int gcc_long_phat(frt_ctx *h, const float *d0_dev, const float *d1_dev, int64_t stride, int n_pairs,
                   float *xcorr_dev, float *smoothed_dev, int have_prev, int *idx_dev, float *val_dev,
                   cudaStream_t st);
-// frt_gcc_phat_pairs: the spectra of the table's n_channels channels, D_c[k] for k = 0..L'/2, whether
-// each channel is constant, and a zero row of L floats when n_channels is odd (else NULL).
+// frt_gcc_phat_pairs: the spectra of the table's n_channels channels, D_c[k] for k = 0..L'/2, and
+// whether each channel is constant.
 struct GccSpectra {
     float2 *spec;
     int *quiet;
-    float *zero;
 };
 int gcc_long_phat_pairs(frt_ctx *h, const float *x_dev, int64_t stride, const GccSpectra &w, float *xcorr_dev,
                         float *smoothed_dev, int have_prev, int *idx_dev, float *val_dev, cudaStream_t st);
@@ -184,6 +182,7 @@ struct frt_ctx {
     PlanPtr<GccPlan> gcc;             // frt_gcc_plan keeps one plan of each route, so that switching
     PlanPtr<GccLongPlan> gcc_long;    // lengths back and forth rebuilds neither
     bool gcc_long_route = false;      // the last accepted frt_gcc_plan length runs on gcc_long
+    int gcc_length = 0;               // that length; 0 before the first accepted plan
     DeviceArray<unsigned char> gcc_long_ws;   // the Bluestein route's workspace, grow-only
     DeviceArray<int2> gcc_pairs;      // frt_gcc_set_pairs: the pair table (i, j) on the device
     int gcc_pairs_n = -1;             // its entries; -1 before the first accepted table

@@ -85,9 +85,9 @@ struct GlArgs {
     int *idx;
     float *val;
     // frt_gcc_phat_pairs.  Phase 1 (a group of packed channel pairs d0 = channel ch0 + 2p, d1 = the next
-    // one): per_channel = 1, so that a pair is skipped only when both channels are constant, and the
-    // spectra and flags of channels < n_ch land in spec / quiet.  Phase 2 (a group of table entries):
-    // pair p correlates channels pairs[p].
+    // one, read as zeros past the last channel): per_channel = 1, so that a pair is skipped only when
+    // both channels are constant, and the spectra and flags of channels < n_ch land in spec / quiet.
+    // Phase 2 (a group of table entries): pair p correlates channels pairs[p].
     int per_channel, ch0, n_ch;
     float2 *spec;              // [n_ch][L'/2+1]
     int *quiet;                // [n_ch]
@@ -100,6 +100,17 @@ __device__ __forceinline__ int brev(int k, int bits) { return (int)(__brev((unsi
 // "no previous" NaN in slot 0.  Read before the last pass rewrites slot 0.
 __device__ __forceinline__ int gl_prev(const GlArgs &a, int pair) {
     return a.have_prev == 1 || (a.have_prev == 2 && !isnan(a.smoothed[(size_t)pair * a.Lp]));
+}
+// Whether the pair has a d1: in phase 1 of frt_gcc_phat_pairs an odd last channel has no partner.
+__device__ __forceinline__ bool gl_has_d1(const GlArgs &a, int pair) {
+    return !a.per_channel || a.ch0 + 2 * pair + 1 < a.n_ch;
+}
+// A pair's state before its transforms: means, constant flags (bit 0: d0, bit 1: d1), whether it is
+// skipped -- in phase 1 of frt_gcc_phat_pairs only when both channels are constant -- and whether it
+// blends with its smoothed row; max|G| and the peak still to come.
+__device__ __forceinline__ void gl_init_state(const GlArgs &a, int pair, float m0, float m1, unsigned quiet) {
+    const int silent = a.per_channel ? quiet == 3u : quiet != 0u;
+    a.st[pair] = PairState{m0, m1, silent, gl_prev(a, pair), 0u, quiet, 0ull};
 }
 __device__ __forceinline__ float2 tw_m(const GlArgs &a, unsigned e) {
     return cmul(__ldg(a.tw_hi + (e >> a.tw_shift)), __ldg(a.tw_lo + (e & ((1u << a.tw_shift) - 1u))));
@@ -187,10 +198,11 @@ __global__ void __launch_bounds__(256) gl_stats(const GlArgs a) {
     __shared__ float s_red[33];
     const int pair = blockIdx.y;
     const float *d0 = a.d0 + (size_t)pair * a.stride, *d1 = a.d1 + (size_t)pair * a.stride;
+    const bool has1 = gl_has_d1(a, pair);
     const int n0 = blockIdx.x * GL_STATS_CHUNK, n1 = min(a.L, n0 + GL_STATS_CHUNK);
     float s0 = 0.f, s1 = 0.f, mn0 = INFINITY, mx0 = -INFINITY, mn1 = INFINITY, mx1 = -INFINITY;
     for (int n = n0 + threadIdx.x; n < n1; n += blockDim.x) {
-        const float u = __ldg(d0 + n), v = __ldg(d1 + n);
+        const float u = __ldg(d0 + n), v = has1 ? __ldg(d1 + n) : 0.f;
         s0 += u;
         s1 += v;
         mn0 = fminf(mn0, u); mx0 = fmaxf(mx0, u);
@@ -217,18 +229,9 @@ __global__ void __launch_bounds__(256) gl_stats_finish(const GlArgs a) {
     const float s0 = block_sum(v[0], s_red), s1 = block_sum(v[1], s_red);
     const float span0 = block_max(v[2], s_red) + block_max(v[3], s_red);
     const float span1 = block_max(v[4], s_red) + block_max(v[5], s_red);
-    if (threadIdx.x == 0) {
-        PairState st;
-        st.m0 = s0 / (float)a.L;
-        st.m1 = s1 / (float)a.L;
-        // constant inputs (std == 0) are skipped by the reference (delay_estimator.py:129-131)
-        st.quiet = (span0 > 0.f ? 0u : 1u) | (span1 > 0.f ? 0u : 2u);
-        st.silent = a.per_channel ? st.quiet == 3u : st.quiet != 0u;
-        st.prev = gl_prev(a, pair);
-        st.gmax = 0u;
-        st.best = 0ull;
-        a.st[pair] = st;
-    }
+    // constant inputs (std == 0) are skipped by the reference (delay_estimator.py:129-131)
+    if (threadIdx.x == 0)
+        gl_init_state(a, pair, s0 / (float)a.L, s1 / (float)a.L, (span0 > 0.f ? 0u : 1u) | (span1 > 0.f ? 0u : 2u));
 }
 
 // ---- column pass of a forward transform.  PHAT = false: the first transform's input
@@ -243,6 +246,7 @@ __global__ void __launch_bounds__(GL_THREADS) gl_cols_fwd(const GlArgs a) {
     const int C = 1 << a.lgc, M1 = 1 << a.log1, sst = M1 + 1;   // +1: columns start in different banks
     const int col0 = blockIdx.x << a.lgc;
     const float *d0 = a.d0 + (size_t)pair * a.stride, *d1 = a.d1 + (size_t)pair * a.stride;
+    const bool has1 = PHAT || gl_has_d1(a, pair);
     const float2 *g = a.g + (size_t)pair * (a.Lp / 2 + 1);
     const int half = a.Lp / 2;
     const float floor_ = 1e-10f * __uint_as_float(st.gmax);
@@ -252,7 +256,8 @@ __global__ void __launch_bounds__(GL_THREADS) gl_cols_fwd(const GlArgs a) {
         float2 v = make_float2(0.f, 0.f);
         if (!PHAT && n < a.L) {
             const float w = __ldg(a.window + n);
-            v = cmul(make_float2((__ldg(d0 + n) - st.m0) * w, (__ldg(d1 + n) - st.m1) * w), __ldg(a.chirp + n));
+            const float u1 = has1 ? __ldg(d1 + n) : 0.f;
+            v = cmul(make_float2((__ldg(d0 + n) - st.m0) * w, (u1 - st.m1) * w), __ldg(a.chirp + n));
         } else if (PHAT && n < a.Lp) {
             const int k = n <= half ? n : a.Lp - n;
             const float2 gk = g[k];
@@ -406,14 +411,7 @@ __global__ void __launch_bounds__(256) gl_pair_state(const GlArgs a, int n_pairs
     const int pair = blockIdx.x * blockDim.x + threadIdx.x;
     if (pair >= n_pairs) return;
     const int2 ij = a.pairs[pair];
-    PairState st;
-    st.m0 = st.m1 = 0.f;
-    st.quiet = (a.quiet[ij.x] ? 1u : 0u) | (a.quiet[ij.y] ? 2u : 0u);
-    st.silent = st.quiet != 0u;
-    st.prev = gl_prev(a, pair);
-    st.gmax = 0u;
-    st.best = 0ull;
-    a.st[pair] = st;
+    gl_init_state(a, pair, 0.f, 0.f, (a.quiet[ij.x] ? 1u : 0u) | (a.quiet[ij.y] ? 2u : 0u));
 }
 
 // ---- phase 2: G = conj(D_i) D_j for k = 0..L'/2 from the stored spectra, and max|G| (as gl_split)
@@ -571,8 +569,6 @@ int gcc_long_plan(frt_ctx *h, int length) {
     return FRT_OK;
 }
 
-int gcc_long_length(const frt_ctx *h) { return h->gcc_long->L; }
-
 // The arguments every pass of a call shares, and its workspace: groups of pairs whose buffers fit
 // GL_WORKSPACE_BUDGET, at most n_pairs.  Returns the group size through `group`.
 static int gl_setup(frt_ctx *h, const GccLongPlan *pl, int n_pairs, int64_t stride, int have_prev, GlArgs &a,
@@ -689,23 +685,16 @@ int gcc_long_phat_pairs(frt_ctx *h, const float *x_dev, int64_t stride, const Gc
     a.spec = w.spec;
     a.quiet = w.quiet;
     a.n_ch = C;
-    // phase 1: channels 2q and 2q+1 packed as d0 + j d1 (row stride 2 * stride); an odd last channel is
-    // packed with the zero row, in a group of its own
+    // phase 1: channels 2q and 2q+1 packed as d0 + j d1 (row stride 2 * stride); the partner of an odd
+    // last channel reads as zeros
     a.per_channel = 1;
     for (int q0 = 0; q0 < packs && rc == FRT_OK; q0 += group) {
-        int np = packs - q0 < group ? packs - q0 : group;
-        const bool odd_last = (C & 1) && q0 + np == packs;
-        if (odd_last) np--;
-        for (int part = 0; part < 2 && rc == FRT_OK; part++) {
-            if (part == 1 && !odd_last) break;
-            const int qa = part == 0 ? q0 : packs - 1, nq = part == 0 ? np : 1;
-            if (nq == 0) continue;
-            a.ch0 = 2 * qa;
-            a.d0 = x_dev + (size_t)a.ch0 * stride;
-            a.d1 = part == 0 ? a.d0 + stride : w.zero;
-            rc = gl_forward(h, pl, a, nq, st);
-            if (rc == FRT_OK) rc = frt_launch(h, gl_split_spec, dim3(split_blocks, nq), GL_THREADS, 0, st, a);
-        }
+        const int np = packs - q0 < group ? packs - q0 : group;
+        a.ch0 = 2 * q0;
+        a.d0 = x_dev + (size_t)a.ch0 * stride;
+        a.d1 = a.d0 + stride;
+        rc = gl_forward(h, pl, a, np, st);
+        if (rc == FRT_OK) rc = frt_launch(h, gl_split_spec, dim3(split_blocks, np), GL_THREADS, 0, st, a);
     }
     // phase 2: the table's entries in groups; d0 / d1 are not read
     a.per_channel = 0;

@@ -12,6 +12,7 @@
 // transform is a second complex FFT of the conjugated Hermitian spectrum.  The FFT is an in-place
 // mixed-radix (4/2/3/5) decimation-in-frequency over the 8*L-byte shared-memory buffer; results
 // are addressed through the mixed-radix digit reversal instead of being permuted.
+#include <algorithm>
 #include <cmath>
 
 #include "frt_internal.cuh"
@@ -175,10 +176,14 @@ static int digit_reverse(int k, int L, const GccRadices &rd) {
     return pos;
 }
 
+// The arguments of the three shared-memory kernels: gcc_args fills the plan's tables and the call's
+// outputs, the entry points add the inputs.  The spectra workspace and the pair table of
+// frt_gcc_phat_pairs are separate kernel parameters: the kernels copy this struct to the stack, and a
+// larger one changes gcc_phat_kernel's code.
 struct GccArgs {
-    const float *d0, *d1;
-    long long stride;
-    int n_pairs, L;
+    const float *d0, *d1;      // pair p: rows d0 + p*stride, d1 + p*stride (gcc_spectra_kernel: pair p
+    long long stride;          // packs channels 2p and 2p+1)
+    int n, L;                  // n: pairs, or channels in gcc_spectra_kernel
     const float *window;       // [L] np.hanning(L)
     const float2 *tw;          // [L] W_L^i
     const int *perm;           // [L] storage position of index k after the in-place DIF passes
@@ -195,12 +200,14 @@ struct GccArgs {
 
 // Loads two rows into z as d0 + j d1 and returns their means and spans (max - min); a span that is
 // not > 0 marks a constant row, which the reference skips (delay_estimator.py:129-131).
+// D1_MAY_BE_NULL: a NULL d1 reads as a row of zeros (mean 0, span 0: a constant row).
+template <bool D1_MAY_BE_NULL = false>
 __device__ __forceinline__ void gcc_load(float2 *z, const float *d0, const float *d1, int L, float *s_red,
                                          float &m0, float &m1, float &span0, float &span1) {
     const int tid = threadIdx.x, nt = blockDim.x;
     float s0 = 0.f, s1 = 0.f, mn0 = INFINITY, mx0 = -INFINITY, mn1 = INFINITY, mx1 = -INFINITY;
     for (int n = tid; n < L; n += nt) {
-        const float u = __ldg(d0 + n), v = __ldg(d1 + n);
+        const float u = __ldg(d0 + n), v = (D1_MAY_BE_NULL && !d1) ? 0.f : __ldg(d1 + n);
         z[n] = make_float2(u, v);
         s0 += u;
         s1 += v;
@@ -328,7 +335,7 @@ __global__ void __launch_bounds__(GCC_THREADS, 1) gcc_phat_kernel(const GccArgs 
     __shared__ int s_idx[33];
     const int L = a.L, half = L / 2;
     const int tid = threadIdx.x, nt = blockDim.x;
-    for (int pair = blockIdx.x; pair < a.n_pairs; pair += gridDim.x) {
+    for (int pair = blockIdx.x; pair < a.n; pair += gridDim.x) {
         float m0, m1, span0, span1;
         gcc_load(z, a.d0 + (size_t)pair * a.stride, a.d1 + (size_t)pair * a.stride, L, s_red, m0, m1, span0,
                  span1);
@@ -358,78 +365,52 @@ __global__ void __launch_bounds__(GCC_THREADS, 1) gcc_phat_kernel(const GccArgs 
 }
 
 // ---- frt_gcc_phat_pairs on the shared-memory route.  Phase 1: one CTA per two channels (2q, 2q+1;
-// an odd last channel is packed with a zero row) transforms them with one complex FFT, exactly as
+// an odd last channel is packed with zeros) transforms them with one complex FFT, exactly as
 // gcc_phat_kernel transforms a pair, and stores both spectra D_c[k], k = 0..L/2, and whether each
 // channel is constant.  Phase 2: one CTA per table entry (i, j) forms G = conj(D_i) D_j and runs
 // gcc_phat_kernel's PHAT weighting, inverse transform, smoothing and peak pick.
-struct GccSpecArgs {
-    const float *x;            // channel c at x[c*stride + n]
-    long long stride;
-    int n_channels, L;
-    const float *zero;         // [L] zeros: the partner of an odd last channel
-    const float *window;
-    const float2 *tw;
-    const int *perm;
-    float2 *spec;              // [n_channels][L/2+1] D_c
-    int *quiet;                // [n_channels] 1 = constant channel
-    GccRadices rd;
-};
-
-__global__ void __launch_bounds__(GCC_THREADS, 1) gcc_spectra_kernel(const GccSpecArgs a) {
+__global__ void __launch_bounds__(GCC_THREADS, 1) gcc_spectra_kernel(const GccArgs a, const GccSpectra w) {
     extern __shared__ float2 z[];
     __shared__ float s_red[40];
     const int L = a.L, H = L / 2 + 1;
     const int tid = threadIdx.x, nt = blockDim.x;
-    for (int q = blockIdx.x; 2 * q < a.n_channels; q += gridDim.x) {
+    for (int q = blockIdx.x; 2 * q < a.n; q += gridDim.x) {
         const int c0 = 2 * q, c1 = 2 * q + 1;
-        const bool has1 = c1 < a.n_channels;
+        const bool has1 = c1 < a.n;
         float m0, m1, span0, span1;
-        gcc_load(z, a.x + (size_t)c0 * a.stride, has1 ? a.x + (size_t)c1 * a.stride : a.zero, L, s_red, m0, m1,
-                 span0, span1);
+        gcc_load<true>(z, a.d0 + (size_t)q * a.stride, has1 ? a.d1 + (size_t)q * a.stride : nullptr, L, s_red, m0,
+                       m1, span0, span1);
         const bool quiet0 = !(span0 > 0.f), quiet1 = !(span1 > 0.f);
         if (tid == 0) {
-            a.quiet[c0] = quiet0;
-            if (has1) a.quiet[c1] = quiet1;
+            w.quiet[c0] = quiet0;
+            if (has1) w.quiet[c1] = quiet1;
         }
         if (quiet0 && quiet1) continue;   // gcc_load's reductions ordered every read of z
         fft_inplace(z, L, a.rd, a.tw, a.window, m0, m1);
         for (int k = tid; k < H; k += nt) {
             float2 D0, D1;
             split_packed(z[__ldg(a.perm + k)], z[__ldg(a.perm + (k == 0 ? 0 : L - k))], D0, D1);
-            a.spec[(size_t)c0 * H + k] = D0;
-            if (has1) a.spec[(size_t)c1 * H + k] = D1;
+            w.spec[(size_t)c0 * H + k] = D0;
+            if (has1) w.spec[(size_t)c1 * H + k] = D1;
         }
         __syncthreads();
     }
 }
 
-struct GccPairArgs {
-    const int2 *pairs;         // [n_pairs] (i, j): G = conj(D_i) D_j
-    int n_pairs, L;
-    const float2 *spec;
-    const int *quiet;
-    const float2 *tw;
-    const int *perm;
-    float *xcorr, *smoothed;
-    int have_prev;
-    int *idx;
-    float *val;
-    GccRadices rd;
-};
-
-__global__ void __launch_bounds__(GCC_THREADS, 1) gcc_pairs_kernel(const GccPairArgs a) {
+__global__ void __launch_bounds__(GCC_THREADS, 1) gcc_pairs_kernel(const GccArgs a, const GccSpectra w,
+                                                                   const int2 *pairs) {
     extern __shared__ float2 z[];
     __shared__ float s_red[40];
     __shared__ int s_idx[33];
     const int L = a.L, half = L / 2, H = half + 1;
     const int tid = threadIdx.x, nt = blockDim.x;
-    for (int pair = blockIdx.x; pair < a.n_pairs; pair += gridDim.x) {
-        const int2 ij = __ldg(a.pairs + pair);
-        if (__ldg(a.quiet + ij.x) || __ldg(a.quiet + ij.y)) {
+    for (int pair = blockIdx.x; pair < a.n; pair += gridDim.x) {
+        const int2 ij = __ldg(pairs + pair);
+        if (__ldg(w.quiet + ij.x) || __ldg(w.quiet + ij.y)) {
             gcc_silent(pair, L, a.xcorr, a.smoothed, a.have_prev, a.idx, a.val);
             continue;
         }
-        const float2 *Di = a.spec + (size_t)ij.x * H, *Dj = a.spec + (size_t)ij.y * H;
+        const float2 *Di = w.spec + (size_t)ij.x * H, *Dj = w.spec + (size_t)ij.y * H;
         float2 g[GCC_MAX_PER_THREAD];
         float gmax = 0.f;
 #pragma unroll
@@ -528,45 +509,66 @@ extern "C" int frt_gcc_plan(frt_handle h, int length) {
     GccRadices rd;
     const bool fits = gcc_rule(length, rd) == nullptr;
     const int rc = fits ? gcc_smem_plan(h, length, rd) : gcc_long_plan(h, length);
-    if (rc == FRT_OK) h->gcc_long_route = !fits;
+    if (rc == FRT_OK) {
+        h->gcc_long_route = !fits;
+        h->gcc_length = length;
+    }
     return rc;
+}
+
+// The checks frt_gcc_phat and frt_gcc_phat_pairs share, after each one's own state checks: a plan,
+// n_pairs, and unless there are no pairs (nothing to do) the buffers (`inputs`: the entry point's
+// input pointers are all set), the row stride and have_prev.  L is the planned length.
+static int gcc_call_checks(frt_ctx *h, const char *fn, int n_pairs, bool inputs, int64_t stride, int have_prev,
+                           const float *smoothed_dev, const int *idx_dev, const float *val_dev, int &L) {
+    L = h->gcc_length;
+    if (L == 0) return frt_fail(h, FRT_ESTATE, "%s: call frt_gcc_plan first", fn);
+    FRT_CHECK_ARG(h, n_pairs >= 0, "negative n_pairs");
+    if (n_pairs == 0) return FRT_OK;
+    FRT_CHECK_ARG(h, inputs && idx_dev && val_dev, "NULL buffer");
+    FRT_CHECK_ARG(h, stride >= L, "stride smaller than the frame length");
+    FRT_CHECK_ARG(h, have_prev >= 0 && have_prev <= 2, "have_prev must be 0, 1 or 2");
+    FRT_CHECK_ARG(h, !have_prev || smoothed_dev, "have_prev needs the smoothed buffer");
+    return FRT_OK;
+}
+
+// The shared-memory kernels' arguments from the plan and the call's outputs; the inputs are left to
+// the caller.
+static GccArgs gcc_args(const GccPlan *pl, float *xcorr_dev, float *smoothed_dev, int have_prev, int *idx_dev,
+                        float *val_dev) {
+    GccArgs a{};
+    a.L = pl->L;
+    a.window = pl->window.get();
+    a.tw = pl->tw.get();
+    a.perm = pl->perm.get();
+    a.rd = pl->rd;
+    a.xcorr = xcorr_dev;
+    a.smoothed = smoothed_dev;
+    a.have_prev = have_prev;
+    a.idx = idx_dev;
+    a.val = val_dev;
+    return a;
 }
 
 extern "C" int frt_gcc_phat(frt_handle h, const float *d0_dev, const float *d1_dev, int64_t stride,
                             int n_pairs, float *xcorr_dev, float *smoothed_dev, int have_prev,
                             int *idx_dev, float *val_dev, void *stream) {
     if (!h) return FRT_EINVAL;
-    if (!(h->gcc_long_route ? (bool)h->gcc_long : (bool)h->gcc))
-        return frt_fail(h, FRT_ESTATE, "frt_gcc_phat: call frt_gcc_plan first");
+    int L;
+    const int rc = gcc_call_checks(h, "frt_gcc_phat", n_pairs, d0_dev && d1_dev, stride, have_prev, smoothed_dev,
+                                   idx_dev, val_dev, L);
+    if (rc != FRT_OK || n_pairs == 0) return rc;
     DeviceGuard g(h->device);
-    const int L = h->gcc_long_route ? gcc_long_length(h) : h->gcc->L;
-    FRT_CHECK_ARG(h, n_pairs >= 0, "negative n_pairs");
-    if (n_pairs == 0) return FRT_OK;
-    FRT_CHECK_ARG(h, d0_dev && d1_dev && idx_dev && val_dev, "NULL buffer");
-    FRT_CHECK_ARG(h, stride >= L, "stride smaller than the frame length");
-    FRT_CHECK_ARG(h, have_prev >= 0 && have_prev <= 2, "have_prev must be 0, 1 or 2");
-    FRT_CHECK_ARG(h, !have_prev || smoothed_dev, "have_prev needs the smoothed buffer");
+    const cudaStream_t st = (cudaStream_t)stream;
     if (h->gcc_long_route)
         return gcc_long_phat(h, d0_dev, d1_dev, stride, n_pairs, xcorr_dev, smoothed_dev, have_prev, idx_dev,
-                             val_dev, (cudaStream_t)stream);
-    const GccPlan *pl = h->gcc.get();
-    GccArgs a;
+                             val_dev, st);
+    GccArgs a = gcc_args(h->gcc.get(), xcorr_dev, smoothed_dev, have_prev, idx_dev, val_dev);
     a.d0 = d0_dev;
     a.d1 = d1_dev;
     a.stride = stride;
-    a.n_pairs = n_pairs;
-    a.L = pl->L;
-    a.window = pl->window.get();
-    a.tw = pl->tw.get();
-    a.perm = pl->perm.get();
-    a.xcorr = xcorr_dev;
-    a.smoothed = smoothed_dev;
-    a.have_prev = have_prev;
-    a.idx = idx_dev;
-    a.val = val_dev;
-    a.rd = pl->rd;
-    int blocks = n_pairs < h->sm_count ? n_pairs : h->sm_count;
-    return frt_launch(h, gcc_phat_kernel, blocks, GCC_THREADS, sizeof(float2) * pl->L, (cudaStream_t)stream, a);
+    a.n = n_pairs;
+    return frt_launch(h, gcc_phat_kernel, std::min(n_pairs, h->sm_count), GCC_THREADS, sizeof(float2) * L, st, a);
 }
 
 extern "C" int frt_gcc_set_pairs(frt_handle h, int n_channels, const int *pairs_host, int n_pairs) {
@@ -593,23 +595,20 @@ extern "C" int frt_gcc_set_pairs(frt_handle h, int n_channels, const int *pairs_
     return FRT_OK;
 }
 
-// The spectrum workspace of frt_gcc_phat_pairs: [C][H] float2 spectra, [C] int flags, and an L-float
-// zero row when C is odd.  Grow-only; a failed allocation is FRT_ENOMEM and leaves the handle usable.
-static int gcc_spectra_workspace(frt_ctx *h, int L, int H, GccSpectra &w) {
+// The spectrum workspace of frt_gcc_phat_pairs: [C][H] float2 spectra and [C] int flags.  Grow-only; a
+// failed allocation is FRT_ENOMEM and leaves the handle usable.
+static int gcc_spectra_workspace(frt_ctx *h, int H, GccSpectra &w) {
     const size_t C = (size_t)h->gcc_pairs_channels;
     auto up = [](size_t b) { return (b + 255) & ~size_t(255); };
-    const size_t o_quiet = up(C * H * sizeof(float2)), o_zero = o_quiet + up(C * sizeof(int));
-    const size_t bytes = o_zero + ((C & 1) ? (size_t)L * sizeof(float) : 0);
+    const size_t o_quiet = up(C * H * sizeof(float2)), bytes = o_quiet + up(C * sizeof(int));
     const cudaError_t e = h->gcc_spec_ws.grow(bytes);
     if (e == cudaErrorMemoryAllocation) {
         cudaGetLastError();
         return frt_fail(h, FRT_ENOMEM, "the spectra of %zu channels (%zu bytes) do not fit", C, bytes);
     }
     FRT_CUDA(h, e);
-    unsigned char *ws = h->gcc_spec_ws.get();
-    w.spec = (float2 *)ws;
-    w.quiet = (int *)(ws + o_quiet);
-    w.zero = (C & 1) ? (float *)(ws + o_zero) : nullptr;
+    w.spec = (float2 *)h->gcc_spec_ws.get();
+    w.quiet = (int *)(h->gcc_spec_ws.get() + o_quiet);
     return FRT_OK;
 }
 
@@ -618,56 +617,32 @@ extern "C" int frt_gcc_phat_pairs(frt_handle h, const float *x_dev, int64_t stri
                                   void *stream) {
     if (!h) return FRT_EINVAL;
     if (h->gcc_pairs_n < 0) return frt_fail(h, FRT_ESTATE, "frt_gcc_phat_pairs: call frt_gcc_set_pairs first");
-    if (!(h->gcc_long_route ? (bool)h->gcc_long : (bool)h->gcc))
-        return frt_fail(h, FRT_ESTATE, "frt_gcc_phat_pairs: call frt_gcc_plan first");
-    DeviceGuard g(h->device);
-    const int L = h->gcc_long_route ? gcc_long_length(h) : h->gcc->L;
-    FRT_CHECK_ARG(h, stride >= L, "stride smaller than the frame length");
+    // the stride is checked right after the plan, so a short one is refused even with an empty table
+    // (with no plan, gcc_call_checks refuses the call first)
+    int L = h->gcc_length;
+    if (L > 0) FRT_CHECK_ARG(h, stride >= L, "stride smaller than the frame length");
     const int n_pairs = h->gcc_pairs_n;
-    if (n_pairs == 0) return FRT_OK;
-    FRT_CHECK_ARG(h, x_dev && idx_dev && val_dev, "NULL buffer");
-    FRT_CHECK_ARG(h, have_prev >= 0 && have_prev <= 2, "have_prev must be 0, 1 or 2");
-    FRT_CHECK_ARG(h, !have_prev || smoothed_dev, "have_prev needs the smoothed buffer");
+    int rc = gcc_call_checks(h, "frt_gcc_phat_pairs", n_pairs, x_dev != nullptr, stride, have_prev, smoothed_dev,
+                             idx_dev, val_dev, L);
+    if (rc != FRT_OK || n_pairs == 0) return rc;
+    DeviceGuard g(h->device);
     const cudaStream_t st = (cudaStream_t)stream;
-    const int Lp = L - (L & 1);
     GccSpectra w;
-    int rc = gcc_spectra_workspace(h, L, Lp / 2 + 1, w);
+    rc = gcc_spectra_workspace(h, (L - (L & 1)) / 2 + 1, w);
     if (rc != FRT_OK) return rc;
-    if (w.zero) FRT_CUDA(h, cudaMemsetAsync(w.zero, 0, sizeof(float) * L, st));
     if (h->gcc_long_route)
         return gcc_long_phat_pairs(h, x_dev, stride, w, xcorr_dev, smoothed_dev, have_prev, idx_dev, val_dev, st);
-    const GccPlan *pl = h->gcc.get();
-    const int C = h->gcc_pairs_channels;
-    GccSpecArgs s;
-    s.x = x_dev;
-    s.stride = stride;
-    s.n_channels = C;
-    s.L = L;
-    s.zero = w.zero;
-    s.window = pl->window.get();
-    s.tw = pl->tw.get();
-    s.perm = pl->perm.get();
-    s.spec = w.spec;
-    s.quiet = w.quiet;
-    s.rd = pl->rd;
-    const int packs = (C + 1) / 2;
-    rc = frt_launch(h, gcc_spectra_kernel, packs < h->sm_count ? packs : h->sm_count, GCC_THREADS,
-                    sizeof(float2) * L, st, s);
-    if (rc != FRT_OK) return rc;
-    GccPairArgs a;
-    a.pairs = h->gcc_pairs.get();
-    a.n_pairs = n_pairs;
-    a.L = L;
-    a.spec = w.spec;
-    a.quiet = w.quiet;
-    a.tw = pl->tw.get();
-    a.perm = pl->perm.get();
-    a.xcorr = xcorr_dev;
-    a.smoothed = smoothed_dev;
-    a.have_prev = have_prev;
-    a.idx = idx_dev;
-    a.val = val_dev;
-    a.rd = pl->rd;
-    return frt_launch(h, gcc_pairs_kernel, n_pairs < h->sm_count ? n_pairs : h->sm_count, GCC_THREADS,
-                      sizeof(float2) * L, st, a);
+    // phase 1: pair q packs channels 2q and 2q+1, rows x + 2q*stride and x + (2q+1)*stride
+    GccArgs a = gcc_args(h->gcc.get(), xcorr_dev, smoothed_dev, have_prev, idx_dev, val_dev);
+    a.d0 = x_dev;
+    a.d1 = x_dev + stride;
+    a.stride = 2 * stride;
+    a.n = h->gcc_pairs_channels;
+    rc = frt_launch(h, gcc_spectra_kernel, std::min((a.n + 1) / 2, h->sm_count), GCC_THREADS, sizeof(float2) * L,
+                    st, a, w);
+    a.n = n_pairs;
+    if (rc == FRT_OK)
+        rc = frt_launch(h, gcc_pairs_kernel, std::min(n_pairs, h->sm_count), GCC_THREADS, sizeof(float2) * L, st, a,
+                        w, h->gcc_pairs.get());
+    return rc;
 }

@@ -153,6 +153,25 @@ def test_bluestein_groups_all_pairs_of_ten_channels():
         assert abs(float(val[p]) - ref[k]) < ABS_TOL, (i, j)
 
 
+def test_odd_last_channel_joins_its_bluestein_group():
+    """L = 240 000, table (0, 1), (2, 3), (4, 5): a call on 7 channels launches as many kernels as a
+    call on 8, because the odd last channel's pack runs in the same workspace group as the others."""
+    from friture_b200 import _lib
+    from friture_b200.correlation import PairGccPhat
+    L = 240000
+    h = _lib.Handle(0)
+    launches = []
+    for C in (7, 8):
+        est = PairGccPhat(L, C, [(0, 1), (2, 3), (4, 5)], handle=h)
+        x = cuda(planted(C, L, 600)[0])
+        est.estimate(x, smooth=False)                 # plans and sets the table
+        n = h.launch_count
+        est.estimate(x, smooth=False)
+        launches.append(h.launch_count - n)
+    assert launches[0] == launches[1], launches
+    h.close()
+
+
 @pytest.mark.parametrize("L", [2400, 16800])
 def test_refused_calls_then_a_good_one(L):
     """Each refused call returns its code and changes nothing: a following call is still right."""
@@ -189,7 +208,11 @@ def test_refused_calls_then_a_good_one(L):
     assert torch.equal(idx, want[0]) and torch.equal(val, want[1])
     assert table([]) == _lib.FRT_OK                  # an empty table: a call does nothing
     idx.fill_(-7)
+    assert run(stride=L - 1) == _lib.FRT_EINVAL      # but a short stride is still refused
     assert run() == _lib.FRT_OK
+    # frt_gcc_phat with no pairs returns before it checks the stride
+    assert lib.frt_gcc_phat(hh, _lib._ptr(xd), _lib._ptr(xd), L - 1, 0, None, None, 0, None, None,
+                            stream) == _lib.FRT_OK
     torch.cuda.synchronize()
     assert idx.tolist() == [-7, -7]
     h.close()
