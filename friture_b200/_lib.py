@@ -87,6 +87,10 @@ SIGNATURES = {
     "frt_gcc_set_pairs": (c_int, [c_void_p, c_int, c_void_p, c_int]),
     "frt_gcc_phat_pairs": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_int, c_void_p,
                                    c_void_p, c_void_p]),
+    "frt_gcc_phat_frames": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int, c_int, c_void_p,
+                                    c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "frt_gcc_phat_pairs_frames": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int, c_void_p, c_int,
+                                          c_void_p, c_void_p, c_void_p, c_void_p]),
     "frt_spectrum_reduce": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int, c_int, c_int,
                                     c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                     c_void_p]),

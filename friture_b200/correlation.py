@@ -87,6 +87,59 @@ class GccPhat:
             self._have_prev = True
         return idx, val, xc
 
+    def estimate_frames(self, d0, d1, hop, n_frames, stream=None):
+        """``estimate`` over ``n_frames`` frames of every pair in one library call, smoothing on: frame f
+        of pair p is ``d0[p, f*hop : f*hop + length]`` (and the same of ``d1``).  d0, d1: CUDA float32
+        [P, T], contiguous along time, T >= (n_frames - 1) * hop + length; strided views such as a
+        framer's buffer rows are passed as they are, overlapping frames are not copied.  Returns
+        (idx [F, P] int32, val [F, P] float32, std [F, P] float64), std being the population standard
+        deviation of each frame's smoothed row.  idx, val and the smoothing state are the same bits as
+        ``estimate`` called frame by frame."""
+        _lib.check_tensor(self, d0, "d0")
+        with _lib.call_stream(d0.device, stream) as sp:
+            d0, s0 = _lib.device_rows(self, d0, "d0")
+            d1, s1 = _lib.device_rows(self, d1, "d1")
+            if d0.shape != d1.shape:
+                raise ValueError("d0, d1 must be CUDA float32 tensors of the same shape [P, T]")
+            if s0 != s1:   # one row stride for both inputs
+                d0, s0 = _lib.device_rows(self, d0.contiguous(), "d0")
+                d1, s1 = _lib.device_rows(self, d1.contiguous(), "d1")
+            P = d0.shape[0]
+            return self._call_frames("frt_gcc_phat_frames", P, d0, hop, n_frames, sp,
+                                     _lib._ptr(d0), _lib._ptr(d1), s0, int(hop), int(n_frames), int(P))
+
+    def _frame_geometry(self, T, hop, n_frames):
+        hop, n_frames = int(hop), int(n_frames)
+        if n_frames < 0:
+            raise ValueError("n_frames must be >= 0")
+        if n_frames > 1 and hop < 1:
+            raise ValueError("hop must be >= 1")
+        if n_frames > 0 and T < (n_frames - 1) * hop + self.length:
+            raise ValueError("%d frames of %d samples at hop %d need %d samples per row, got %d"
+                             % (n_frames, self.length, hop, (n_frames - 1) * hop + self.length, T))
+
+    def _call_frames(self, symbol, P, x, hop, n_frames, sp, *inputs, after_plan=None):
+        """The frames twin of ``_call``: ``symbol(*inputs, smoothed, have_prev, idx, val, std, stream)``
+        with the smoothing state of P pairs; returns (idx, val, std), each [n_frames, P]."""
+        import torch
+        self._frame_geometry(x.shape[1], hop, n_frames)
+        self.handle.call("frt_gcc_plan", self.length)
+        if after_plan is not None:
+            after_plan()
+        F, device = int(n_frames), x.device
+        idx = torch.empty((F, P), dtype=torch.int32, device=device)
+        val = torch.empty((F, P), dtype=torch.float32, device=device)
+        std = torch.empty((F, P), dtype=torch.float64, device=device)
+        if F == 0 or P == 0:
+            return idx, val, std
+        if self._smoothed is None or tuple(self._smoothed.shape) != (P, self.out_length):
+            self._smoothed = torch.zeros((P, self.out_length), dtype=torch.float32, device=device)
+            self._have_prev = False
+        self.handle.call(symbol, *inputs, _lib._ptr(self._smoothed), 2 if self._have_prev else 0, _lib._ptr(idx),
+                         _lib._ptr(val), _lib._ptr(std), sp)
+        self._have_prev = True
+        return idx, val, std
+
     def delay_ms(self, idx):
         """Index -> delay in ms, wrapped to +-L/2 (delay_estimator.py:147-152)."""
         d = 1e3 * idx.to("cpu").double().numpy() / self.fs
@@ -139,3 +192,17 @@ class PairGccPhat(GccPhat):
                 raise ValueError("frame length %d != planned %d" % (L, self.length))
             return self._call("frt_gcc_phat_pairs", self.n_pairs, x.device, smooth, want_xcorr, sp,
                               _lib._ptr(x), x_stride, after_plan=self._sync_table)
+
+    def estimate_frames(self, x, hop, n_frames, stream=None):
+        """``estimate`` over ``n_frames`` frames in one library call, smoothing on: frame f of channel c
+        is ``x[c, f*hop : f*hop + length]``.  x: CUDA float32 [C, T], contiguous along time, any row
+        stride (a framer's buffer rows as they are).  Returns (idx, val, std), each [F, P], as
+        ``GccPhat.estimate_frames``; the same bits as ``estimate`` called frame by frame."""
+        _lib.check_tensor(self, x, "x")
+        with _lib.call_stream(x.device, stream) as sp:
+            x, x_stride = _lib.device_rows(self, x, "x")
+            if x.shape[0] != self.n_channels:
+                raise ValueError("x has %d channels, the pair table %d" % (x.shape[0], self.n_channels))
+            return self._call_frames("frt_gcc_phat_pairs_frames", self.n_pairs, x, hop, n_frames, sp,
+                                     _lib._ptr(x), x_stride, int(hop), int(n_frames),
+                                     after_plan=self._sync_table)

@@ -26,6 +26,12 @@ __device__ __forceinline__ float2 cross_spectrum(float2 D0, float2 D1) {
     return make_float2(D0.x * D1.x + D0.y * D1.y, D0.x * D1.y - D0.y * D1.x);
 }
 
+// The widget's temporal smoothing Xs = 0.3 X + 0.7 Xs_prev (delay_estimator.py:134-139), rounded as
+// fma(0.3, X, round(0.7 Xs_prev)).  Left to the compiler, the plain expression is contracted into an
+// FFMA on either product depending on the surrounding code; written out, every kernel that blends
+// (gcc_finish, gl_cols_inv, gcc_track_chain) gives the same bits for the same frame.
+__device__ __forceinline__ float gcc_blend(float x, float prev) { return fmaf(0.3f, x, 0.7f * prev); }
+
 // In-register forward DFT of R points, outputs in natural order.
 template <int R> __device__ __forceinline__ void dft(float2 (&v)[R]);
 
@@ -43,15 +49,17 @@ template <> __device__ __forceinline__ void dft<4>(float2 (&v)[4]) {
     v[3] = csub(d02, d13);
 }
 
-// Block-wide sum / max of one float per thread (blockDim.x a multiple of 32); s_red holds 33 floats.
-// Every thread gets the result.  The combination order is fixed, so a sum is the same bits every run.
-__device__ __forceinline__ float block_sum(float v, float *s_red) {
+// Block-wide sum / max of one float (block_sum: or double) per thread (blockDim.x a multiple of 32);
+// s_red holds 33 values.  Every thread gets the result.  The combination order is fixed, so a sum is
+// the same bits every run.
+template <class T>
+__device__ __forceinline__ T block_sum(T v, T *s_red) {
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
     const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
     __syncthreads();
     if (l == 0) s_red[w] = v;
     __syncthreads();
-    float t = (threadIdx.x < (blockDim.x >> 5)) ? s_red[threadIdx.x] : 0.f;
+    T t = (threadIdx.x < (blockDim.x >> 5)) ? s_red[threadIdx.x] : T(0);
     if (w == 0) {
         for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
         if (l == 0) s_red[32] = t;

@@ -155,9 +155,11 @@ using PlanPtr = std::unique_ptr<Plan, PlanDelete>;
 // hold on the Bluestein route of gcc_long.cu.  gcc_long_phat expects the arguments checked.
 std::vector<float> gcc_hanning(int length);   // numpy.hanning(length), evaluated in double
 int gcc_long_plan(frt_ctx *h, int length);
+// silent_dev: NULL or [n_pairs], whether each pair had a constant input (the frames entry points'
+// phase 1 on this route).
 int gcc_long_phat(frt_ctx *h, const float *d0_dev, const float *d1_dev, int64_t stride, int n_pairs,
                   float *xcorr_dev, float *smoothed_dev, int have_prev, int *idx_dev, float *val_dev,
-                  cudaStream_t st);
+                  cudaStream_t st, int *silent_dev = nullptr);
 // frt_gcc_phat_pairs: the spectra of the table's n_channels channels, D_c[k] for k = 0..L'/2, and
 // whether each channel is constant.
 struct GccSpectra {
@@ -165,7 +167,8 @@ struct GccSpectra {
     int *quiet;
 };
 int gcc_long_phat_pairs(frt_ctx *h, const float *x_dev, int64_t stride, const GccSpectra &w, float *xcorr_dev,
-                        float *smoothed_dev, int have_prev, int *idx_dev, float *val_dev, cudaStream_t st);
+                        float *smoothed_dev, int have_prev, int *idx_dev, float *val_dev, cudaStream_t st,
+                        int *silent_dev = nullptr);
 
 // A plan call builds into a local PlanPtr and moves it into its slot only on success, so a call
 // that fails leaves the previous plan of that kind in place.
@@ -188,6 +191,7 @@ struct frt_ctx {
     int gcc_pairs_n = -1;             // its entries; -1 before the first accepted table
     int gcc_pairs_channels = 0;       // the channels of the input it indexes
     DeviceArray<unsigned char> gcc_spec_ws;   // frt_gcc_phat_pairs' per-channel spectra, grow-only
+    DeviceArray<unsigned char> gcc_track_ws;  // frt_gcc_phat_frames / _pairs_frames' frame groups, grow-only
     StftStaging stft_host;
     CombStaging comb_host;
 };

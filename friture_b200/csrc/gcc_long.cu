@@ -84,6 +84,7 @@ struct GlArgs {
     int have_prev;
     int *idx;
     float *val;
+    int *silent;               // NULL or the group's first pair: gl_finish's silent flags
     // frt_gcc_phat_pairs.  Phase 1 (a group of packed channel pairs d0 = channel ch0 + 2p, d1 = the next
     // one, read as zeros past the last channel): per_channel = 1, so that a pair is skipped only when
     // both channels are constant, and the spectra and flags of channels < n_ch land in spec / quiet.
@@ -345,7 +346,7 @@ __global__ void __launch_bounds__(GL_THREADS) gl_cols_inv(const GlArgs a) {
         float v = fmaf(y.x, ch.x, -y.y * ch.y) * a.scale;
         if (xc) xc[n] = v;
         if (sm) {
-            if (st.prev) v = 0.3f * v + 0.7f * sm[n];
+            if (st.prev) v = gcc_blend(v, sm[n]);
             sm[n] = v;
         }
         if (!xc && !sm) buf[n].x = v;                   // where gl_finish reads the peak's value
@@ -438,6 +439,7 @@ __global__ void __launch_bounds__(256) gl_finish(const GlArgs a, int n_pairs) {
     if (pair >= n_pairs) return;
     const PairState st = a.st[pair];
     float *sm = a.smoothed ? a.smoothed + (size_t)pair * a.Lp : nullptr;
+    if (a.silent) a.silent[pair] = st.silent;
     if (st.silent) {
         a.idx[pair] = 0;
         a.val[pair] = 0.f;
@@ -646,16 +648,17 @@ static int gl_inverse(frt_ctx *h, const GccLongPlan *pl, GlArgs &a, int np, cuda
 
 // The outputs of the group starting at pair p0.
 static void gl_outputs(const GccLongPlan *pl, GlArgs &a, int p0, float *xcorr_dev, float *smoothed_dev,
-                       int *idx_dev, float *val_dev) {
+                       int *idx_dev, float *val_dev, int *silent_dev) {
     a.xcorr = xcorr_dev ? xcorr_dev + (size_t)p0 * pl->Lp : nullptr;
     a.smoothed = smoothed_dev ? smoothed_dev + (size_t)p0 * pl->Lp : nullptr;
     a.idx = idx_dev + p0;
     a.val = val_dev + p0;
+    a.silent = silent_dev ? silent_dev + p0 : nullptr;
 }
 
 int gcc_long_phat(frt_ctx *h, const float *d0_dev, const float *d1_dev, int64_t stride, int n_pairs,
                   float *xcorr_dev, float *smoothed_dev, int have_prev, int *idx_dev, float *val_dev,
-                  cudaStream_t st) {
+                  cudaStream_t st, int *silent_dev) {
     const GccLongPlan *pl = h->gcc_long.get();
     GlArgs a;
     int group = 0;
@@ -665,7 +668,7 @@ int gcc_long_phat(frt_ctx *h, const float *d0_dev, const float *d1_dev, int64_t 
         const int np = n_pairs - p0 < group ? n_pairs - p0 : group;
         a.d0 = d0_dev + (size_t)p0 * stride;
         a.d1 = d1_dev + (size_t)p0 * stride;
-        gl_outputs(pl, a, p0, xcorr_dev, smoothed_dev, idx_dev, val_dev);
+        gl_outputs(pl, a, p0, xcorr_dev, smoothed_dev, idx_dev, val_dev, silent_dev);
         rc = gl_forward(h, pl, a, np, st);
         if (rc == FRT_OK) rc = frt_launch(h, gl_split, dim3(split_blocks, np), GL_THREADS, 0, st, a);
         if (rc == FRT_OK) rc = gl_inverse(h, pl, a, np, st);
@@ -674,7 +677,8 @@ int gcc_long_phat(frt_ctx *h, const float *d0_dev, const float *d1_dev, int64_t 
 }
 
 int gcc_long_phat_pairs(frt_ctx *h, const float *x_dev, int64_t stride, const GccSpectra &w, float *xcorr_dev,
-                        float *smoothed_dev, int have_prev, int *idx_dev, float *val_dev, cudaStream_t st) {
+                        float *smoothed_dev, int have_prev, int *idx_dev, float *val_dev, cudaStream_t st,
+                        int *silent_dev) {
     const GccLongPlan *pl = h->gcc_long.get();
     const int C = h->gcc_pairs_channels, n_pairs = h->gcc_pairs_n;
     const int packs = (C + 1) / 2;
@@ -703,7 +707,7 @@ int gcc_long_phat_pairs(frt_ctx *h, const float *x_dev, int64_t stride, const Gc
     for (int p0 = 0; p0 < n_pairs && rc == FRT_OK; p0 += group) {
         const int np = n_pairs - p0 < group ? n_pairs - p0 : group;
         a.pairs = h->gcc_pairs.get() + p0;
-        gl_outputs(pl, a, p0, xcorr_dev, smoothed_dev, idx_dev, val_dev);
+        gl_outputs(pl, a, p0, xcorr_dev, smoothed_dev, idx_dev, val_dev, silent_dev);
         rc = frt_launch(h, gl_pair_state, (np + 255) / 256, 256, 0, st, a, np);
         if (rc == FRT_OK) rc = frt_launch(h, gl_cross, dim3(split_blocks, np), GL_THREADS, 0, st, a);
         if (rc == FRT_OK) rc = gl_inverse(h, pl, a, np, st);

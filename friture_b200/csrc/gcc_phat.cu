@@ -281,7 +281,7 @@ __device__ __forceinline__ void gcc_finish(const float2 *z, int L, const int *__
         float v = z[__ldg(perm + n)].x * inv;
         if (xc) xc[n] = v;
         if (sm) {
-            if (prev) v = 0.3f * v + 0.7f * sm[n];
+            if (prev) v = gcc_blend(v, sm[n]);
             sm[n] = v;
         }
         const float av = fabsf(v);
@@ -329,6 +329,70 @@ __device__ __forceinline__ void gcc_finish(const float2 *z, int L, const int *__
     __syncthreads();
 }
 
+// G[k] = conj(D0[k]) D1[k] for this thread's k = tid + i * blockDim.x <= L/2, from the packed
+// transform Z of d0 + j d1 in z, into the thread's slice g; returns the slice's max |G|.  The same
+// floats as gcc_phat_kernel's loop, which is written out there.
+__device__ __forceinline__ float gcc_packed_cross(const float2 *z, int L, const int *__restrict__ perm,
+                                                  float2 (&g)[GCC_MAX_PER_THREAD]) {
+    const int tid = threadIdx.x, nt = blockDim.x, half = L / 2;
+    float gmax = 0.f;
+#pragma unroll
+    for (int i = 0; i < GCC_MAX_PER_THREAD; i++) {
+        const int k = tid + i * nt;
+        g[i] = make_float2(0.f, 0.f);
+        if (k <= half) {
+            float2 D0, D1;
+            split_packed(z[__ldg(perm + k)], z[__ldg(perm + (k == 0 ? 0 : L - k))], D0, D1);
+            g[i] = cross_spectrum(D0, D1);
+            gmax = fmaxf(gmax, sqrtf(g[i].x * g[i].x + g[i].y * g[i].y));
+        }
+    }
+    return gmax;
+}
+
+// The same slice from two stored spectra D_i, D_j (frt_gcc_phat_pairs' phase 2).
+__device__ __forceinline__ float gcc_table_cross(const float2 *Di, const float2 *Dj, int L,
+                                                 float2 (&g)[GCC_MAX_PER_THREAD]) {
+    const int tid = threadIdx.x, nt = blockDim.x, half = L / 2;
+    float gmax = 0.f;
+#pragma unroll
+    for (int i = 0; i < GCC_MAX_PER_THREAD; i++) {
+        const int k = tid + i * nt;
+        g[i] = make_float2(0.f, 0.f);
+        if (k <= half) {
+            g[i] = cross_spectrum(Di[k], Dj[k]);
+            gmax = fmaxf(gmax, sqrtf(g[i].x * g[i].x + g[i].y * g[i].y));
+        }
+    }
+    return gmax;
+}
+
+// Phase 1 of frt_gcc_phat_pairs for one packed channel pair, rows d0 and d1 (NULL: the missing
+// partner of an odd last channel, read as zeros): the channels' constant flags in quiet[0], quiet[1]
+// and, unless both are constant, their spectra D[k], k = 0..L/2, in spec[k] and spec[L/2+1 + k].
+__device__ __forceinline__ void gcc_spectra_pack(float2 *z, float *s_red, const GccArgs &a, const float *d0,
+                                                 const float *d1, float2 *spec, int *quiet) {
+    const int L = a.L, H = L / 2 + 1;
+    const int tid = threadIdx.x, nt = blockDim.x;
+    const bool has1 = d1 != nullptr;
+    float m0, m1, span0, span1;
+    gcc_load<true>(z, d0, d1, L, s_red, m0, m1, span0, span1);
+    const bool quiet0 = !(span0 > 0.f), quiet1 = !(span1 > 0.f);
+    if (tid == 0) {
+        quiet[0] = quiet0;
+        if (has1) quiet[1] = quiet1;
+    }
+    if (quiet0 && quiet1) return;   // gcc_load's reductions ordered every read of z
+    fft_inplace(z, L, a.rd, a.tw, a.window, m0, m1);
+    for (int k = tid; k < H; k += nt) {
+        float2 D0, D1;
+        split_packed(z[__ldg(a.perm + k)], z[__ldg(a.perm + (k == 0 ? 0 : L - k))], D0, D1);
+        spec[k] = D0;
+        if (has1) spec[H + k] = D1;
+    }
+    __syncthreads();
+}
+
 __global__ void __launch_bounds__(GCC_THREADS, 1) gcc_phat_kernel(const GccArgs a) {
     extern __shared__ float2 z[];
     __shared__ float s_red[40];
@@ -345,7 +409,9 @@ __global__ void __launch_bounds__(GCC_THREADS, 1) gcc_phat_kernel(const GccArgs 
         }
         fft_inplace(z, L, a.rd, a.tw, a.window, m0, m1);   // mean removal + window fused in
 
-        // G[k] = conj(D0[k]) D1[k], k = 0..L/2, kept in registers
+        // G[k] = conj(D0[k]) D1[k], k = 0..L/2, kept in registers.  The loop of gcc_packed_cross, written
+        // out here: calling it changes this kernel's register allocation (304 B of stack and 68 B / 96 B
+        // of spills instead of 296 B and 60 B / 84 B), and this kernel's code is kept as it was.
         float2 g[GCC_MAX_PER_THREAD];
         float gmax = 0.f;
 #pragma unroll
@@ -372,28 +438,12 @@ __global__ void __launch_bounds__(GCC_THREADS, 1) gcc_phat_kernel(const GccArgs 
 __global__ void __launch_bounds__(GCC_THREADS, 1) gcc_spectra_kernel(const GccArgs a, const GccSpectra w) {
     extern __shared__ float2 z[];
     __shared__ float s_red[40];
-    const int L = a.L, H = L / 2 + 1;
-    const int tid = threadIdx.x, nt = blockDim.x;
+    const int L = a.L;
     for (int q = blockIdx.x; 2 * q < a.n; q += gridDim.x) {
-        const int c0 = 2 * q, c1 = 2 * q + 1;
-        const bool has1 = c1 < a.n;
-        float m0, m1, span0, span1;
-        gcc_load<true>(z, a.d0 + (size_t)q * a.stride, has1 ? a.d1 + (size_t)q * a.stride : nullptr, L, s_red, m0,
-                       m1, span0, span1);
-        const bool quiet0 = !(span0 > 0.f), quiet1 = !(span1 > 0.f);
-        if (tid == 0) {
-            w.quiet[c0] = quiet0;
-            if (has1) w.quiet[c1] = quiet1;
-        }
-        if (quiet0 && quiet1) continue;   // gcc_load's reductions ordered every read of z
-        fft_inplace(z, L, a.rd, a.tw, a.window, m0, m1);
-        for (int k = tid; k < H; k += nt) {
-            float2 D0, D1;
-            split_packed(z[__ldg(a.perm + k)], z[__ldg(a.perm + (k == 0 ? 0 : L - k))], D0, D1);
-            w.spec[(size_t)c0 * H + k] = D0;
-            if (has1) w.spec[(size_t)c1 * H + k] = D1;
-        }
-        __syncthreads();
+        const int c0 = 2 * q;
+        const bool has1 = c0 + 1 < a.n;
+        gcc_spectra_pack(z, s_red, a, a.d0 + (size_t)q * a.stride, has1 ? a.d1 + (size_t)q * a.stride : nullptr,
+                         w.spec + (size_t)c0 * (L / 2 + 1), w.quiet + c0);
     }
 }
 
@@ -402,29 +452,228 @@ __global__ void __launch_bounds__(GCC_THREADS, 1) gcc_pairs_kernel(const GccArgs
     extern __shared__ float2 z[];
     __shared__ float s_red[40];
     __shared__ int s_idx[33];
-    const int L = a.L, half = L / 2, H = half + 1;
-    const int tid = threadIdx.x, nt = blockDim.x;
+    const int L = a.L, H = L / 2 + 1;
     for (int pair = blockIdx.x; pair < a.n; pair += gridDim.x) {
         const int2 ij = __ldg(pairs + pair);
         if (__ldg(w.quiet + ij.x) || __ldg(w.quiet + ij.y)) {
             gcc_silent(pair, L, a.xcorr, a.smoothed, a.have_prev, a.idx, a.val);
             continue;
         }
-        const float2 *Di = w.spec + (size_t)ij.x * H, *Dj = w.spec + (size_t)ij.y * H;
         float2 g[GCC_MAX_PER_THREAD];
-        float gmax = 0.f;
-#pragma unroll
-        for (int i = 0; i < GCC_MAX_PER_THREAD; i++) {
-            const int k = tid + i * nt;
-            g[i] = make_float2(0.f, 0.f);
-            if (k <= half) {
-                g[i] = cross_spectrum(Di[k], Dj[k]);
-                gmax = fmaxf(gmax, sqrtf(g[i].x * g[i].x + g[i].y * g[i].y));
-            }
-        }
+        const float gmax = gcc_table_cross(w.spec + (size_t)ij.x * H, w.spec + (size_t)ij.y * H, L, g);
         gcc_inverse(z, g, gmax, L, s_red, a.rd, a.tw);
         gcc_finish(z, L, a.perm, pair, a.xcorr, a.smoothed, a.have_prev, a.idx, a.val, s_red, s_idx);
     }
+}
+
+// ---- frt_gcc_phat_frames / frt_gcc_phat_pairs_frames.  Phase 1 (per route) writes the raw Xcorr of
+// every (frame, pair) of a group of frames and whether the pair is silent in that frame; phase 2
+// (gcc_track_*, both routes) runs the smoothing chain over the frames in order, then the arg-max and
+// the moments of every smoothed row.
+
+// Phase 1's frame geometry and outputs on the shared-memory route: item i = f * n + p of a launch is
+// frame f of pair (or channel pack) p, whose rows start f * frame_stride after frame 0's.  A separate
+// kernel parameter, not part of GccArgs (see there).
+struct GccFrames {
+    long long frame_stride;
+    int n_frames;
+    int n_channels;            // frt_gcc_phat_pairs_frames: the channels of a frame's spectra
+    float *xraw;               // [n_frames][n_pairs][L] raw Xcorr
+    int *silent;               // [n_frames][n_pairs]
+};
+
+// The raw Xcorr x[n] = Re(FFT(conj Yfull))[n] / L from z, as gcc_finish forms it.
+__device__ __forceinline__ void gcc_store_raw(const float2 *z, int L, const int *__restrict__ perm, float *out) {
+    const float inv = 1.0f / (float)L;
+    for (int n = threadIdx.x; n < L; n += blockDim.x) out[n] = z[__ldg(perm + n)].x * inv;
+    __syncthreads();   // the next item rewrites z
+}
+
+// Rows d0, d1 of independent pairs, as gcc_phat_kernel.
+__global__ void __launch_bounds__(GCC_THREADS, 1) gcc_frames_kernel(const GccArgs a, const GccFrames fr) {
+    extern __shared__ float2 z[];
+    __shared__ float s_red[40];
+    const int L = a.L, items = fr.n_frames * a.n;
+    for (int it = blockIdx.x; it < items; it += gridDim.x) {
+        const int f = it / a.n, pair = it - f * a.n;
+        const size_t off = (size_t)pair * a.stride + (size_t)f * fr.frame_stride;
+        float m0, m1, span0, span1;
+        gcc_load(z, a.d0 + off, a.d1 + off, L, s_red, m0, m1, span0, span1);
+        const bool quiet = !(span0 > 0.f) || !(span1 > 0.f);
+        if (threadIdx.x == 0) fr.silent[it] = quiet;
+        if (quiet) continue;   // gcc_load's reductions ordered every read of z
+        fft_inplace(z, L, a.rd, a.tw, a.window, m0, m1);
+        float2 g[GCC_MAX_PER_THREAD];
+        const float gmax = gcc_packed_cross(z, L, a.perm, g);
+        gcc_inverse(z, g, gmax, L, s_red, a.rd, a.tw);
+        gcc_store_raw(z, L, a.perm, fr.xraw + (size_t)it * L);
+    }
+}
+
+// The channel packs of every frame, as gcc_spectra_kernel; frame f's spectra and flags start at
+// channel f * n_channels of the workspace.
+__global__ void __launch_bounds__(GCC_THREADS, 1) gcc_frames_spectra_kernel(const GccArgs a, const GccSpectra w,
+                                                                            const GccFrames fr) {
+    extern __shared__ float2 z[];
+    __shared__ float s_red[40];
+    const int C = fr.n_channels, packs = (C + 1) / 2, H = a.L / 2 + 1, items = fr.n_frames * packs;
+    for (int it = blockIdx.x; it < items; it += gridDim.x) {
+        const int f = it / packs, q = it - f * packs, c0 = 2 * q;
+        const size_t off = (size_t)q * a.stride + (size_t)f * fr.frame_stride;
+        const size_t c = (size_t)f * C + c0;
+        gcc_spectra_pack(z, s_red, a, a.d0 + off, c0 + 1 < C ? a.d1 + off : nullptr, w.spec + c * H, w.quiet + c);
+    }
+}
+
+// The table's entries in every frame, as gcc_pairs_kernel.
+__global__ void __launch_bounds__(GCC_THREADS, 1) gcc_frames_pairs_kernel(const GccArgs a, const GccSpectra w,
+                                                                          const int2 *pairs, const GccFrames fr) {
+    extern __shared__ float2 z[];
+    __shared__ float s_red[40];
+    const int L = a.L, H = L / 2 + 1, C = fr.n_channels, items = fr.n_frames * a.n;
+    for (int it = blockIdx.x; it < items; it += gridDim.x) {
+        const int f = it / a.n, pair = it - f * a.n;
+        const int2 ij = __ldg(pairs + pair);
+        const int *quiet = w.quiet + (size_t)f * C;
+        const bool silent = quiet[ij.x] || quiet[ij.y];
+        if (threadIdx.x == 0) fr.silent[it] = silent;
+        if (silent) continue;
+        const float2 *spec = w.spec + (size_t)f * C * H;
+        float2 g[GCC_MAX_PER_THREAD];
+        const float gmax = gcc_table_cross(spec + (size_t)ij.x * H, spec + (size_t)ij.y * H, L, g);
+        gcc_inverse(z, g, gmax, L, s_red, a.rd, a.tw);
+        gcc_store_raw(z, L, a.perm, fr.xraw + (size_t)it * L);
+    }
+}
+
+// Phase 2 over a group of frames, rows of Lr samples (L on this route, L' on the Bluestein route).
+constexpr int GCC_TRACK_THREADS = 256;
+constexpr int GCC_TRACK_PER_THREAD = 8;
+constexpr int GCC_TRACK_CHUNK = GCC_TRACK_THREADS * GCC_TRACK_PER_THREAD;   // lags per partial
+
+struct GccTrack {
+    float *xs;                     // [n_frames][n_pairs][Lr]: raw Xcorr in, smoothed Xcorr out
+    const int *silent;             // [n_frames][n_pairs]
+    const int *prev_in;            // [n_pairs]: the pair blends its first non-silent frame of the group
+    int *prev_out;                 // [n_pairs]: the same for the next group
+    float *smoothed;               // [n_pairs][Lr] the smoothing state
+    unsigned long long *best;      // [n_frames][n_pairs][n_chunks]: |Xs| bits << 32 | (0xffffffff - index)
+    double2 *moments;              // [n_frames][n_pairs][n_chunks]: mean and sum of squared deviations
+    int *idx;                      // [n_frames][n_pairs] outputs of the group
+    float *val;
+    double *std;
+    int Lr, n_pairs, n_frames, n_chunks;
+    int have_prev;                 // the call's, for frame 0
+};
+
+// Before a call's first group: whether each pair blends its first non-silent frame (frt_gcc_phat's
+// have_prev rule).  Read here, before any block rewrites the NaN marker in slot 0.
+__global__ void __launch_bounds__(256) gcc_track_prev(const GccTrack t, int *prev) {
+    const int p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p < t.n_pairs)
+        prev[p] = t.have_prev == 1 || (t.have_prev == 2 && !isnan(t.smoothed[(size_t)p * t.Lr]));
+}
+
+// The smoothing chain: thread n of pair p walks the group's frames in order and blends each
+// non-silent one into its state, as the per-frame calls would (a pair blends once it has had a
+// non-silent frame); the smoothed rows replace the raw ones.  A silent frame leaves the state alone.
+__global__ void __launch_bounds__(GCC_TRACK_THREADS) gcc_track_chain(const GccTrack t) {
+    const int n = blockIdx.x * blockDim.x + threadIdx.x;
+    if (n >= t.Lr) return;
+    const size_t fstride = (size_t)t.n_pairs * t.Lr;
+    for (int p = blockIdx.y; p < t.n_pairs; p += gridDim.y) {
+        bool prev = t.prev_in[p];
+        float *sm = t.smoothed + (size_t)p * t.Lr;
+        float cur = prev ? sm[n] : 0.f;
+        float *x = t.xs + (size_t)p * t.Lr + n;
+        for (int f = 0; f < t.n_frames; f++) {
+            if (t.silent[(size_t)f * t.n_pairs + p]) continue;
+            float v = x[f * fstride];
+            if (prev) v = gcc_blend(v, cur);
+            x[f * fstride] = v;
+            cur = v;
+            prev = true;
+        }
+        if (prev) sm[n] = cur;
+        else if (n == 0 && t.have_prev == 0) sm[0] = nanf("");   // no non-silent frame yet: "no previous"
+        if (n == 0) t.prev_out[p] = prev;
+    }
+}
+
+// Per (frame, pair, chunk of GCC_TRACK_CHUNK lags) of a non-silent row: the first maximum of |Xs| and
+// the chunk's mean and sum of squared deviations, in double.
+__global__ void __launch_bounds__(GCC_TRACK_THREADS) gcc_track_stats(const GccTrack t) {
+    __shared__ double s_red[33];
+    __shared__ unsigned long long s_best[GCC_TRACK_THREADS / 32];
+    const int it = blockIdx.x, c = blockIdx.y;
+    if (t.silent[it]) return;
+    const float *row = t.xs + (size_t)it * t.Lr;
+    const int n0 = c * GCC_TRACK_CHUNK, cnt = min(GCC_TRACK_CHUNK, t.Lr - n0);
+    float v[GCC_TRACK_PER_THREAD];
+    double s = 0.0;
+    unsigned long long best = 0ull;
+#pragma unroll
+    for (int i = 0; i < GCC_TRACK_PER_THREAD; i++) {
+        const int k = threadIdx.x + i * GCC_TRACK_THREADS;
+        v[i] = 0.f;
+        if (k < cnt) {
+            v[i] = row[n0 + k];
+            s += (double)v[i];
+            const unsigned long long key =
+                ((unsigned long long)__float_as_uint(fabsf(v[i])) << 32) | (0xffffffffu - (unsigned)(n0 + k));
+            best = key > best ? key : best;
+        }
+    }
+    const double mean = block_sum(s, s_red) / (double)cnt;
+    double m2 = 0.0;
+#pragma unroll
+    for (int i = 0; i < GCC_TRACK_PER_THREAD; i++) {
+        const double d = (double)v[i] - mean;
+        if (threadIdx.x + i * GCC_TRACK_THREADS < cnt) m2 += d * d;
+    }
+    m2 = block_sum(m2, s_red);
+    for (int o = 16; o > 0; o >>= 1) {
+        const unsigned long long ob = __shfl_xor_sync(0xffffffffu, best, o);
+        best = ob > best ? ob : best;
+    }
+    if ((threadIdx.x & 31) == 0) s_best[threadIdx.x >> 5] = best;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        for (int w = 1; w < GCC_TRACK_THREADS / 32; w++) best = s_best[w] > best ? s_best[w] : best;
+        const size_t o = (size_t)it * t.n_chunks + c;
+        t.best[o] = best;
+        t.moments[o] = make_double2(mean, m2);
+    }
+}
+
+// Per (frame, pair): the chunks combined in index order (Chan et al.'s pairwise update of the
+// moments), so the result depends on the length alone; silent rows give (0, 0, 0).
+__global__ void __launch_bounds__(256) gcc_track_finish(const GccTrack t) {
+    const int it = blockIdx.x * blockDim.x + threadIdx.x;
+    if (it >= t.n_frames * t.n_pairs) return;
+    if (t.silent[it]) {
+        t.idx[it] = 0;
+        t.val[it] = 0.f;
+        t.std[it] = 0.0;
+        return;
+    }
+    const unsigned long long *b = t.best + (size_t)it * t.n_chunks;
+    const double2 *m = t.moments + (size_t)it * t.n_chunks;
+    unsigned long long best = 0ull;
+    double n = 0.0, mean = 0.0, m2 = 0.0;
+    for (int c = 0; c < t.n_chunks; c++) {
+        best = b[c] > best ? b[c] : best;
+        const double nb = (double)min(GCC_TRACK_CHUNK, t.Lr - c * GCC_TRACK_CHUNK), nn = n + nb;
+        const double2 mc = m[c];
+        const double d = mc.x - mean;
+        mean += d * (nb / nn);
+        m2 += mc.y + d * d * (n * nb / nn);
+        n = nn;
+    }
+    const int bi = (int)(0xffffffffu - (unsigned)(best & 0xffffffffull));
+    t.idx[it] = bi;
+    t.val[it] = t.xs[(size_t)it * t.Lr + bi];
+    t.std[it] = sqrt(m2 / n);
 }
 
 }   // namespace
@@ -645,4 +894,192 @@ extern "C" int frt_gcc_phat_pairs(frt_handle h, const float *x_dev, int64_t stri
         rc = frt_launch(h, gcc_pairs_kernel, std::min(n_pairs, h->sm_count), GCC_THREADS, sizeof(float2) * L, st, a,
                         w, h->gcc_pairs.get());
     return rc;
+}
+
+// ---- frt_gcc_phat_frames / frt_gcc_phat_pairs_frames
+
+// The frames entry points' own checks, after gcc_call_checks.  `work`: false when there is nothing to
+// do (no pairs or no frames).
+static int gcc_frames_checks(frt_ctx *h, int n_pairs, int n_frames, int64_t frame_stride, const float *smoothed_dev,
+                             const double *std_dev, bool &work) {
+    work = false;
+    FRT_CHECK_ARG(h, n_frames >= 0, "negative n_frames");
+    if (n_pairs == 0 || n_frames == 0) return FRT_OK;
+    FRT_CHECK_ARG(h, n_frames == 1 || frame_stride >= 1, "frame_stride must be >= 1");
+    FRT_CHECK_ARG(h, smoothed_dev && std_dev, "NULL buffer");
+    work = true;
+    return FRT_OK;
+}
+
+// Frames run in groups whose workspace (raw and smoothed rows, flags, partials and, for the pair table
+// on the shared-memory route, the frames' spectra) fits this budget; at least one frame per group.
+constexpr size_t GCC_TRACK_BUDGET = size_t(2) << 30;
+
+// The workspace of a frames call, grow-only: groups of `group` frames of n_pairs rows of Lr samples,
+// plus spec_channels spectra of H bins per frame.  t gets its buffers and the call's constants; prev is
+// the two [n_pairs] halves the groups alternate between.  FRT_ENOMEM when it cannot grow (the handle
+// stays usable).
+static int gcc_track_workspace(frt_ctx *h, int n_pairs, int n_frames, int Lr, int spec_channels, int H,
+                               GccTrack &t, int *&prev, GccSpectra &w, int &group) {
+    auto up = [](size_t b) { return (b + 255) & ~size_t(255); };
+    const size_t P = (size_t)n_pairs, C = (size_t)spec_channels;
+    const int nc = (Lr + GCC_TRACK_CHUNK - 1) / GCC_TRACK_CHUNK;
+    const size_t per_frame = P * ((size_t)Lr * sizeof(float) + sizeof(int) +
+                                  (size_t)nc * (sizeof(unsigned long long) + sizeof(double2))) +
+                             C * ((size_t)H * sizeof(float2) + sizeof(int));
+    const size_t fixed = up(2 * P * sizeof(int)) + 7 * 256;
+    size_t g = GCC_TRACK_BUDGET > fixed ? (GCC_TRACK_BUDGET - fixed) / per_frame : 0;
+    g = g < 1 ? 1 : g > (size_t)n_frames ? (size_t)n_frames : g;
+    const size_t o_sil = up(g * P * Lr * sizeof(float)), o_best = o_sil + up(g * P * sizeof(int)),
+                 o_mom = o_best + up(g * P * nc * sizeof(unsigned long long)),
+                 o_prev = o_mom + up(g * P * nc * sizeof(double2)), o_spec = o_prev + up(2 * P * sizeof(int)),
+                 o_quiet = o_spec + up(g * C * H * sizeof(float2)), bytes = o_quiet + up(g * C * sizeof(int));
+    const cudaError_t e = h->gcc_track_ws.grow(bytes);
+    if (e == cudaErrorMemoryAllocation) {
+        cudaGetLastError();
+        return frt_fail(h, FRT_ENOMEM, "the workspace of one frame (%zu bytes) does not fit", per_frame);
+    }
+    FRT_CUDA(h, e);
+    unsigned char *ws = h->gcc_track_ws.get();
+    t = GccTrack{};
+    t.xs = (float *)ws;
+    t.silent = (const int *)(ws + o_sil);
+    t.best = (unsigned long long *)(ws + o_best);
+    t.moments = (double2 *)(ws + o_mom);
+    t.Lr = Lr;
+    t.n_pairs = n_pairs;
+    t.n_chunks = nc;
+    prev = (int *)(ws + o_prev);
+    if (C) {
+        w.spec = (float2 *)(ws + o_spec);
+        w.quiet = (int *)(ws + o_quiet);
+    }
+    group = (int)g;
+    return FRT_OK;
+}
+
+// Both entry points after their checks: per group of frames, phase1(f0, nf, xraw, silent) writes the
+// raw rows and flags of frames f0 .. f0+nf-1, then phase 2 smooths them in order and reduces them.
+template <class Phase1>
+static int gcc_frames_run(frt_ctx *h, int n_pairs, int n_frames, int Lr, int spec_channels, int H, float *smoothed_dev,
+                          int have_prev, int *idx_dev, float *val_dev, double *std_dev, cudaStream_t st, GccSpectra &w,
+                          Phase1 phase1) {
+    GccTrack t;
+    int *prev = nullptr, group = 0;
+    int rc = gcc_track_workspace(h, n_pairs, n_frames, Lr, spec_channels, H, t, prev, w, group);
+    if (rc != FRT_OK) return rc;
+    t.smoothed = smoothed_dev;
+    t.have_prev = have_prev;
+    rc = frt_launch(h, gcc_track_prev, (n_pairs + 255) / 256, 256, 0, st, t, prev);
+    const unsigned row_blocks = (unsigned)((Lr + GCC_TRACK_THREADS - 1) / GCC_TRACK_THREADS);
+    for (int f0 = 0, g = 0; f0 < n_frames && rc == FRT_OK; f0 += group, g++) {
+        const int nf = std::min(group, n_frames - f0);
+        rc = phase1(f0, nf, t.xs, const_cast<int *>(t.silent));
+        t.n_frames = nf;
+        t.prev_in = prev + (size_t)(g & 1) * n_pairs;
+        t.prev_out = prev + (size_t)((g + 1) & 1) * n_pairs;
+        t.idx = idx_dev + (size_t)f0 * n_pairs;
+        t.val = val_dev + (size_t)f0 * n_pairs;
+        t.std = std_dev + (size_t)f0 * n_pairs;
+        const int items = nf * n_pairs;
+        if (rc == FRT_OK)
+            rc = frt_launch(h, gcc_track_chain, dim3(row_blocks, std::min(n_pairs, 65535)), GCC_TRACK_THREADS, 0, st,
+                            t);
+        if (rc == FRT_OK)
+            rc = frt_launch(h, gcc_track_stats, dim3(items, t.n_chunks), GCC_TRACK_THREADS, 0, st, t);
+        if (rc == FRT_OK) rc = frt_launch(h, gcc_track_finish, (items + 255) / 256, 256, 0, st, t);
+    }
+    return rc;
+}
+
+extern "C" int frt_gcc_phat_frames(frt_handle h, const float *d0_dev, const float *d1_dev, int64_t stride,
+                                   int64_t frame_stride, int n_frames, int n_pairs, float *smoothed_dev,
+                                   int have_prev, int *idx_dev, float *val_dev, double *std_dev, void *stream) {
+    if (!h) return FRT_EINVAL;
+    int L;
+    bool work;
+    int rc = gcc_call_checks(h, "frt_gcc_phat_frames", n_pairs, d0_dev && d1_dev, stride, have_prev, smoothed_dev,
+                             idx_dev, val_dev, L);
+    if (rc == FRT_OK) rc = gcc_frames_checks(h, n_pairs, n_frames, frame_stride, smoothed_dev, std_dev, work);
+    if (rc != FRT_OK || !work) return rc;
+    DeviceGuard g(h->device);
+    const cudaStream_t st = (cudaStream_t)stream;
+    const int Lr = L - (L & 1);
+    GccSpectra w{};
+    if (h->gcc_long_route)
+        return gcc_frames_run(h, n_pairs, n_frames, Lr, 0, 0, smoothed_dev, have_prev, idx_dev, val_dev, std_dev, st, w,
+                              [&](int f0, int nf, float *xraw, int *silent) {
+                                  int r = FRT_OK;
+                                  for (int f = 0; f < nf && r == FRT_OK; f++) {
+                                      const size_t off = (size_t)(f0 + f) * frame_stride, o = (size_t)f * n_pairs;
+                                      // idx / val of the frame's rows are scratch until phase 2 fills them
+                                      r = gcc_long_phat(h, d0_dev + off, d1_dev + off, stride, n_pairs, xraw + o * Lr,
+                                                        nullptr, 0, idx_dev + (size_t)f0 * n_pairs + o,
+                                                        val_dev + (size_t)f0 * n_pairs + o, st, silent + o);
+                                  }
+                                  return r;
+                              });
+    GccArgs a = gcc_args(h->gcc.get(), nullptr, nullptr, 0, nullptr, nullptr);
+    a.stride = stride;
+    a.n = n_pairs;
+    return gcc_frames_run(h, n_pairs, n_frames, Lr, 0, 0, smoothed_dev, have_prev, idx_dev, val_dev, std_dev, st, w,
+                          [&](int f0, int nf, float *xraw, int *silent) {
+                              a.d0 = d0_dev + (size_t)f0 * frame_stride;
+                              a.d1 = d1_dev + (size_t)f0 * frame_stride;
+                              const GccFrames fr{frame_stride, nf, 0, xraw, silent};
+                              return frt_launch(h, gcc_frames_kernel, std::min(nf * n_pairs, h->sm_count), GCC_THREADS,
+                                                sizeof(float2) * L, st, a, fr);
+                          });
+}
+
+extern "C" int frt_gcc_phat_pairs_frames(frt_handle h, const float *x_dev, int64_t stride, int64_t frame_stride,
+                                         int n_frames, float *smoothed_dev, int have_prev, int *idx_dev, float *val_dev,
+                                         double *std_dev, void *stream) {
+    if (!h) return FRT_EINVAL;
+    if (h->gcc_pairs_n < 0)
+        return frt_fail(h, FRT_ESTATE, "frt_gcc_phat_pairs_frames: call frt_gcc_set_pairs first");
+    int L = h->gcc_length;
+    if (L > 0) FRT_CHECK_ARG(h, stride >= L, "stride smaller than the frame length");
+    const int n_pairs = h->gcc_pairs_n, C = h->gcc_pairs_channels;
+    bool work;
+    int rc = gcc_call_checks(h, "frt_gcc_phat_pairs_frames", n_pairs, x_dev != nullptr, stride, have_prev,
+                             smoothed_dev, idx_dev, val_dev, L);
+    if (rc == FRT_OK) rc = gcc_frames_checks(h, n_pairs, n_frames, frame_stride, smoothed_dev, std_dev, work);
+    if (rc != FRT_OK || !work) return rc;
+    DeviceGuard g(h->device);
+    const cudaStream_t st = (cudaStream_t)stream;
+    const int Lr = L - (L & 1), H = Lr / 2 + 1;
+    GccSpectra w{};
+    if (h->gcc_long_route) {
+        rc = gcc_spectra_workspace(h, H, w);   // one frame's spectra, reused frame by frame
+        if (rc != FRT_OK) return rc;
+        return gcc_frames_run(h, n_pairs, n_frames, Lr, 0, 0, smoothed_dev, have_prev, idx_dev, val_dev, std_dev, st, w,
+                              [&](int f0, int nf, float *xraw, int *silent) {
+                                  int r = FRT_OK;
+                                  for (int f = 0; f < nf && r == FRT_OK; f++) {
+                                      const size_t off = (size_t)(f0 + f) * frame_stride, o = (size_t)f * n_pairs;
+                                      r = gcc_long_phat_pairs(h, x_dev + off, stride, w, xraw + o * Lr, nullptr, 0,
+                                                              idx_dev + (size_t)f0 * n_pairs + o,
+                                                              val_dev + (size_t)f0 * n_pairs + o, st, silent + o);
+                                  }
+                                  return r;
+                              });
+    }
+    // phase 1 as frt_gcc_phat_pairs': pack q of a frame is channels 2q and 2q+1
+    GccArgs a = gcc_args(h->gcc.get(), nullptr, nullptr, 0, nullptr, nullptr);
+    a.stride = 2 * stride;
+    return gcc_frames_run(h, n_pairs, n_frames, Lr, C, H, smoothed_dev, have_prev, idx_dev, val_dev, std_dev, st, w,
+                          [&](int f0, int nf, float *xraw, int *silent) {
+                              a.d0 = x_dev + (size_t)f0 * frame_stride;
+                              a.d1 = a.d0 + stride;
+                              const GccFrames fr{frame_stride, nf, C, xraw, silent};
+                              a.n = C;
+                              int r = frt_launch(h, gcc_frames_spectra_kernel, std::min(nf * ((C + 1) / 2), h->sm_count),
+                                                 GCC_THREADS, sizeof(float2) * L, st, a, w, fr);
+                              a.n = n_pairs;
+                              if (r == FRT_OK)
+                                  r = frt_launch(h, gcc_frames_pairs_kernel, std::min(nf * n_pairs, h->sm_count),
+                                                 GCC_THREADS, sizeof(float2) * L, st, a, w, h->gcc_pairs.get(), fr);
+                              return r;
+                          });
 }

@@ -4,6 +4,8 @@ overlap and end-index semantics, GCC-PHAT, temporal smoothing, peak pick, delay 
 confidence."""
 from __future__ import annotations
 
+from typing import NamedTuple
+
 import numpy as np
 
 from . import _lib, filter_data
@@ -45,6 +47,18 @@ class Decimator:
         return out
 
 
+class DelayTrack(NamedTuple):
+    """Every frame of an estimator's last ``handle_new_data`` call, oldest first.  ``end_index`` [r]:
+    the widget's ``old_index`` after the frame (its last sample, in 12 kHz samples since the stream
+    began); the others are [r, n_pairs] and mean what the estimator's attributes of the same names
+    mean for the last frame."""
+    end_index: np.ndarray
+    delay_ms: np.ndarray
+    distance_m: np.ndarray
+    correlation: np.ndarray
+    Xcorr_extremum: np.ndarray
+
+
 class _DelayWidget:
     """What the widget's numeric part shares between the pair and the channel-array estimators: the
     frame geometry of a delay range and the published values."""
@@ -66,28 +80,48 @@ class _DelayWidget:
         self.distance_m = np.zeros(n_pairs)
         self.correlation = np.zeros(n_pairs, dtype=int)
         self.Xcorr_extremum = np.zeros(n_pairs)
+        self.track = self._track(np.zeros(0, dtype=np.int64), np.zeros((0, n_pairs), dtype=np.int64),
+                                 np.zeros((0, n_pairs)), np.zeros((0, n_pairs)))
 
-    def _publish(self, idx, val):
-        import torch
-        sm = self.gcc._smoothed
-        i = idx.cpu().numpy().astype(np.int64)
-        v = val.cpu().numpy().astype(np.float64)
-        std = torch.std(sm.double(), dim=1, unbiased=False).cpu().numpy()
+    def _run_frames(self, r, gcc_frames):
+        """Runs the r frames the framer just took with one ``estimate_frames`` call (gcc_frames) and
+        publishes them; the framer's old_index has already moved past them."""
+        end_index = self._framer.old_index - self.needed * np.arange(r - 1, -1, -1, dtype=np.int64)
+        if r == 0:
+            self.track = self._track(end_index, np.zeros((0, self.n_pairs), dtype=np.int64),
+                                     np.zeros((0, self.n_pairs)), np.zeros((0, self.n_pairs)))
+            return
+        idx, val, std = gcc_frames()
+        self._publish(end_index, idx, val, std)
+
+    def _publish(self, end_index, idx, val, std):
+        """idx, val, std: [r, P] per frame (any tensor or array on any device).  The widget's formulas
+        (delay_estimator.py:146-176) on every frame; the attributes take the last one."""
+        track = self._track(np.asarray(end_index, dtype=np.int64), np.asarray(idx.cpu()).astype(np.int64),
+                            np.asarray(val.cpu()).astype(np.float64), np.asarray(std.cpu()).astype(np.float64))
+        self.track = track
+        if track.end_index.shape[0]:
+            self.delay_ms = track.delay_ms[-1]
+            self.Xcorr_extremum = track.Xcorr_extremum[-1]
+            self.distance_m = track.distance_m[-1]
+            self.correlation = track.correlation[-1]
+
+    def _track(self, end_index, i, v, std):
         time = 2 * self.delayrange_s
         with np.errstate(divide="ignore", invalid="ignore"):
             norm = np.where(std > 0, np.abs(v) / (3 * std), 0.0)           # :146
         delay = 1e3 * i / self.subsampled_sampling_rate                     # :147
         delay = np.where(delay > 1e3 * time / 2., delay - 1e3 * time, delay)   # :150-151
-        self.delay_ms = delay
-        self.Xcorr_extremum = v
-        self.distance_m = delay * 1e-3 * 340.                              # :169-170
         x = (norm > 1.) * (norm - 1.)                                      # :173-176
         x = (0.12 * x) ** 3
-        self.correlation = ((x / (1. + x)) * 100).astype(int)
+        return DelayTrack(end_index=end_index, delay_ms=delay, distance_m=delay * 1e-3 * 340.,   # :169-170
+                          correlation=((x / (1. + x)) * 100).astype(int), Xcorr_extremum=v)
 
 
 class DelayEstimator(_DelayWidget):
-    """Per pair (channel 0 vs channel 1 of each stream): push 48 kHz chunks, get the delay."""
+    """Per pair (channel 0 vs channel 1 of each stream): push 48 kHz chunks, get the delay.  Each
+    ``handle_new_data`` runs all the frames the chunk completes in one library call; ``track`` keeps
+    every one of them, and ``delay_ms`` etc. are the last one's."""
 
     def __init__(self, n_pairs, delayrange_s=DEFAULT_DELAYRANGE, device=None):
         self._setup_range(delayrange_s, device)
@@ -98,6 +132,7 @@ class DelayEstimator(_DelayWidget):
                                 pre_increment=True)
         self.fr1 = StreamFramer(n_pairs, self.length, self.needed, self.device, capacity=self.capacity,
                                 pre_increment=True)
+        self._framer = self.fr0
         self.gcc = GccPhat(self.length, handle=self.dec0.handle, fs=self.subsampled_sampling_rate)
         self._setup_outputs(n_pairs)
 
@@ -109,11 +144,7 @@ class DelayEstimator(_DelayWidget):
         self.fr1.push(d1)
         v0, r = self.fr0.take()
         v1, _ = self.fr1.take()
-        for i in range(r):
-            a = v0[:, i * self.needed:i * self.needed + self.length]
-            b = v1[:, i * self.needed:i * self.needed + self.length]
-            idx, val, xc = self.gcc.estimate(a, b, smooth=True, want_xcorr=False)
-            self._publish(idx, val)
+        self._run_frames(r, lambda: self.gcc.estimate_frames(v0, v1, self.needed, r))
         return r
 
 
@@ -121,7 +152,7 @@ class ArrayDelayEstimator(_DelayWidget):
     """Delays between channels of one multichannel stream: for every entry (i, j) of ``pairs``,
     channel i is the widget's channel 0 and channel j its channel 1.  Push [C, n] chunks at 48 kHz;
     each channel is decimated, framed and transformed once.  ``delay_ms``, ``distance_m``,
-    ``correlation`` and ``Xcorr_extremum`` are indexed by pair, as ``DelayEstimator``'s are."""
+    ``correlation``, ``Xcorr_extremum`` and ``track`` are indexed by pair, as ``DelayEstimator``'s are."""
 
     def __init__(self, n_channels, pairs, delayrange_s=DEFAULT_DELAYRANGE, device=None):
         self._setup_range(delayrange_s, device)
@@ -129,6 +160,7 @@ class ArrayDelayEstimator(_DelayWidget):
         self.dec = Decimator(self.n_channels, self.Ndec, self.device)
         self.fr = StreamFramer(self.n_channels, self.length, self.needed, self.device, capacity=self.capacity,
                                pre_increment=True)
+        self._framer = self.fr
         self.gcc = PairGccPhat(self.length, self.n_channels, pairs, handle=self.dec.handle,
                                fs=self.subsampled_sampling_rate)
         self.n_pairs = self.gcc.n_pairs
@@ -138,7 +170,5 @@ class ArrayDelayEstimator(_DelayWidget):
         """x: CUDA float32 [n_channels, n] chunk at 48 kHz.  Returns the number of frames run."""
         self.fr.push(self.dec.process(x))
         v, r = self.fr.take()
-        for i in range(r):
-            idx, val, _ = self.gcc.estimate(v[:, i * self.needed:i * self.needed + self.length], smooth=True)
-            self._publish(idx, val)
+        self._run_frames(r, lambda: self.gcc.estimate_frames(v, self.needed, r))
         return r

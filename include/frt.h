@@ -238,6 +238,32 @@ int frt_gcc_set_pairs(frt_handle h, int n_channels, const int *pairs_host, int n
  * table or a plan; FRT_ENOMEM when the spectra do not fit on the device (the handle stays usable). */
 int frt_gcc_phat_pairs(frt_handle h, const float *x_dev, int64_t stride, float *xcorr_dev,
                        float *smoothed_dev, int have_prev, int *idx_dev, float *val_dev, void *stream);
+/* frt_gcc_phat over n_frames frames of every pair in one call, with each frame's result kept: frame f
+ * of pair p is d0/d1[p*stride + f*frame_stride + n], n < L (frames may overlap; the widget's hop is
+ * L/2).  The frames run in order through the smoothing: have_prev applies to frame 0 as in
+ * frt_gcc_phat, and a later frame blends once its pair has had a non-silent frame (have_prev = 2's
+ * rule).  smoothed_dev [n_pairs][L'] is required; it ends holding the state after the last frame.
+ * Outputs, each [n_frames][n_pairs]:
+ *   idx_dev/val_dev  the frame's argmax |Xs| (first maximum) and Xs there;
+ *   std_dev          the population standard deviation of the frame's smoothed row, in double
+ *                    (numpy.std(smoothed_Xcorr), delay_estimator.py:147).
+ * A pair silent in a frame (a constant input) gives (0, 0, 0) and keeps its smoothing row.  idx, val
+ * and the final smoothed buffer are the same bits as n_frames frt_gcc_phat calls, one per frame.
+ * Frames run in groups within a grow-only workspace of about 4*L' + 24*ceil(L'/2048) bytes per pair
+ * and frame, kept within 2 GiB (one frame at least; FRT_ENOMEM, handle usable, when it cannot grow);
+ * the Bluestein route also uses frt_gcc_phat's workspace, frame by frame.  n_frames = 0 or n_pairs = 0
+ * does nothing; frame_stride >= 1 when n_frames > 1.                                              */
+int frt_gcc_phat_frames(frt_handle h, const float *d0_dev, const float *d1_dev, int64_t stride,
+                        int64_t frame_stride, int n_frames, int n_pairs, float *smoothed_dev,
+                        int have_prev, int *idx_dev, float *val_dev, double *std_dev, void *stream);
+/* frt_gcc_phat_pairs over n_frames frames: frame f of channel c is x[c*stride + f*frame_stride + n].
+ * Everything else as frt_gcc_phat_frames, indexed [n_frames][table entry]; each channel of each frame
+ * is transformed once.  On the shared-memory route the workspace also holds the frames' spectra,
+ * about 8 * n_channels * (L/2+1) bytes per frame.  With the table (0,1), (2,3), ... the results are
+ * the same bits as frt_gcc_phat_frames(x[0::2], x[1::2]).                                           */
+int frt_gcc_phat_pairs_frames(frt_handle h, const float *x_dev, int64_t stride, int64_t frame_stride,
+                              int n_frames, float *smoothed_dev, int have_prev, int *idx_dev,
+                              float *val_dev, double *std_dev, void *stream);
 
 /* ---------------------------------------------------------------- N-fold decimation
  * Stands behind `decimate_multiple(Ndec, bdec, adec, x, zis)` (friture/signal/decimate.py:45-71),
