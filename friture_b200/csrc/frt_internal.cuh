@@ -192,6 +192,7 @@ struct frt_ctx {
     int gcc_pairs_channels = 0;       // the channels of the input it indexes
     DeviceArray<unsigned char> gcc_spec_ws;   // frt_gcc_phat_pairs' per-channel spectra, grow-only
     DeviceArray<unsigned char> gcc_track_ws;  // frt_gcc_phat_frames / _pairs_frames' frame groups, grow-only
+    DeviceArray<unsigned char> spec_ticks_ws;  // frt_spectrum_reduce_ticks / _dual_ticks' state rows, grow-only
     StftStaging stft_host;
     CombStaging comb_host;
 };

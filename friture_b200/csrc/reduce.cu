@@ -4,6 +4,8 @@
 // friture/signal/exp_smoothing.py:59-107; log_spectrogram spectrum.py:95-101;
 // harmonic_product_spectrum spectrum.py:103-123), and in the widget's dual-channel mode the transfer
 // function between a reference and a measurement channel (spectrum.py:141-182).
+#include <algorithm>
+
 #include "frt_internal.cuh"
 
 namespace {
@@ -43,12 +45,22 @@ __device__ int block_argmax(double best, int besti, double *s_val, int *s_idx) {
     return s_idx[32];
 }
 
-// s <- alpha x + (1-alpha) s  (exp_smoothing.py:59-107), as s + alpha (x - s) in double across the
-// tick's frames of one bin of NCH channels side by side (their loads in flight together); the
-// carried states d are read and written back rounded to float32.  In float32, (1-alpha) rounded
-// biases the fixed point by about eps/alpha, and rounding every frame walks s off by about
-// eps/sqrt(alpha): 1e-4 and 4e-6 of the peak at N = 32, T = 5 s (alpha = 3.5e-5).  Here s is
-// rounded once per tick.
+// s <- alpha x + (1-alpha) s  (exp_smoothing.py:59-107), as s + alpha (x - s) in double across
+// n_frames frames of one bin of NCH channels side by side (their loads in flight together).
+template <int NCH>
+__device__ __forceinline__ void smooth_frames(const float *const (&p)[NCH], long long stride_f,
+                                              int n_frames, double a, double (&s)[NCH]) {
+    for (int f = 0; f < n_frames; f++) {
+#pragma unroll
+        for (int i = 0; i < NCH; i++)
+            s[i] = fma(a, (double)__ldg(p[i] + (size_t)f * stride_f) - s[i], s[i]);
+    }
+}
+
+// One tick of smooth_frames; the carried states d are read and written back rounded to float32.  In
+// float32, (1-alpha) rounded biases the fixed point by about eps/alpha, and rounding every frame walks
+// s off by about eps/sqrt(alpha): 1e-4 and 4e-6 of the peak at N = 32, T = 5 s (alpha = 3.5e-5).
+// Here s is rounded once per tick.
 template <int NCH>
 __device__ __forceinline__ void smooth_bin(const float *const (&p)[NCH], long long stride_f,
                                            int n_frames, double a, float *const (&d)[NCH],
@@ -56,16 +68,44 @@ __device__ __forceinline__ void smooth_bin(const float *const (&p)[NCH], long lo
     double s[NCH];
 #pragma unroll
     for (int i = 0; i < NCH; i++) s[i] = *d[i];
-    for (int f = 0; f < n_frames; f++) {
-#pragma unroll
-        for (int i = 0; i < NCH; i++)
-            s[i] = fma(a, (double)__ldg(p[i] + (size_t)f * stride_f) - s[i], s[i]);
-    }
+    smooth_frames<NCH>(p, stride_f, n_frames, a, s);
 #pragma unroll
     for (int i = 0; i < NCH; i++) {
         out[i] = (float)s[i];
         *d[i] = out[i];
     }
+}
+
+// dB of one smoothed bin, 10 log10(sp + 1e-30) + weight (spectrum.py:95-101,171).  The product and
+// the sum are rounded separately, as the widget's NumPy does.
+__device__ __forceinline__ float db_single(float sp, const float *__restrict__ weight, int k) {
+    float v = __fmul_rn(kLog10Scale, lg2_fast(sp + 1e-30f));
+    if (weight) v = __fadd_rn(v, __ldg(weight + k));
+    return v;
+}
+
+// The transfer function 10 log10(sp2 + 1e-30) - 10 log10(sp1 + 1e-30) (spectrum.py:168-169), as the
+// log of the ratio in double: two float32 dB values near -160 dB carry an ulp of 1.5e-5 dB each, and a
+// silent reference against a loud measurement gives a ratio past the float32 range (1e10 / 1e-30).
+__device__ __forceinline__ float db_dual(float sp1, float sp2) {
+    return (float)(10.0 * log10(((double)sp2 + 1e-30) / ((double)sp1 + 1e-30)));
+}
+
+// The first arg-max of the harmonic product spectrum of sp[0 .. nbins), 3 harmonics
+// (spectrum.py:103-123), in double: a float32 product of three quiet bins (power 1e-16) underflows to
+// 0 and the arg-max falls to index 0.
+__device__ __forceinline__ int hps_argmax(const float *sp, int nbins, double *s_val, int *s_idx) {
+    const int h = nbins / 3;
+    double bestp = -INFINITY;
+    int besti = 0x7fffffff;
+    for (int k = threadIdx.x; k < h; k += blockDim.x) {
+        const double r = (double)sp[k] * sp[2 * k] * sp[3 * k];
+        if (r > bestp) {
+            bestp = r;
+            besti = k;
+        }
+    }
+    return block_argmax(bestp, besti, s_val, s_idx);
 }
 
 // DUAL = false: one channel, dB = 10 log10(sp + 1e-30) + weight (spectrum.py:171).
@@ -95,18 +135,14 @@ spectrum_reduce_kernel(const float *__restrict__ power, const float *__restrict_
             float sp[2];
             smooth_bin<2>(pk, stride_f, n_frames, a, dk, sp);
             s_sp[k] = sp[0];
-            // the log of the ratio in double: two float32 dB values near -160 dB carry an ulp of
-            // 1.5e-5 dB each, and a silent reference against a loud measurement gives a ratio
-            // past the float32 range (1e10 / 1e-30)
-            v = (float)(10.0 * log10(((double)sp[1] + 1e-30) / ((double)sp[0] + 1e-30)));
+            v = db_dual(sp[0], sp[1]);
         } else {
             const float *const pk[1] = {p + k};
             float *const dk[1] = {d + k};
             float sp[1];
             smooth_bin<1>(pk, stride_f, n_frames, a, dk, sp);
             s_sp[k] = sp[0];
-            v = kLog10Scale * lg2_fast(sp[0] + 1e-30f);   // spectrum.py:95-101
-            if (weight) v += __ldg(weight + k);
+            v = db_single(sp[0], weight, k);
         }
         db[(size_t)c * nbins + k] = v;
         if (v > best) {     // on the stored float32 value, so that db[imax] == max(db)
@@ -115,19 +151,7 @@ spectrum_reduce_kernel(const float *__restrict__ power, const float *__restrict_
         }
     }
     const int imax = block_argmax(best, besti, s_val, s_idx);      // spectrum.py:175
-    // harmonic product spectrum, 3 harmonics (spectrum.py:103-123), in double: a float32 product
-    // of three quiet bins (power 1e-16) underflows to 0 and the arg-max falls to index 0
-    const int h = nbins / 3;
-    double bestp = -INFINITY;
-    besti = 0x7fffffff;
-    for (int k = threadIdx.x; k < h; k += blockDim.x) {
-        const double r = (double)s_sp[k] * s_sp[2 * k] * s_sp[3 * k];
-        if (r > bestp) {
-            bestp = r;
-            besti = k;
-        }
-    }
-    const int ipitch = block_argmax(bestp, besti, s_val, s_idx);   // spectrum.py:180
+    const int ipitch = hps_argmax(s_sp, nbins, s_val, s_idx);      // spectrum.py:180
     if (threadIdx.x == 0) {
         fmax_idx[c] = imax;
         pitch_idx[c] = ipitch;
@@ -174,6 +198,199 @@ extern "C" int frt_spectrum_reduce_dual(frt_handle h, const float *power1_dev,
     return frt_launch(h, spectrum_reduce_kernel<true>, n_pairs, 256, smem, (cudaStream_t)stream,
                       power1_dev, power2_dev, stride_c, stride_f, n_frames, nbins, alpha, disp1_dev, disp2_dev,
                       nullptr, db_dev, fmax_idx_dev, pitch_idx_dev);
+}
+
+// ---------------------------------------------------------------------------------------------
+// frt_spectrum_reduce_ticks / _dual_ticks: n_ticks consecutive ticks of frames_per_tick frames in one
+// call, each tick's result kept.  The smoothing is elementwise per bin and only the arg-maxes cross
+// bins, so the call runs in two kernels per group of ticks: a chain kernel walks every (channel, bin)
+// through the group's frames in order, rounding its state to float32 at every tick end as
+// smooth_bin does, and stores each tick's state row in the workspace; a stats kernel, one CTA per
+// (tick, channel), forms that tick's dB and arg-maxes from the stored rows as spectrum_reduce_kernel
+// does from its own.
+namespace {
+
+struct SpecTicks {
+    const float *power[2];   // [C][frames][nbins] (strides in floats) at the group's first frame
+    long long stride_c, stride_f;
+    int n_channels, frames_per_tick, n_ticks, nbins;   // n_ticks: the group's
+    double a;
+    float *disp[2];          // [C][nbins] carried states
+    float *state[2];         // [n_ticks][C][nbins] the workspace's state rows
+    const float *weight;     // [nbins] or NULL (single mode)
+    float *db;               // [C][R][nbins] at the group's first tick, or NULL
+    int R;                   // ticks of the call: db's row count per channel
+    int *fmax_idx, *pitch_idx;   // [ticks][C] at the group's first tick
+};
+
+template <int NCH>
+__global__ void __launch_bounds__(256) spectrum_ticks_chain(SpecTicks t) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (long long)t.n_channels * t.nbins) return;
+    const size_t plane = (size_t)t.n_channels * t.nbins;
+    const size_t o = (size_t)i;   // c * nbins + k
+    const int c = (int)(i / t.nbins), k = (int)(i - (long long)c * t.nbins);
+    const float *p[NCH];
+    double s[NCH];
+#pragma unroll
+    for (int j = 0; j < NCH; j++) {
+        p[j] = t.power[j] + (size_t)c * t.stride_c + k;
+        s[j] = t.disp[j][o];
+    }
+    const size_t tick_stride = (size_t)t.frames_per_tick * t.stride_f;
+    for (int r = 0; r < t.n_ticks; r++) {
+        smooth_frames<NCH>(p, t.stride_f, t.frames_per_tick, t.a, s);
+#pragma unroll
+        for (int j = 0; j < NCH; j++) {
+            const float v = (float)s[j];
+            t.state[j][(size_t)r * plane + o] = v;
+            s[j] = v;
+            p[j] += tick_stride;
+        }
+    }
+#pragma unroll
+    for (int j = 0; j < NCH; j++) t.disp[j][o] = (float)s[j];
+}
+
+template <bool DUAL>
+__global__ void __launch_bounds__(256) spectrum_ticks_stats(SpecTicks t) {
+    __shared__ double s_val[32];
+    __shared__ int s_idx[33];
+    const int r = blockIdx.x / t.n_channels, c = blockIdx.x - r * t.n_channels;
+    const size_t row = ((size_t)r * t.n_channels + c) * t.nbins;
+    const float *sp = t.state[0] + row;
+    float *db = t.db ? t.db + ((size_t)c * t.R + r) * t.nbins : nullptr;
+    float best = -INFINITY;
+    int besti = 0x7fffffff;
+    for (int k = threadIdx.x; k < t.nbins; k += blockDim.x) {
+        float v;
+        if constexpr (DUAL) v = db_dual(__ldg(sp + k), __ldg(t.state[1] + row + k));
+        else v = db_single(__ldg(sp + k), t.weight, k);
+        if (db) db[k] = v;
+        if (v > best) {     // on the float32 value, as spectrum_reduce_kernel
+            best = v;
+            besti = k;
+        }
+    }
+    const int imax = block_argmax(best, besti, s_val, s_idx);
+    const int ipitch = hps_argmax(sp, t.nbins, s_val, s_idx);
+    if (threadIdx.x == 0) {
+        t.fmax_idx[(size_t)r * t.n_channels + c] = imax;
+        t.pitch_idx[(size_t)r * t.n_channels + c] = ipitch;
+    }
+}
+
+}   // namespace
+
+// Ticks run in groups whose state rows fit this budget; at least one tick per group.
+constexpr size_t SPEC_TICKS_BUDGET = size_t(256) << 20;
+
+// Both entry points: the checks they add to frt_spectrum_reduce's, the workspace and the groups.
+// nch = 1 (single) or 2 (dual: power[1], disp[1] the measurement).  `work` is false when there is
+// nothing to do.
+static int spectrum_ticks_checks(frt_ctx *h, int n_channels, int frames_per_tick, int n_ticks, int nbins,
+                                 float alpha, bool buffers, bool &work) {
+    work = false;
+    FRT_CHECK_ARG(h, n_channels >= 0 && n_ticks >= 0 && nbins >= 3, "bad shape");
+    FRT_CHECK_ARG(h, frames_per_tick >= 1 && frames_per_tick <= 8192,
+                  "frames_per_tick must be in 1..8192, the reference's 8192-tap kernel");
+    FRT_CHECK_ARG(h, alpha > 0.f && alpha <= 1.f, "alpha must be in (0, 1]");
+    if (n_channels == 0 || n_ticks == 0) return FRT_OK;
+    FRT_CHECK_ARG(h, buffers, "NULL buffer");
+    FRT_CHECK_ARG(h, sizeof(float) * (size_t)nbins <= 200 * 1024, "nbins too large");
+    work = true;
+    return FRT_OK;
+}
+
+template <int NCH>
+static int spectrum_ticks_run(frt_ctx *h, SpecTicks t, int n_ticks, cudaStream_t st) {
+    const size_t per_tick = NCH * (size_t)t.n_channels * t.nbins * sizeof(float);
+    size_t g = SPEC_TICKS_BUDGET / per_tick;
+    g = g < 1 ? 1 : g > (size_t)n_ticks ? (size_t)n_ticks : g;
+    const cudaError_t e = h->spec_ticks_ws.grow(g * per_tick);
+    if (e == cudaErrorMemoryAllocation) {
+        cudaGetLastError();
+        return frt_fail(h, FRT_ENOMEM, "the state rows of one tick (%zu bytes) do not fit", per_tick);
+    }
+    FRT_CUDA(h, e);
+    float *ws = (float *)h->spec_ticks_ws.get();
+    for (int j = 0; j < NCH; j++) t.state[j] = ws + (size_t)j * g * t.n_channels * t.nbins;
+    const long long items = (long long)t.n_channels * t.nbins;
+    const unsigned chain_blocks = (unsigned)((items + 255) / 256);
+    const SpecTicks first = t;
+    int rc = FRT_OK;
+    for (int r0 = 0; r0 < n_ticks && rc == FRT_OK; r0 += (int)g) {
+        t.n_ticks = std::min((int)g, n_ticks - r0);
+        const size_t f0 = (size_t)r0 * t.frames_per_tick;
+        for (int j = 0; j < NCH; j++) t.power[j] = first.power[j] + f0 * t.stride_f;
+        t.db = first.db ? first.db + (size_t)r0 * t.nbins : nullptr;
+        t.fmax_idx = first.fmax_idx + (size_t)r0 * t.n_channels;
+        t.pitch_idx = first.pitch_idx + (size_t)r0 * t.n_channels;
+        rc = frt_launch(h, spectrum_ticks_chain<NCH>, chain_blocks, 256, 0, st, t);
+        if (rc == FRT_OK)
+            rc = frt_launch(h, spectrum_ticks_stats<NCH == 2>, (unsigned)(t.n_ticks * t.n_channels), 256, 0, st, t);
+    }
+    return rc;
+}
+
+extern "C" int frt_spectrum_reduce_ticks(frt_handle h, const float *power_dev, int64_t stride_c,
+                                         int64_t stride_f, int n_channels, int frames_per_tick,
+                                         int n_ticks, int nbins, float alpha, float *disp_dev,
+                                         const float *weight_dev, float *db_dev, int *fmax_idx_dev,
+                                         int *pitch_idx_dev, void *stream) {
+    if (!h) return FRT_EINVAL;
+    DeviceGuard g(h->device);
+    bool work;
+    const int rc = spectrum_ticks_checks(h, n_channels, frames_per_tick, n_ticks, nbins, alpha,
+                                         power_dev && disp_dev && fmax_idx_dev && pitch_idx_dev, work);
+    if (rc != FRT_OK || !work) return rc;
+    SpecTicks t{};
+    t.power[0] = power_dev;
+    t.stride_c = stride_c;
+    t.stride_f = stride_f;
+    t.n_channels = n_channels;
+    t.frames_per_tick = frames_per_tick;
+    t.nbins = nbins;
+    t.a = alpha;
+    t.disp[0] = disp_dev;
+    t.weight = weight_dev;
+    t.db = db_dev;
+    t.R = n_ticks;
+    t.fmax_idx = fmax_idx_dev;
+    t.pitch_idx = pitch_idx_dev;
+    return spectrum_ticks_run<1>(h, t, n_ticks, (cudaStream_t)stream);
+}
+
+extern "C" int frt_spectrum_reduce_dual_ticks(frt_handle h, const float *power1_dev,
+                                              const float *power2_dev, int64_t stride_c,
+                                              int64_t stride_f, int n_pairs, int frames_per_tick,
+                                              int n_ticks, int nbins, float alpha, float *disp1_dev,
+                                              float *disp2_dev, float *db_dev, int *fmax_idx_dev,
+                                              int *pitch_idx_dev, void *stream) {
+    if (!h) return FRT_EINVAL;
+    DeviceGuard g(h->device);
+    bool work;
+    const int rc = spectrum_ticks_checks(h, n_pairs, frames_per_tick, n_ticks, nbins, alpha,
+                                         power1_dev && power2_dev && disp1_dev && disp2_dev &&
+                                             fmax_idx_dev && pitch_idx_dev,
+                                         work);
+    if (rc != FRT_OK || !work) return rc;
+    SpecTicks t{};
+    t.power[0] = power1_dev;
+    t.power[1] = power2_dev;
+    t.stride_c = stride_c;
+    t.stride_f = stride_f;
+    t.n_channels = n_pairs;
+    t.frames_per_tick = frames_per_tick;
+    t.nbins = nbins;
+    t.a = alpha;
+    t.disp[0] = disp1_dev;
+    t.disp[1] = disp2_dev;
+    t.db = db_dev;
+    t.R = n_ticks;
+    t.fmax_idx = fmax_idx_dev;
+    t.pitch_idx = pitch_idx_dev;
+    return spectrum_ticks_run<2>(h, t, n_ticks, (cudaStream_t)stream);
 }
 
 // ---------------------------------------------------------------------------------------------

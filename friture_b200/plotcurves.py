@@ -236,10 +236,35 @@ class SpectrumPlot(_PlotState):
             return self._last
         if db.dim() != 2:
             raise ValueError("db must be [C, K]")
-        fmax = np.broadcast_to(np.asarray(fmax, dtype=np.float64), (self.n_channels,))
-        fpitch = np.broadcast_to(np.asarray(fpitch, dtype=np.float64), (self.n_channels,))
-        y, z, peak, z_peak = self._run(db[:, None, :], self.peaks_enabled)
-        x_left, x_right = self.edges(db.shape[1])
+        fmax, fpitch = self._trackers(fmax, fpitch)
+        return self._publish(self._run(db[:, None, :], self.peaks_enabled), db.shape[1], fmax, fpitch)
+
+    def push_ticks(self, ticks):
+        """``SpectrumAnalyzer.process_ticks``'s outputs (a ``SpectrumTicks`` with dB): the widget's
+        setdata once per tick, in tick order, in one launch -- the peak state steps through every
+        tick.  The curves are those after the last tick, with that tick's frequency trackers: the
+        same as one ``push`` per tick.  With no ticks, or while paused, nothing changes and the
+        previous call's curves are returned (None before the first)."""
+        if self.paused:
+            return self._last
+        db = ticks.db
+        if db is None:
+            raise ValueError("the ticks carry no dB (process_ticks was called with want_db=False)")
+        if db.dim() != 3:
+            raise ValueError("db must be [C, n_ticks, K]")
+        if db.shape[1] == 0:
+            return self._last
+        fmax, fpitch = self._trackers(ticks.fmax_hz[-1], ticks.fpitch_hz[-1])
+        return self._publish(self._run(db, self.peaks_enabled), db.shape[2], fmax, fpitch)
+
+    def _trackers(self, fmax, fpitch):
+        return (np.broadcast_to(np.asarray(fmax, dtype=np.float64), (self.n_channels,)),
+                np.broadcast_to(np.asarray(fpitch, dtype=np.float64), (self.n_channels,)))
+
+    def _publish(self, curves, nbins, fmax, fpitch):
+        """The drawing data of one call from its curves and its last tick's frequency trackers."""
+        y, z, peak, z_peak = curves
+        x_left, x_right = self.edges(nbins)
         baseline = 1.0 - to_screen(Linear, self.spec_min, self.spec_max, 0.0) if self.data_baseline else 1.0
         self._last = SpectrumCurves(
             x_left, x_right, baseline, y, z, peak, z_peak, fmax_hz=fmax, fpitch_hz=fpitch,

@@ -10,15 +10,26 @@ the two."""
 from __future__ import annotations
 
 from ctypes import c_float
+from dataclasses import dataclass
 
 import numpy as np
 
 from . import _lib
-from .audioproc import SAMPLING_RATE, audioproc, frame_count
+from .audioproc import FRAMES_PER_BUFFER, SAMPLING_RATE, audioproc, frame_count
 
 DEFAULT_FFT_SIZE = 8192        # friture/spectrum_settings.py:27 (2**7 * 32 ... the widget default)
 DEFAULT_RESPONSE_TIME = 0.025  # friture/spectrum_settings.py
 OVERLAP = 0.75                 # friture/spectrum.py:66
+MAX_FRAMES_PER_TICK = 8192     # the frames one tick may smooth (the reference's 8192-tap kernel)
+
+
+@dataclass
+class SpectrumTicks:
+    """``SpectrumAnalyzer.process_ticks``'s outputs, one row per tick: ``db`` CUDA float32
+    [C, R, bins] (None when not requested), ``fmax_hz`` and ``fpitch_hz`` host float64 [R, C]."""
+    db: object
+    fmax_hz: np.ndarray
+    fpitch_hz: np.ndarray
 
 
 class SpectrumAnalyzer:
@@ -74,18 +85,11 @@ class SpectrumAnalyzer:
         [C, 2, T] input, dB is the transfer function 10 log10(sp2) - 10 log10(sp1), unweighted, and
         fmax its peak; otherwise dB is 10 log10(sp1) + weighting of row 0.  The pitch always comes
         from row 0 (spectrum.py:180)."""
-        import torch
-        if x.dim() == 1:
-            x = x[None, :]
-        if x.dim() not in (2, 3) or (x.dim() == 3 and x.shape[1] != 2):
-            raise ValueError("expected [C, T] or [C, 2, T] input, got %s" % (tuple(x.shape),))
-        C = x.shape[0]
-        if C != self.n_channels:
-            raise ValueError("expected %d channels" % self.n_channels)
-        if x.dim() == 3 and self.dual_channels:
+        x, dual = self._input(x)
+        if dual:
             return self._process_dual(x, stream)
-        if x.dim() == 3:
-            x = x[:, 0]
+        import torch
+        C = x.shape[0]
         nb = self.fft_size // 2 + 1
         nf = frame_count(x.shape[1], self.fft_size, self.hop)
         with _lib.call_stream(x.device, stream) as sp:
@@ -106,6 +110,87 @@ class SpectrumAnalyzer:
                 # (spectrum.py:142,158-159): dispbuffers2 * (1-alpha)^frames
                 self._disp2.mul_((1. - self.alpha) ** nf)
             return self._indices_to_hz(db, imax, ipitch)
+
+    def _input(self, x):
+        """x as [C, T] or [C, 2, T] and whether it runs in dual mode; [C, 2, T] outside dual mode is
+        its reference rows."""
+        if x.dim() == 1:
+            x = x[None, :]
+        if x.dim() not in (2, 3) or (x.dim() == 3 and x.shape[1] != 2):
+            raise ValueError("expected [C, T] or [C, 2, T] input, got %s" % (tuple(x.shape),))
+        if x.shape[0] != self.n_channels:
+            raise ValueError("expected %d channels" % self.n_channels)
+        if x.dim() == 3 and self.dual_channels:
+            return x, True
+        return (x[:, 0] if x.dim() == 3 else x), False
+
+    def default_frames_per_tick(self):
+        """The frames of one tick of the widget's feed: one 512-sample buffer per tick
+        (friture/audiobackend.py:32), at least one frame."""
+        return max(1, FRAMES_PER_BUFFER // self.hop)
+
+    def tick_geometry(self, n_samples, frames_per_tick=None):
+        """(frames_per_tick, ticks) of a ``process_ticks`` call over ``n_samples`` samples per row;
+        raises FrtValueError unless the frames are a whole number of ticks of 1..8192 frames."""
+        g = self.default_frames_per_tick() if frames_per_tick is None else frames_per_tick
+        if isinstance(g, (bool, np.bool_)) or not isinstance(g, (int, np.integer)) or \
+                not 1 <= g <= MAX_FRAMES_PER_TICK:
+            raise _lib.FrtValueError(_lib.FRT_EINVAL, "frames_per_tick must be an integer in 1..%d, got %r"
+                                     % (MAX_FRAMES_PER_TICK, frames_per_tick))
+        nf = frame_count(n_samples, self.fft_size, self.hop)
+        if nf % g:
+            raise _lib.FrtValueError(_lib.FRT_EINVAL, "%d frames are not a whole number of %d-frame ticks"
+                                     % (nf, g))
+        return int(g), nf // g
+
+    # -- many ticks --------------------------------------------------------------------------
+    def process_ticks(self, x, frames_per_tick=None, want_db=True, stream=None):
+        """R = frames / frames_per_tick consecutive ticks in one call: x as for ``process``, holding
+        the frames of all of them (tick r is x[..., r*g*hop : (r+1)*g*hop + N - hop] for g =
+        frames_per_tick, by default the widget's feed, ``default_frames_per_tick()``).  Returns a
+        ``SpectrumTicks`` with every tick's row: the same bits as R ``process`` calls on those
+        slices, and the same carried states afterwards.  One STFT launch, one reduction call and
+        one read of each index array for all R ticks."""
+        import torch
+        x, dual = self._input(x)
+        g, R = self.tick_geometry(x.shape[-1], frames_per_tick)
+        C = self.n_channels
+        nb = self.fft_size // 2 + 1
+        nf = g * R
+        dev = x.device
+        with _lib.call_stream(dev, stream) as sp:
+            rows = x.view(2 * C, x.shape[-1]) if dual else x
+            power = self.proc.stft(rows, hop=self.hop, log=False, stream=stream)
+            if self._disp is None:
+                self._disp = torch.zeros((C, nb), dtype=torch.float32, device=dev)
+            if dual and self._disp2 is None:
+                self._disp2 = torch.zeros((C, nb), dtype=torch.float32, device=dev)
+            if not dual and self._w_dev is None:
+                self._w_dev = torch.from_numpy(np.ascontiguousarray(self.w, dtype=np.float32)).to(dev)
+            db = torch.empty((C, R, nb), dtype=torch.float32, device=dev) if want_db else None
+            imax = torch.empty((R, C), dtype=torch.int32, device=dev)
+            ipitch = torch.empty((R, C), dtype=torch.int32, device=dev)
+            if R:
+                h = self.proc.handle
+                if dual:
+                    # power [2C, nf, nb]: pair c's reference at row 2c, its measurement at row 2c + 1
+                    p1 = power.data_ptr()
+                    h.call("frt_spectrum_reduce_dual_ticks", _lib._ptr(p1), _lib._ptr(p1 + 4 * nf * nb),
+                           int(2 * nf * nb), int(nb), int(C), g, int(R), int(nb), c_float(self.alpha),
+                           _lib._ptr(self._disp), _lib._ptr(self._disp2), _lib._ptr(db), _lib._ptr(imax),
+                           _lib._ptr(ipitch), sp)
+                else:
+                    h.call("frt_spectrum_reduce_ticks", _lib._ptr(power), int(nf * nb), int(nb), int(C), g,
+                           int(R), int(nb), c_float(self.alpha), _lib._ptr(self._disp),
+                           _lib._ptr(self._w_dev) if self.weighting else None, _lib._ptr(db),
+                           _lib._ptr(imax), _lib._ptr(ipitch), sp)
+                    if self._disp2 is not None:
+                        # process's decay of the unfilled second state, once per tick: each rounds
+                        decay = (1. - self.alpha) ** g
+                        for _ in range(R):
+                            self._disp2.mul_(decay)
+            _, fmax, fpitch = self._indices_to_hz(None, imax, ipitch)
+            return SpectrumTicks(db, fmax, fpitch)
 
     def _indices_to_hz(self, db, imax, ipitch):
         # on the call's stream, which is current: the reads wait for the kernel that writes them

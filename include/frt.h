@@ -303,6 +303,30 @@ int frt_spectrum_reduce_dual(frt_handle h, const float *power1_dev, const float 
                              int nbins, float alpha, float *disp1_dev, float *disp2_dev,
                              float *db_dev, int *fmax_idx_dev, int *pitch_idx_dev, void *stream);
 
+/* n_ticks consecutive ticks of frames_per_tick frames each in one call, each tick's result kept: tick
+ * r covers frames r*frames_per_tick .. (r+1)*frames_per_tick - 1 of power_dev [C][n_frames][nbins].
+ * db_dev [C][n_ticks][nbins] (contiguous) or NULL for no dB; fmax_idx_dev / pitch_idx_dev
+ * [n_ticks][C].  Every row, and disp_dev afterwards, are the same bits as n_ticks
+ * frt_spectrum_reduce calls, one per tick.  Argument checks as frt_spectrum_reduce, with
+ * frames_per_tick in 1..8192; n_ticks == 0 or n_channels == 0 does nothing.  The ticks run in groups
+ * within a grow-only workspace of 4*C*nbins bytes per tick, kept within 256 MiB (one tick at least;
+ * FRT_ENOMEM, handle usable, when it cannot grow); such a call is asynchronous on `stream` unless the
+ * workspace has to grow.                                                                          */
+int frt_spectrum_reduce_ticks(frt_handle h, const float *power_dev, int64_t stride_c,
+                              int64_t stride_f, int n_channels, int frames_per_tick, int n_ticks,
+                              int nbins, float alpha, float *disp_dev, const float *weight_dev,
+                              float *db_dev, int *fmax_idx_dev, int *pitch_idx_dev, void *stream);
+
+/* frt_spectrum_reduce_dual over n_ticks ticks, as frt_spectrum_reduce_ticks over
+ * frt_spectrum_reduce: db_dev [P][n_ticks][nbins] or NULL, fmax_idx_dev / pitch_idx_dev
+ * [n_ticks][P], disp1_dev and disp2_dev the same bits afterwards as n_ticks frt_spectrum_reduce_dual
+ * calls.  The workspace holds both states' rows, 8*P*nbins bytes per tick.                       */
+int frt_spectrum_reduce_dual_ticks(frt_handle h, const float *power1_dev, const float *power2_dev,
+                                   int64_t stride_c, int64_t stride_f, int n_pairs,
+                                   int frames_per_tick, int n_ticks, int nbins, float alpha,
+                                   float *disp1_dev, float *disp2_dev, float *db_dev,
+                                   int *fmax_idx_dev, int *pitch_idx_dev, void *stream);
+
 /* ---------------------------------------------------------------- plotted curves and peak hold
  * The last numeric step of the spectrum and octave widgets: SpectrumPlotWidget.setdata and
  * compute_peaks (friture/spectrumPlotWidget.py:122-200), HistPlot.setdata and compute_peaks
