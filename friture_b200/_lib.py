@@ -111,6 +111,10 @@ SIGNATURES = {
     "frt_display_columns": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int, c_int, c_int,
                                     c_void_p, c_float, c_float, c_void_p, c_void_p, c_int, c_void_p,
                                     c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "frt_stft_screen_rows": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int64, c_int, c_void_p, c_float,
+                                     c_float, c_void_p, c_void_p, c_int, c_void_p, c_int64, c_int64, c_void_p]),
+    "frt_display_rows": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int, c_int, c_int, c_void_p, c_void_p,
+                                 c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
 }
 
 _lib = None

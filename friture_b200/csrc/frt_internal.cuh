@@ -270,6 +270,28 @@ __device__ __forceinline__ float lg2_fast(float v) {
 }
 constexpr float kLog10Scale = 3.01029995663981195f;   // 10 / log2(10): 10 log10(v) = kLog10Scale log2(v)
 
+// One screen row of a log-power column: np.interp between bins i0 and i0+1 of
+// (dB + w - spec_min) / (spec_max - spec_min) (friture/spectrogram.py:127-129,161-162;
+// friture/signal/frequency_resampler.py:67-83), unclipped.  The column is read from global memory
+// through the read-only path (display_kernel) or, SMEM, from the STFT kernels' shared-memory column
+// (stft.cu).
+template <bool SMEM = false>
+__device__ __forceinline__ float screen_value(const float *__restrict__ col, const float *__restrict__ weight,
+                                              int i0, float t, float spec_min, float inv_range) {
+    auto ld = [](const float *p) {
+        if constexpr (SMEM) return *p;
+        else return __ldg(p);
+    };
+    float a = ld(col + i0), b = ld(col + i0 + 1);
+    if (weight) {
+        a += __ldg(weight + i0);
+        b += __ldg(weight + i0 + 1);
+    }
+    a = (a - spec_min) * inv_range;
+    b = (b - spec_min) * inv_range;
+    return fmaf(t, b - a, a);
+}
+
 // cp.async: global -> shared copies that bypass the registers, waited for by commit group
 __device__ __forceinline__ unsigned smem_u32(const void *p) {
     return (unsigned)__cvta_generic_to_shared(p);

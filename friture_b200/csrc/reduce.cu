@@ -501,22 +501,21 @@ extern "C" int frt_plot_curves(frt_handle h, const float *y_dev, int64_t stride_
 // (friture/signal/color_tranform.py:48-51, friture/signal/lookup_table.py:32-52), one kernel.
 // The host works out which input column feeds which output column and with what weight (the
 // resampler's scalar bookkeeping); the kernel is one thread per output pixel.
+// ROWS = false: db holds log-power columns [C][n_frames][nbins] and each screen value is
+// screen_value of two bins.  ROWS = true: db holds screen rows [C][n_frames][height] that
+// frt_stft_screen_rows already interpolated (weight, spec_min, inv_range, row_i0 and row_t are not
+// read), and the value of row r is read directly.  Both keep the same resampling expression.
 namespace {
 
-__device__ __forceinline__ float screen_value(const float *__restrict__ col,
-                                              const float *__restrict__ weight, int i0, float t,
-                                              float spec_min, float inv_range) {
-    // np.interp between bins i0 and i0+1 of (dB + w - spec_min) / (spec_max - spec_min)
-    float a = __ldg(col + i0), b = __ldg(col + i0 + 1);
-    if (weight) {
-        a += __ldg(weight + i0);
-        b += __ldg(weight + i0 + 1);
-    }
-    a = (a - spec_min) * inv_range;
-    b = (b - spec_min) * inv_range;
-    return fmaf(t, b - a, a);
+// the screen value of row r in the input column at col
+template <bool ROWS>
+__device__ __forceinline__ float display_value(const float *col, const float *__restrict__ weight, int r, int i0,
+                                               float t, float spec_min, float inv_range) {
+    if constexpr (ROWS) return __ldg(col + r);
+    else return screen_value(col, weight, i0, t, spec_min, inv_range);
 }
 
+template <bool ROWS>
 __global__ void display_kernel(const float *__restrict__ db, long long stride_c, long long stride_f,
                                int n_frames, const float *__restrict__ weight, float spec_min,
                                float inv_range, const int *__restrict__ row_i0,
@@ -531,14 +530,14 @@ __global__ void display_kernel(const float *__restrict__ db, long long stride_c,
     const int r = (int)(gid / (n_out > 0 ? n_out : 1));
     const int o = (int)(gid - (long long)r * (n_out > 0 ? n_out : 1));
     const float *base = db + (size_t)c * stride_c;
-    const int i0 = __ldg(row_i0 + r);
-    const float t = __ldg(row_t + r);
+    const int i0 = ROWS ? 0 : __ldg(row_i0 + r);
+    const float t = ROWS ? 0.f : __ldg(row_t + r);
     if (n_out > 0) {
         const int j = __ldg(out_col + o);       // input column this output column is drawn from
         const float a = __ldg(out_a + o);       // weight of the previous input column
-        const float cur = screen_value(base + (size_t)j * stride_f, weight, i0, t, spec_min, inv_range);
-        const float old = (j > 0) ? screen_value(base + (size_t)(j - 1) * stride_f, weight, i0, t,
-                                                 spec_min, inv_range)
+        const float cur = display_value<ROWS>(base + (size_t)j * stride_f, weight, r, i0, t, spec_min, inv_range);
+        const float old = (j > 0) ? display_value<ROWS>(base + (size_t)(j - 1) * stride_f, weight, r, i0, t,
+                                                        spec_min, inv_range)
                                   : old_data[(size_t)c * height + r];
         float v = cur * (1.0f - a) + old * a;   // linear_interp.py:56-59
         v = fminf(fmaxf(v, 0.f), 1.f);          // color_tranform.py:50
@@ -547,8 +546,31 @@ __global__ void display_kernel(const float *__restrict__ db, long long stride_c,
     // carry the last column of this tick (online_linear_2D_resampler.py "shift"); one writer per row
     // and only after every reader of the old value is done -> done by a second launch (n_out == 0)
     if (n_out == 0 && n_frames > 0)
-        old_data[(size_t)c * height + r] =
-            screen_value(base + (size_t)(n_frames - 1) * stride_f, weight, i0, t, spec_min, inv_range);
+        old_data[(size_t)c * height + r] = display_value<ROWS>(base + (size_t)(n_frames - 1) * stride_f, weight, r,
+                                                               i0, t, spec_min, inv_range);
+}
+
+// Both entry points: the pixels (n_out > 0), then the carried column in a second launch.
+int display_run(frt_ctx *h, bool rows, const float *src, int64_t stride_c, int64_t stride_f, int n_channels,
+                int n_frames, const float *weight, float spec_min, float inv_range, const int *row_i0,
+                const float *row_t, int height, const int *out_col, const float *out_a, int n_out,
+                float *old_data, const uint32_t *lut, uint32_t *pixels, cudaStream_t st) {
+    auto launch = [&](auto kernel) {
+        if (n_out > 0) {
+            const long long total = (long long)height * n_out;
+            dim3 grid((unsigned)((total + 255) / 256), (unsigned)n_channels);
+            const int rc = frt_launch(h, kernel, grid, 256, 0, st, src, stride_c, stride_f, n_frames, weight,
+                                      spec_min, inv_range, row_i0, row_t, height, out_col, out_a, n_out,
+                                      old_data, reinterpret_cast<const unsigned *>(lut),
+                                      reinterpret_cast<unsigned *>(pixels));
+            if (rc) return rc;
+        }
+        dim3 grid2((unsigned)((height + 255) / 256), (unsigned)n_channels);
+        return frt_launch(h, kernel, grid2, 256, 0, st, src, stride_c, stride_f, n_frames, weight, spec_min,
+                          inv_range, row_i0, row_t, height, nullptr, nullptr, 0, old_data,
+                          reinterpret_cast<const unsigned *>(lut), nullptr);
+    };
+    return rows ? launch(display_kernel<true>) : launch(display_kernel<false>);
 }
 
 }   // namespace
@@ -569,19 +591,22 @@ extern "C" int frt_display_columns(frt_handle h, const float *db_dev, int64_t st
     FRT_CHECK_ARG(h, db_dev && row_i0_dev && row_t_dev && old_data_dev && lut_dev, "NULL buffer");
     FRT_CHECK_ARG(h, n_out == 0 || (out_col_dev && out_a_dev && pixels_dev), "NULL output buffer");
     const float inv_range = 1.0f / (spec_max - spec_min);
-    cudaStream_t st = (cudaStream_t)stream;
-    if (n_out > 0) {
-        const long long total = (long long)height * n_out;
-        dim3 grid((unsigned)((total + 255) / 256), (unsigned)n_channels);
-        const int rc = frt_launch(h, display_kernel, grid, 256, 0, st, db_dev, stride_c, stride_f, n_frames,
-                                  weight_dev, spec_min, inv_range, row_i0_dev, row_t_dev, height,
-                                  out_col_dev, out_a_dev, n_out, old_data_dev,
-                                  reinterpret_cast<const unsigned *>(lut_dev),
-                                  reinterpret_cast<unsigned *>(pixels_dev));
-        if (rc) return rc;
-    }
-    dim3 grid2((unsigned)((height + 255) / 256), (unsigned)n_channels);
-    return frt_launch(h, display_kernel, grid2, 256, 0, st, db_dev, stride_c, stride_f, n_frames, weight_dev,
-                      spec_min, inv_range, row_i0_dev, row_t_dev, height, nullptr, nullptr, 0, old_data_dev,
-                      reinterpret_cast<const unsigned *>(lut_dev), nullptr);
+    return display_run(h, false, db_dev, stride_c, stride_f, n_channels, n_frames, weight_dev, spec_min, inv_range,
+                       row_i0_dev, row_t_dev, height, out_col_dev, out_a_dev, n_out, old_data_dev, lut_dev,
+                       pixels_dev, (cudaStream_t)stream);
+}
+
+extern "C" int frt_display_rows(frt_handle h, const float *rows_dev, int64_t stride_c, int64_t stride_f,
+                                int n_channels, int n_frames, int height, const int *out_col_dev,
+                                const float *out_a_dev, int n_out, float *old_data_dev,
+                                const uint32_t *lut_dev, uint32_t *pixels_dev, void *stream) {
+    if (!h) return FRT_EINVAL;
+    DeviceGuard g(h->device);
+    FRT_CHECK_ARG(h, n_channels >= 0 && n_frames >= 0 && height >= 1 && n_out >= 0, "bad shape");
+    if (n_channels == 0 || n_frames == 0) return FRT_OK;
+    FRT_CHECK_ARG(h, rows_dev && old_data_dev && lut_dev, "NULL buffer");
+    FRT_CHECK_ARG(h, n_out == 0 || (out_col_dev && out_a_dev && pixels_dev), "NULL output buffer");
+    return display_run(h, true, rows_dev, stride_c, stride_f, n_channels, n_frames, nullptr, 0.f, 0.f, nullptr,
+                       nullptr, height, out_col_dev, out_a_dev, n_out, old_data_dev, lut_dev, pixels_dev,
+                       (cudaStream_t)stream);
 }

@@ -20,6 +20,7 @@
 //   combine through shared memory (stft_large_kernel; stft_multi_kernel for unaligned input and 16384).
 // Generic path (N = 32): one CTA per frame, Stockham radix-4 (+ one radix-2 pass when log2(M) is
 //   odd) ping-ponging between two shared-memory buffers.
+#include <algorithm>
 #include <cmath>
 #include <type_traits>
 #include <utility>
@@ -132,6 +133,28 @@ __device__ __forceinline__ float finish(float mag2, float scale) {
     // mag2*scale = |X|^2/N^2 (audioproc.py:49-50); log mode: spectrogram.py:119-125
     if (MODE == FRT_STFT_POWER) return mag2 * scale;
     return kLog10Scale * lg2_fast(fmaf(mag2, scale, kEps));
+}
+
+// Third output of the STFT kernels (frt_stft_screen_rows): the frame's log-power column, computed as
+// FRT_STFT_LOGPOWER computes it, stays in shared memory and only its `height` screen rows are written,
+// row r = screen_value of the column (what display_kernel computes from a stored column).  Each kernel
+// family has a __global__ wrapper of this mode next to its existing one; both run the same body.
+constexpr int kModeScreen = 2;
+
+struct ScreenRows {
+    const float *weight;   // [nbins] dB or NULL
+    const int *i0;         // [height] bin index of each row, 0 <= i0 <= nbins - 2
+    const float *t;        // [height] its fraction toward bin i0 + 1
+    float spec_min, inv_range;
+    int height;
+};
+
+// Rows i, i + n, .. of one frame from its column in shared memory.  The barrier before it makes the
+// column's values opaque to the compiler, so that no contraction reaches across into screen_value.
+__device__ __forceinline__ void write_rows(const float *s_col, float *__restrict__ rows, const ScreenRows &s,
+                                           int i, int n) {
+    for (int r = i; r < s.height; r += n)
+        rows[r] = screen_value<true>(s_col, s.weight, __ldg(s.i0 + r), __ldg(s.t + r), s.spec_min, s.inv_range);
 }
 
 // ---- TMA bulk copy (cp.async.bulk, SASS UBLKCP) + mbarrier helpers ------------------------------
@@ -277,17 +300,19 @@ __device__ __forceinline__ void combine_split(float *__restrict__ o, const float
     }
 }
 
+// kModeScreen: the frame's column goes to s_col, after the tiles, and its rows to out.
 template <int R, int MODE>
-__global__ void __launch_bounds__(32 * R)
-stft_multi_kernel(const float *__restrict__ x, long long x_stride, long long n_frames, int hop,
-                  float *__restrict__ out, long long out_stride_c, long long out_stride_f,
-                  const float2 *__restrict__ win2, const float2 *__restrict__ tw32,
-                  const float2 *__restrict__ comb, const float2 *__restrict__ post,
-                  long long total_items, int vec_ok) {
+__device__ __forceinline__ void
+stft_multi_body(const float *__restrict__ x, long long x_stride, long long n_frames, int hop,
+                float *__restrict__ out, long long out_stride_c, long long out_stride_f,
+                const float2 *__restrict__ win2, const float2 *__restrict__ tw32,
+                const float2 *__restrict__ comb, const float2 *__restrict__ post,
+                long long total_items, int vec_ok, const ScreenRows &scr) {
     constexpr int M = 1024 * R, N = 2 * M;
     extern __shared__ float2 smem[];
     float2 *s_tw = smem;                       // [32][32] W_1024^(k1 t)
     float2 *s_tiles = s_tw + 1024;             // R padded tiles
+    float *s_col = reinterpret_cast<float *>(s_tiles + R * TILE);   // kModeScreen: [M + 1]
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, tid = threadIdx.x;
     float2 *s_x = s_tiles + warp * TILE;
     for (int i = tid; i < 1024; i += blockDim.x) s_tw[i] = tw32[i];
@@ -317,11 +342,41 @@ stft_multi_kernel(const float *__restrict__ x, long long x_stride, long long n_f
         for (int r = 0; r < 32; r++) s_x[lane + 32 * brev5(r)] = v[r];   // natural order
         __syncthreads();
 
-        combine_split<R, MODE>(out + c * out_stride_c + f * out_stride_f, s_tiles,
-                               [=](int w, int k0) { return __ldg(comb + (w - 1) * 1024 + k0); },
-                               [=](int kk) { return __ldg(post + kk); }, tid, scale);
-        __syncthreads();
+        auto comb_at = [=](int w, int k0) { return __ldg(comb + (w - 1) * 1024 + k0); };
+        auto post_at = [=](int kk) { return __ldg(post + kk); };
+        if constexpr (MODE == kModeScreen) {
+            combine_split<R, MODE>(s_col, s_tiles, comb_at, post_at, tid, scale);
+            __syncthreads();
+            // s_col is rewritten only after the next frame's tile barrier
+            write_rows(s_col, out + c * out_stride_c + f * out_stride_f, scr, tid, 32 * R);
+        } else {
+            combine_split<R, MODE>(out + c * out_stride_c + f * out_stride_f, s_tiles, comb_at, post_at, tid,
+                                   scale);
+            __syncthreads();
+        }
     }
+}
+
+template <int R, int MODE>
+__global__ void __launch_bounds__(32 * R)
+stft_multi_kernel(const float *__restrict__ x, long long x_stride, long long n_frames, int hop,
+                  float *__restrict__ out, long long out_stride_c, long long out_stride_f,
+                  const float2 *__restrict__ win2, const float2 *__restrict__ tw32,
+                  const float2 *__restrict__ comb, const float2 *__restrict__ post,
+                  long long total_items, int vec_ok) {
+    stft_multi_body<R, MODE>(x, x_stride, n_frames, hop, out, out_stride_c, out_stride_f, win2, tw32, comb, post,
+                             total_items, vec_ok, ScreenRows{});
+}
+
+template <int R>
+__global__ void __launch_bounds__(32 * R)
+stft_multi_screen_kernel(const float *__restrict__ x, long long x_stride, long long n_frames, int hop,
+                         float *__restrict__ rows, long long rows_stride_c, long long rows_stride_f,
+                         const float2 *__restrict__ win2, const float2 *__restrict__ tw32,
+                         const float2 *__restrict__ comb, const float2 *__restrict__ post,
+                         long long total_items, int vec_ok, const ScreenRows scr) {
+    stft_multi_body<R, kModeScreen>(x, x_stride, n_frames, hop, rows, rows_stride_c, rows_stride_f, win2, tw32,
+                                    comb, post, total_items, vec_ok, scr);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -344,12 +399,19 @@ constexpr size_t small_smem() {
            (Q == 32 ? sizeof(unsigned long long) * small_warps<Q>() : 0);
 }
 
+// kModeScreen: the warp's G columns go to its tile, free again after the transpose; with TMA the tile
+// already holds the next frame by then, so each warp has a column buffer of its own after the mbarriers.
+template <int Q, bool TMA>
+constexpr size_t small_screen_smem() {
+    return small_smem<Q>() + (TMA ? sizeof(float) * (size_t)small_warps<Q>() * (32 * Q + 1) : 0);
+}
+
 template <int Q, int MODE, bool TMA>
-__global__ void __launch_bounds__(small_warps<Q>() * 32, small_ctas_per_sm<Q>())
-stft_small_kernel(const float *__restrict__ x, long long x_stride, long long n_frames, int hop,
-                  float *__restrict__ out, long long out_stride_c, long long out_stride_f,
-                  const float2 *__restrict__ win2, const float2 *__restrict__ tw,
-                  const float2 *__restrict__ post, long long total_items, int vec_ok) {
+__device__ __forceinline__ void
+stft_small_body(const float *__restrict__ x, long long x_stride, long long n_frames, int hop,
+                float *__restrict__ out, long long out_stride_c, long long out_stride_f,
+                const float2 *__restrict__ win2, const float2 *__restrict__ tw,
+                const float2 *__restrict__ post, long long total_items, int vec_ok, const ScreenRows &scr) {
     static_assert(!TMA || Q == 32, "TMA staging is for one frame per warp");
     constexpr int G = 32 / Q, M = 32 * Q, N = 2 * M, WARPS = small_warps<Q>();
     extern __shared__ float2 smem[];
@@ -451,7 +513,16 @@ stft_small_kernel(const float *__restrict__ x, long long x_stride, long long n_f
         }
         dft32(v);   // v[r] = Z_g[k1 + Q*brev5(r)] of this lane's (g, k1)
 
-        float *o = out + myc * out_stride_c + myf * out_stride_f;
+        float *o;
+        if constexpr (MODE == kModeScreen) {
+            float *s_col = reinterpret_cast<float *>(s_x);
+            if (TMA)
+                s_col = reinterpret_cast<float *>(reinterpret_cast<unsigned long long *>(s_post + 16 * Q + WARPS * TILE) +
+                                                  WARPS) + warp * (M + 1);
+            o = s_col + gsel * (M + 1);
+        } else {
+            o = out + myc * out_stride_c + myf * out_stride_f;
+        }
 #pragma unroll
         for (int m = 0; m < 16; m++) {
             const float2 z = v[brev5(m)];
@@ -477,7 +548,40 @@ stft_small_kernel(const float *__restrict__ x, long long x_stride, long long n_f
             const float2 z = v[brev5(16)];   // bin M/2: X = conj(Z)
             o[M / 2] = finish<MODE>(4.0f * fmaf(z.x, z.x, z.y * z.y), scale);
         }
+        if constexpr (MODE == kModeScreen) {
+            __syncwarp();   // the warp's G columns are complete
+            const float *s_col = o - gsel * (M + 1);
+#pragma unroll
+            for (int g = 0; g < G; g++) {   // frame g's (channel, frame) from the lanes that hold it
+                const long long cg = __shfl_sync(0xffffffffu, myc, g * Q);
+                const long long fg = __shfl_sync(0xffffffffu, myf, g * Q);
+                if (__shfl_sync(0xffffffffu, (int)myok, g * Q))
+                    write_rows(s_col + g * (M + 1), out + cg * out_stride_c + fg * out_stride_f, scr, lane, 32);
+            }
+            __syncwarp();   // every lane is done with the columns before the tile is written again
+        }
     }
+}
+
+template <int Q, int MODE, bool TMA>
+__global__ void __launch_bounds__(small_warps<Q>() * 32, small_ctas_per_sm<Q>())
+stft_small_kernel(const float *__restrict__ x, long long x_stride, long long n_frames, int hop,
+                  float *__restrict__ out, long long out_stride_c, long long out_stride_f,
+                  const float2 *__restrict__ win2, const float2 *__restrict__ tw,
+                  const float2 *__restrict__ post, long long total_items, int vec_ok) {
+    stft_small_body<Q, MODE, TMA>(x, x_stride, n_frames, hop, out, out_stride_c, out_stride_f, win2, tw, post,
+                                  total_items, vec_ok, ScreenRows{});
+}
+
+template <int Q, bool TMA>
+__global__ void __launch_bounds__(small_warps<Q>() * 32, small_ctas_per_sm<Q>())
+stft_small_screen_kernel(const float *__restrict__ x, long long x_stride, long long n_frames, int hop,
+                         float *__restrict__ rows, long long rows_stride_c, long long rows_stride_f,
+                         const float2 *__restrict__ win2, const float2 *__restrict__ tw,
+                         const float2 *__restrict__ post, long long total_items, int vec_ok,
+                         const ScreenRows scr) {
+    stft_small_body<Q, kModeScreen, TMA>(x, x_stride, n_frames, hop, rows, rows_stride_c, rows_stride_f, win2, tw,
+                                         post, total_items, vec_ok, scr);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -495,14 +599,20 @@ stft_small_kernel(const float *__restrict__ x, long long x_stride, long long n_f
 // the frame 0.5 - 0.5 cos(theta n) cancels (a relative error of up to 1.5e-2, and w[N-1] = 1e-8
 // instead of 0), so register blocks n1 = 0 and 31 take float32(Hann) from the window table, read
 // once per thread; the other blocks stay within 2.4e-6 of the exact window.
-constexpr int LARGE_WARPS = 16;
+// kModeScreen: each frame group's column goes to a buffer of its own after the tiles (the tiles are read
+// until the split step ends).  At R = 4 sixteen warps' tiles, tables and four such buffers exceed the
+// 227 KB a CTA may hold, so that instantiation runs twelve warps (three frame groups).
+template <int R, int MODE>
+__host__ __device__ constexpr int large_warps() { return (MODE == kModeScreen && R == 4) ? 12 : 16; }
 struct HannA {
     float2 v[32];     // (0.5 cos(theta 64 R n1), 0.5 sin(theta 64 R n1))
 };
-template <int R>
+template <int R, int MODE>
 constexpr size_t large_smem() {
-    // tw [1024] + comb [R-1][1024] + post [512 R + 1 -> even] + tiles
-    return sizeof(float2) * (1024 + 1024 * (R - 1) + 512 * R + 2 + (size_t)LARGE_WARPS * TILE);
+    // tw [1024] + comb [R-1][1024] + post [512 R + 1 -> even] + tiles (+ kModeScreen: the groups' columns)
+    constexpr int W = large_warps<R, MODE>();
+    return sizeof(float2) * (1024 + 1024 * (R - 1) + 512 * R + 2 + (size_t)W * TILE) +
+           (MODE == kModeScreen ? sizeof(float) * (size_t)(W / R) * (1024 * R + 1) : 0);
 }
 
 __device__ __forceinline__ void group_barrier(int id, int nthreads) {
@@ -517,15 +627,16 @@ __device__ __forceinline__ float2 post_lookup(const float2 *s_post, int kk, int 
 }
 
 template <int R, int MODE>
-__global__ void __launch_bounds__(LARGE_WARPS * 32, 1)
-stft_large_kernel(const float *__restrict__ x, long long x_stride, long long n_frames, int hop,
-                  float *__restrict__ out, long long out_stride_c, long long out_stride_f,
-                  const float2 *__restrict__ win2, const float4 *__restrict__ wlane,
-                  const float2 *__restrict__ tw32, const float2 *__restrict__ comb,
-                  const float2 *__restrict__ post, long long total_items,
-                  const __grid_constant__ HannA hann_a) {
+__device__ __forceinline__ void
+stft_large_body(const float *__restrict__ x, long long x_stride, long long n_frames, int hop,
+                float *__restrict__ out, long long out_stride_c, long long out_stride_f,
+                const float2 *__restrict__ win2, const float4 *__restrict__ wlane,
+                const float2 *__restrict__ tw32, const float2 *__restrict__ comb,
+                const float2 *__restrict__ post, long long total_items, const HannA &hann_a,
+                const ScreenRows &scr) {
     // STAG: 8-byte shared accesses are served per half-warp; the 16/R elements a half-warp sends to
     // each of the R tiles must fall on different banks
+    constexpr int LARGE_WARPS = large_warps<R, MODE>();
     constexpr int M = 1024 * R, N = 2 * M, NG = LARGE_WARPS / R, GT = 32 * R, STAG = 16 / R;
     extern __shared__ float2 smem[];
     float2 *s_tw = smem;                          // [32][32] W_1024^(k1 t)
@@ -536,6 +647,7 @@ stft_large_kernel(const float *__restrict__ x, long long x_stride, long long n_f
     const int grp = warp / R, w = warp % R, gtid = tid - grp * GT;
     float2 *s_tiles = s_tiles_all + (size_t)grp * R * TILE;   // this group's R tiles
     float2 *s_x = s_tiles + w * TILE;
+    float *s_col = reinterpret_cast<float *>(s_tiles_all + (size_t)LARGE_WARPS * TILE) + grp * (M + 1);
     for (int i = tid; i < 1024; i += blockDim.x) s_tw[i] = tw32[i];
     for (int i = tid; i < 1024 * (R - 1); i += blockDim.x) s_comb[i] = comb[i];
     for (int i = tid; i <= 512 * R; i += blockDim.x) s_post[i] = post[i];
@@ -593,7 +705,8 @@ stft_large_kernel(const float *__restrict__ x, long long x_stride, long long n_f
         for (int r = 0; r < 32; r++) s_x[lane + 32 * brev5(r)] = v[r];   // natural order
         group_barrier(1 + grp, GT);
 
-        combine_split<R, MODE>(out + c * out_stride_c + f * out_stride_f, s_tiles,
+        float *rows = out + c * out_stride_c + f * out_stride_f;
+        combine_split<R, MODE>(MODE == kModeScreen ? s_col : rows, s_tiles,
                                [=](int w, int k0) { return s_comb[(w - 1) * 1024 + k0]; },
                                [=](int kk) { return post_lookup(s_post, kk, M / 2); }, gtid, scale);
         if (++f == n_frames) {
@@ -602,7 +715,33 @@ stft_large_kernel(const float *__restrict__ x, long long x_stride, long long n_f
         }
         group_barrier(1 + grp, GT);          // every Z_w has been read: the tiles are free again
         if (item + 1 < item_end) fetch(c, f);
+        // (the group's column is written again only after the next frame's first barrier)
+        if constexpr (MODE == kModeScreen) write_rows(s_col, rows, scr, gtid, GT);
     }
+}
+
+template <int R, int MODE>
+__global__ void __launch_bounds__(large_warps<R, MODE>() * 32, 1)
+stft_large_kernel(const float *__restrict__ x, long long x_stride, long long n_frames, int hop,
+                  float *__restrict__ out, long long out_stride_c, long long out_stride_f,
+                  const float2 *__restrict__ win2, const float4 *__restrict__ wlane,
+                  const float2 *__restrict__ tw32, const float2 *__restrict__ comb,
+                  const float2 *__restrict__ post, long long total_items,
+                  const __grid_constant__ HannA hann_a) {
+    stft_large_body<R, MODE>(x, x_stride, n_frames, hop, out, out_stride_c, out_stride_f, win2, wlane, tw32, comb,
+                             post, total_items, hann_a, ScreenRows{});
+}
+
+template <int R>
+__global__ void __launch_bounds__(large_warps<R, kModeScreen>() * 32, 1)
+stft_large_screen_kernel(const float *__restrict__ x, long long x_stride, long long n_frames, int hop,
+                         float *__restrict__ rows, long long rows_stride_c, long long rows_stride_f,
+                         const float2 *__restrict__ win2, const float4 *__restrict__ wlane,
+                         const float2 *__restrict__ tw32, const float2 *__restrict__ comb,
+                         const float2 *__restrict__ post, long long total_items,
+                         const __grid_constant__ HannA hann_a, const ScreenRows scr) {
+    stft_large_body<R, kModeScreen>(x, x_stride, n_frames, hop, rows, rows_stride_c, rows_stride_f, win2, wlane,
+                                    tw32, comb, post, total_items, hann_a, scr);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -632,13 +771,15 @@ __device__ __forceinline__ void stockham_radix4(const float2 *__restrict__ in,
     }
 }
 
-__global__ void stft_generic_kernel(const float *__restrict__ x, long long x_stride,
-                                    long long n_frames, int hop, float *__restrict__ out,
-                                    long long out_stride_c, long long out_stride_f,
-                                    const float *__restrict__ win,
-                                    const float2 *__restrict__ tw,
-                                    const float2 *__restrict__ post, int mode, int n_fft,
-                                    int log2m) {
+// SCREEN: the column goes to the buffer the FFT does not end in, and the frame's rows to out.
+template <bool SCREEN>
+__device__ __forceinline__ void stft_generic_body(const float *__restrict__ x, long long x_stride,
+                                                  long long n_frames, int hop, float *__restrict__ out,
+                                                  long long out_stride_c, long long out_stride_f,
+                                                  const float *__restrict__ win,
+                                                  const float2 *__restrict__ tw,
+                                                  const float2 *__restrict__ post, int mode, int n_fft,
+                                                  int log2m, const ScreenRows &scr) {
     extern __shared__ float2 smem[];
     const int M = n_fft >> 1;
     float2 *buf0 = smem;
@@ -674,7 +815,7 @@ __global__ void stft_generic_kernel(const float *__restrict__ x, long long x_str
     }
     // `in` now holds Z[0..M)
     const float scale = 1.0f / (4.0f * (float)n_fft * (float)n_fft);
-    float *o = out + c * out_stride_c + f * out_stride_f;
+    float *o = SCREEN ? reinterpret_cast<float *>(ob) : out + c * out_stride_c + f * out_stride_f;
     for (int k = tid; k <= M / 2; k += nthreads) {
         const float2 z = in[k];
         const float2 zp = in[(M - k) & (M - 1)];
@@ -692,6 +833,31 @@ __global__ void stft_generic_kernel(const float *__restrict__ x, long long x_str
             o[M - k] = finish<FRT_STFT_LOGPOWER>(p2, scale);
         }
     }
+    if constexpr (SCREEN) {
+        __syncthreads();
+        write_rows(o, out + c * out_stride_c + f * out_stride_f, scr, tid, nthreads);
+    }
+}
+
+__global__ void stft_generic_kernel(const float *__restrict__ x, long long x_stride,
+                                    long long n_frames, int hop, float *__restrict__ out,
+                                    long long out_stride_c, long long out_stride_f,
+                                    const float *__restrict__ win,
+                                    const float2 *__restrict__ tw,
+                                    const float2 *__restrict__ post, int mode, int n_fft,
+                                    int log2m) {
+    stft_generic_body<false>(x, x_stride, n_frames, hop, out, out_stride_c, out_stride_f, win, tw, post, mode,
+                             n_fft, log2m, ScreenRows{});
+}
+
+__global__ void stft_generic_screen_kernel(const float *__restrict__ x, long long x_stride,
+                                           long long n_frames, int hop, float *__restrict__ rows,
+                                           long long rows_stride_c, long long rows_stride_f,
+                                           const float *__restrict__ win, const float2 *__restrict__ tw,
+                                           const float2 *__restrict__ post, int n_fft, int log2m,
+                                           const ScreenRows scr) {
+    stft_generic_body<true>(x, x_stride, n_frames, hop, rows, rows_stride_c, rows_stride_f, win, tw, post,
+                            FRT_STFT_LOGPOWER, n_fft, log2m, scr);
 }
 
 size_t multi_smem(int r) { return sizeof(float2) * (1024 + (size_t)r * TILE); }
@@ -709,8 +875,8 @@ int frame_alignment(const float *x, long long x_stride, int hop) {
     return (((uintptr_t)x & 7) == 0) && ((x_stride & 1) == 0) && ((hop & 1) == 0);
 }
 
-// one frt_stft_process call: total = channels x frames items, frame f of channel c at
-// x + c x_stride + f hop, its spectrum at out + c osc + f osf
+// one frt_stft_process / frt_stft_screen_rows call: total = channels x frames items, frame f of
+// channel c at x + c x_stride + f hop, its spectrum (or, kModeScreen, its rows) at out + c osc + f osf
 struct Frames {
     const float *x;
     long long x_stride, n_frames;
@@ -719,6 +885,7 @@ struct Frames {
     long long osc, osf, total;
     int mode, vec_ok;
     cudaStream_t st;
+    ScreenRows scr;   // kModeScreen
 };
 
 template <int Q, bool TMA = false>
@@ -728,6 +895,10 @@ int launch_small(frt_ctx *h, const StftPlan &pl, const Frames &a) {
     long long blocks = ((a.total + G - 1) / G + WARPS - 1) / WARPS;
     if (blocks > max_blocks) blocks = max_blocks;
     const float2 *w2 = reinterpret_cast<const float2 *>(pl.win_dev.get());
+    if (a.mode == kModeScreen)
+        return frt_launch(h, stft_small_screen_kernel<Q, TMA>, (unsigned)blocks, WARPS * 32, small_screen_smem<Q, TMA>(),
+                          a.st, a.x, a.x_stride, a.n_frames, a.hop, a.out, a.osc, a.osf, w2, pl.tw_dev.get(),
+                          pl.post_dev.get(), a.total, a.vec_ok, a.scr);
     return with_mode(a.mode, [&](auto m) {
         return frt_launch(h, stft_small_kernel<Q, decltype(m)::value, TMA>, (unsigned)blocks, WARPS * 32,
                           small_smem<Q>(), a.st, a.x, a.x_stride, a.n_frames, a.hop, a.out, a.osc, a.osf, w2,
@@ -736,7 +907,7 @@ int launch_small(frt_ctx *h, const StftPlan &pl, const Frames &a) {
 }
 template <int R>
 int launch_large(frt_ctx *h, const StftPlan &pl, const Frames &a) {
-    constexpr int NG = LARGE_WARPS / R;
+    const int NG = (a.mode == kModeScreen ? large_warps<R, kModeScreen>() : large_warps<R, FRT_STFT_POWER>()) / R;
     long long blocks = (a.total + NG - 1) / NG;
     if (blocks > h->sm_count) blocks = h->sm_count;
     HannA ha;
@@ -745,18 +916,32 @@ int launch_large(frt_ctx *h, const StftPlan &pl, const Frames &a) {
         const double a = theta * 64.0 * R * n1;
         ha.v[n1] = make_float2((float)(0.5 * cos(a)), (float)(0.5 * sin(a)));
     }
+    if (a.mode == kModeScreen)
+        return frt_launch(h, stft_large_screen_kernel<R>, (unsigned)blocks, large_warps<R, kModeScreen>() * 32,
+                          large_smem<R, kModeScreen>(), a.st, a.x, a.x_stride, a.n_frames, a.hop, a.out, a.osc,
+                          a.osf, reinterpret_cast<const float2 *>(pl.win_dev.get()), pl.wlane_dev.get(),
+                          pl.tw_dev.get(), pl.comb_dev.get(), pl.post_dev.get(), a.total, ha, a.scr);
     return with_mode(a.mode, [&](auto m) {
-        return frt_launch(h, stft_large_kernel<R, decltype(m)::value>, (unsigned)blocks, LARGE_WARPS * 32,
-                          large_smem<R>(), a.st, a.x, a.x_stride, a.n_frames, a.hop, a.out, a.osc, a.osf,
+        constexpr int MODE = decltype(m)::value;
+        return frt_launch(h, stft_large_kernel<R, MODE>, (unsigned)blocks, large_warps<R, MODE>() * 32,
+                          large_smem<R, MODE>(), a.st, a.x, a.x_stride, a.n_frames, a.hop, a.out, a.osc, a.osf,
                           reinterpret_cast<const float2 *>(pl.win_dev.get()), pl.wlane_dev.get(), pl.tw_dev.get(),
                           pl.comb_dev.get(), pl.post_dev.get(), a.total, ha);
     });
 }
 template <int R>
 int launch_multi(frt_ctx *h, const StftPlan &pl, const Frames &a) {
-    long long blocks = (long long)h->sm_count * (R == 8 ? 2 : (R == 4 ? 4 : 8));
+    long long per_sm = R == 8 ? 2 : (R == 4 ? 4 : 8);
+    const size_t screen_smem = multi_smem(R) + sizeof(float) * (1024 * R + 1);
+    // kModeScreen: as many CTAs per SM as its 228 KB hold (1 KB of each CTA's is reserved)
+    if (a.mode == kModeScreen) per_sm = std::min<long long>(per_sm, (228 * 1024) / (screen_smem + 1024));
+    long long blocks = (long long)h->sm_count * per_sm;
     if (blocks > a.total) blocks = a.total;
     const float2 *w2 = reinterpret_cast<const float2 *>(pl.win_dev.get());
+    if (a.mode == kModeScreen)
+        return frt_launch(h, stft_multi_screen_kernel<R>, (unsigned)blocks, 32 * R, screen_smem, a.st, a.x,
+                          a.x_stride, a.n_frames, a.hop, a.out, a.osc, a.osf, w2, pl.tw_dev.get(), pl.comb_dev.get(),
+                          pl.post_dev.get(), a.total, a.vec_ok, a.scr);
     return with_mode(a.mode, [&](auto m) {
         return frt_launch(h, stft_multi_kernel<R, decltype(m)::value>, (unsigned)blocks, 32 * R, multi_smem(R),
                           a.st, a.x, a.x_stride, a.n_frames, a.hop, a.out, a.osc, a.osf, w2, pl.tw_dev.get(),
@@ -858,6 +1043,8 @@ extern "C" int frt_stft_window(frt_handle h, float *window_host) {
     return FRT_OK;
 }
 
+static int stft_dispatch(frt_ctx *h, const StftPlan &pl, const Frames &a);
+
 extern "C" int frt_stft_process(frt_handle h, const float *x_dev, int64_t x_stride,
                                 int n_channels, int64_t n_frames, int hop, float *out_dev,
                                 int64_t out_stride_c, int64_t out_stride_f, int mode,
@@ -874,9 +1061,14 @@ extern "C" int frt_stft_process(frt_handle h, const float *x_dev, int64_t x_stri
     const int nbins = pl.n_fft / 2 + 1;
     FRT_CHECK_ARG(h, out_stride_f >= nbins, "out_stride_f smaller than n_fft/2+1");
     const long long total = (long long)n_channels * n_frames;
-    const int N = pl.n_fft, align = frame_alignment(x_dev, x_stride, hop);
     const Frames a{x_dev, x_stride, n_frames, hop, out_dev, out_stride_c, out_stride_f, total,
-                   mode, align >= 1, (cudaStream_t)stream};
+                   mode, frame_alignment(x_dev, x_stride, hop) >= 1, (cudaStream_t)stream, ScreenRows{}};
+    return stft_dispatch(h, pl, a);
+}
+
+// the kernel family for the plan's size and the frames' alignment, for every output mode
+static int stft_dispatch(frt_ctx *h, const StftPlan &pl, const Frames &a) {
+    const int N = pl.n_fft, align = frame_alignment(a.x, a.x_stride, a.hop);
     if (N >= 64 && N <= 2048) {
         switch (N / 64) {
             case 1: return launch_small<1>(h, pl, a);
@@ -898,14 +1090,39 @@ extern "C" int frt_stft_process(frt_handle h, const float *x_dev, int64_t x_stri
         if (N == 8192) return launch_multi<4>(h, pl, a);
         return launch_multi<8>(h, pl, a);
     }
-    FRT_CHECK_ARG(h, total <= 0x7fffffffLL, "too many frames for one launch");
+    FRT_CHECK_ARG(h, a.total <= 0x7fffffffLL, "too many frames for one launch");
     const int M = N / 2;
     int threads = M / 4;
     if (threads < 32) threads = 32;
     if (threads > 512) threads = 512;
-    return frt_launch(h, stft_generic_kernel, (unsigned)total, threads, sizeof(float2) * 2 * M, a.st, x_dev,
-                      x_stride, n_frames, hop, out_dev, out_stride_c, out_stride_f, pl.win_dev.get(),
-                      pl.tw_dev.get(), pl.post_dev.get(), mode, N, ilog2(M));
+    if (a.mode == kModeScreen)
+        return frt_launch(h, stft_generic_screen_kernel, (unsigned)a.total, threads, sizeof(float2) * 2 * M, a.st,
+                          a.x, a.x_stride, a.n_frames, a.hop, a.out, a.osc, a.osf, pl.win_dev.get(), pl.tw_dev.get(),
+                          pl.post_dev.get(), N, ilog2(M), a.scr);
+    return frt_launch(h, stft_generic_kernel, (unsigned)a.total, threads, sizeof(float2) * 2 * M, a.st, a.x,
+                      a.x_stride, a.n_frames, a.hop, a.out, a.osc, a.osf, pl.win_dev.get(),
+                      pl.tw_dev.get(), pl.post_dev.get(), a.mode, N, ilog2(M));
+}
+
+extern "C" int frt_stft_screen_rows(frt_handle h, const float *x_dev, int64_t x_stride, int n_channels,
+                                    int64_t n_frames, int hop, const float *weight_dev, float spec_min,
+                                    float spec_max, const int *row_i0_dev, const float *row_t_dev, int height,
+                                    float *rows_dev, int64_t rows_stride_c, int64_t rows_stride_f,
+                                    void *stream) {
+    if (!h) return FRT_EINVAL;
+    DeviceGuard g(h->device);
+    if (!h->stft) return frt_fail(h, FRT_ESTATE, "frt_stft_screen_rows: call frt_stft_plan first");
+    FRT_CHECK_ARG(h, n_channels >= 0 && n_frames >= 0 && height >= 1, "bad shape");
+    FRT_CHECK_ARG(h, hop >= 1, "hop must be >= 1");
+    FRT_CHECK_ARG(h, spec_max != spec_min, "empty dB range");
+    if (n_channels == 0 || n_frames == 0) return FRT_OK;   // empty input: nothing to do
+    FRT_CHECK_ARG(h, x_dev && row_i0_dev && row_t_dev && rows_dev, "NULL buffer");
+    FRT_CHECK_ARG(h, rows_stride_f >= height, "rows_stride_f smaller than height");
+    ScreenRows scr{weight_dev, row_i0_dev, row_t_dev, spec_min, 1.0f / (spec_max - spec_min), height};
+    const Frames a{x_dev, x_stride, n_frames, hop, rows_dev, rows_stride_c, rows_stride_f,
+                   (long long)n_channels * n_frames, kModeScreen, frame_alignment(x_dev, x_stride, hop) >= 1,
+                   (cudaStream_t)stream, scr};
+    return stft_dispatch(h, *h->stft, a);
 }
 
 extern "C" int frt_stft_process_host(frt_handle h, const float *x_host, int64_t x_stride,

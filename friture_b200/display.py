@@ -107,6 +107,13 @@ class OnlineResamplerIndex:
         return np.asarray(cols, dtype=np.int32), np.asarray(avals, dtype=np.float64)
 
 
+def _upload(arr, device):
+    """Host array -> device tensor, ordered on the current stream without blocking the host: a copy
+    from pageable memory would first wait for the work already queued on the stream."""
+    import torch
+    return torch.from_numpy(np.ascontiguousarray(arr)).pin_memory().to(device, non_blocking=True)
+
+
 def load_lut():
     path = os.path.join(os.path.dirname(os.path.abspath(__file__)), "data", "cmrmap.npz")
     with np.load(path) as d:
@@ -116,7 +123,9 @@ def load_lut():
 class SpectrogramDisplay:
     """Spectrogram_Widget's transform pipeline for C channels.  ``push(db)`` takes the tick's
     log-power columns [C, F, bins] (``audioproc.stft(..., log=True)``) and returns the new screen
-    columns as an int32 CUDA tensor [C, height, n_out] holding 0xAARRGGBB words."""
+    columns as an int32 CUDA tensor [C, height, n_out] holding 0xAARRGGBB words.  ``push_rows(rows)``
+    does the same from rows already interpolated to the screen height ([C, F, height],
+    ``frt_stft_screen_rows`` with this object's ``tables``)."""
 
     def __init__(self, n_channels, fft_size=4096, freqscale=Mel, minfreq=20., maxfreq=SAMPLING_RATE / 2,
                  spec_min=-140., spec_max=0., weighting=0, height=512, width=1024, timerange_s=10.,
@@ -135,6 +144,7 @@ class SpectrogramDisplay:
         self.height, self.width = int(height), int(width)
         self.timerange_s = timerange_s
         # spectrogram.py:98,166-167: input columns per ms / screen columns per ms
+        self.overlap_frac = overlap_frac
         self.sfft_rate_frac = Fraction(SAMPLING_RATE, fft_size) / (Fraction(1) - overlap_frac) / 1000
         self.index = OnlineResamplerIndex()
         self._tables = None
@@ -150,6 +160,30 @@ class SpectrogramDisplay:
             self.index.reset()                # online_linear_2D_resampler.py:46-57
         self.width = int(width)
 
+    def set_fftsize(self, fft_size):
+        """Spectrogram_Widget.setfftsize (friture/spectrogram.py:225-238): new bin frequencies and
+        weighting tables, and a new input-column rate, which restarts the resampler's index on the
+        next push (set_ratio).  The carried column is on the screen grid and is kept."""
+        if fft_size != self.fft_size:
+            self.fft_size = fft_size
+            self.proc.set_fftsize(fft_size)
+            self.freq = self.proc.get_freq_scale()
+            self.sfft_rate_frac = Fraction(SAMPLING_RATE, fft_size) / (Fraction(1) - self.overlap_frac) / 1000
+            self._tables = None
+
+    def set_rows(self, freqscale, minfreq, maxfreq, weighting):
+        """Frequency scale, range and weighting (setfreqscale / setminfreq / setmaxfreq /
+        setweighting, friture/spectrogram.py:203-249): the screen-row and weighting tables are
+        rebuilt on the next push; nothing else is reset."""
+        self.scale, self.minfreq, self.maxfreq, self.weighting = freqscale, minfreq, maxfreq, weighting
+        self._tables = None
+
+    def tables(self, device):
+        """The screen-row table (``i0`` int32, ``t`` float32 [height]), the weighting (``w`` float32
+        [bins] or None) and the LUT on ``device``, built for the current settings."""
+        self._ensure(device)
+        return self._tables
+
     def _ensure(self, device):
         import torch
         screen_rate_frac = Fraction(max(self.width, 1), int(self.timerange_s * 1000))
@@ -159,10 +193,10 @@ class SpectrogramDisplay:
             A, B, C = self.proc.get_freq_weighting()
             w = [None, A, B, C][self.weighting]
             self._tables = {
-                "i0": torch.from_numpy(i0).to(device),
-                "t": torch.from_numpy(t.astype(np.float32)).to(device),
-                "w": None if w is None else torch.from_numpy(np.asarray(w, dtype=np.float32)).to(device),
-                "lut": torch.from_numpy(load_lut().view(np.int32)).to(device),
+                "i0": _upload(i0, device),
+                "t": _upload(t.astype(np.float32), device),
+                "w": None if w is None else _upload(np.asarray(w, dtype=np.float32), device),
+                "lut": _upload(load_lut().view(np.int32), device),
             }
         if self._old is None:
             self._old = torch.zeros((self.n_channels, self.height), dtype=torch.float32, device=device)
@@ -182,12 +216,36 @@ class SpectrogramDisplay:
             pixels = torch.empty((C, self.height, n_out), dtype=torch.int32, device=db.device)
             if F == 0:
                 return pixels
-            cols_d = torch.from_numpy(cols).to(db.device) if n_out else None
-            a_d = torch.from_numpy(a.astype(np.float32)).to(db.device) if n_out else None
+            cols_d = _upload(cols, db.device) if n_out else None
+            a_d = _upload(a.astype(np.float32), db.device) if n_out else None
             T = self._tables
             self.handle.call("frt_display_columns", _lib._ptr(db), int(F * nb), int(nb), int(C), int(F),
                              int(nb), _lib._ptr(T["w"]), c_float(self.spec_min), c_float(self.spec_max),
                              _lib._ptr(T["i0"]), _lib._ptr(T["t"]), int(self.height), _lib._ptr(cols_d),
                              _lib._ptr(a_d), int(n_out), _lib._ptr(self._old), _lib._ptr(T["lut"]),
                              _lib._ptr(pixels) if n_out else None, sp)
+        return pixels
+
+    def push_rows(self, rows, stream=None):
+        """``push`` for rows already on the screen grid: rows [C, F, height] contiguous CUDA float32,
+        made with this object's current ``tables`` and dB range."""
+        import torch
+        if rows.dim() != 3 or rows.shape[0] != self.n_channels or rows.shape[2] != self.height:
+            raise ValueError("rows must be [%d, F, %d]" % (self.n_channels, self.height))
+        if not rows.is_contiguous():
+            raise ValueError("rows must be a contiguous CUDA float32 tensor")
+        _lib.check_tensor(self, rows, "rows")
+        C, F, H = rows.shape
+        with _lib.call_stream(rows.device, stream) as sp:
+            self._ensure(rows.device)
+            cols, a = self.index.push(F)
+            n_out = len(cols)
+            pixels = torch.empty((C, H, n_out), dtype=torch.int32, device=rows.device)
+            if F == 0:
+                return pixels
+            cols_d = _upload(cols, rows.device) if n_out else None
+            a_d = _upload(a.astype(np.float32), rows.device) if n_out else None
+            self.handle.call("frt_display_rows", _lib._ptr(rows), int(F * H), int(H), int(C), int(F), int(H),
+                             _lib._ptr(cols_d), _lib._ptr(a_d), int(n_out), _lib._ptr(self._old),
+                             _lib._ptr(self._tables["lut"]), _lib._ptr(pixels) if n_out else None, sp)
         return pixels

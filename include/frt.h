@@ -74,6 +74,20 @@ int frt_stft_process(frt_handle h, const float *x_dev, int64_t x_stride, int n_c
  * out_host is [n_channels][frames][n_fft/2+1] contiguous.                                   */
 int frt_stft_process_host(frt_handle h, const float *x_host, int64_t x_stride, int n_channels,
                           int64_t n_samples, int hop, float *out_host, int mode);
+/* The spectrogram's screen rows straight from the frames: frame f of channel c (framed as in
+ * frt_stft_process, with the frt_stft_plan'ed size) is transformed to its FRT_STFT_LOGPOWER column,
+ * which stays on chip, and only its `height` rows are written,
+ *   rows[c*rows_stride_c + f*rows_stride_f + r] = fmaf(t[r], b - a, a),
+ *   a = (db[i0[r]] + w[i0[r]] - spec_min) / (spec_max - spec_min), b = the same at i0[r] + 1,
+ * bit for bit what frt_display_columns interpolates from the stored column (w = weight_dev, or 0
+ * when it is NULL).  row_i0_dev/row_t_dev are the screen-row table of frt_display_columns:
+ * 0 <= i0[r] <= n_fft/2 - 1 (= nbins - 2) is the caller's precondition.  Needs height >= 1,
+ * spec_max != spec_min and rows_stride_f >= height; n_channels == 0 or n_frames == 0 is a no-op.
+ * Feed the rows to frt_display_rows.                                                           */
+int frt_stft_screen_rows(frt_handle h, const float *x_dev, int64_t x_stride, int n_channels,
+                         int64_t n_frames, int hop, const float *weight_dev, float spec_min,
+                         float spec_max, const int *row_i0_dev, const float *row_t_dev, int height,
+                         float *rows_dev, int64_t rows_stride_c, int64_t rows_stride_f, void *stream);
 
 /* ---------------------------------------------------------------- filterbank (Octave_Filters)
  * Stands behind friture/octavefilters.py:37-158 (`Octave_Filters.filter`, `setbandsperoctave`)
@@ -367,6 +381,14 @@ int frt_display_columns(frt_handle h, const float *db_dev, int64_t stride_c, int
                         const float *row_t_dev, int height, const int *out_col_dev,
                         const float *out_a_dev, int n_out, float *old_data_dev,
                         const uint32_t *lut_dev, uint32_t *pixels_dev, void *stream);
+/* The same time resampling, clip and colour look-up on rows already on the screen grid
+ * (frt_stft_screen_rows): rows_dev [C][n_frames][height] (strides in floats), the rest as in
+ * frt_display_columns.  Gives frt_display_columns' pixels and carried column bit for bit when the
+ * rows come from the same frames and screen-row table.                                         */
+int frt_display_rows(frt_handle h, const float *rows_dev, int64_t stride_c, int64_t stride_f,
+                     int n_channels, int n_frames, int height, const int *out_col_dev,
+                     const float *out_a_dev, int n_out, float *old_data_dev, const uint32_t *lut_dev,
+                     uint32_t *pixels_dev, void *stream);
 
 #ifdef __cplusplus
 }
