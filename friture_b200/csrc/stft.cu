@@ -137,8 +137,9 @@ __device__ __forceinline__ float finish(float mag2, float scale) {
 
 // Third output of the STFT kernels (frt_stft_screen_rows): the frame's log-power column, computed as
 // FRT_STFT_LOGPOWER computes it, stays in shared memory and only its `height` screen rows are written,
-// row r = screen_value of the column (what display_kernel computes from a stored column).  Each kernel
-// family has a __global__ wrapper of this mode next to its existing one; both run the same body.
+// row r = screen_value of the column (what display_kernel computes from a stored column).  Every kernel
+// family takes the output as its MODE template argument and the screen tables as its last parameter,
+// which the other two modes leave unused (launched as ScreenRows{}).
 constexpr int kModeScreen = 2;
 
 struct ScreenRows {
@@ -302,12 +303,12 @@ __device__ __forceinline__ void combine_split(float *__restrict__ o, const float
 
 // kModeScreen: the frame's column goes to s_col, after the tiles, and its rows to out.
 template <int R, int MODE>
-__device__ __forceinline__ void
-stft_multi_body(const float *__restrict__ x, long long x_stride, long long n_frames, int hop,
-                float *__restrict__ out, long long out_stride_c, long long out_stride_f,
-                const float2 *__restrict__ win2, const float2 *__restrict__ tw32,
-                const float2 *__restrict__ comb, const float2 *__restrict__ post,
-                long long total_items, int vec_ok, const ScreenRows &scr) {
+__global__ void __launch_bounds__(32 * R)
+stft_multi_kernel(const float *__restrict__ x, long long x_stride, long long n_frames, int hop,
+                  float *__restrict__ out, long long out_stride_c, long long out_stride_f,
+                  const float2 *__restrict__ win2, const float2 *__restrict__ tw32,
+                  const float2 *__restrict__ comb, const float2 *__restrict__ post,
+                  long long total_items, int vec_ok, const ScreenRows scr) {
     constexpr int M = 1024 * R, N = 2 * M;
     extern __shared__ float2 smem[];
     float2 *s_tw = smem;                       // [32][32] W_1024^(k1 t)
@@ -357,28 +358,6 @@ stft_multi_body(const float *__restrict__ x, long long x_stride, long long n_fra
     }
 }
 
-template <int R, int MODE>
-__global__ void __launch_bounds__(32 * R)
-stft_multi_kernel(const float *__restrict__ x, long long x_stride, long long n_frames, int hop,
-                  float *__restrict__ out, long long out_stride_c, long long out_stride_f,
-                  const float2 *__restrict__ win2, const float2 *__restrict__ tw32,
-                  const float2 *__restrict__ comb, const float2 *__restrict__ post,
-                  long long total_items, int vec_ok) {
-    stft_multi_body<R, MODE>(x, x_stride, n_frames, hop, out, out_stride_c, out_stride_f, win2, tw32, comb, post,
-                             total_items, vec_ok, ScreenRows{});
-}
-
-template <int R>
-__global__ void __launch_bounds__(32 * R)
-stft_multi_screen_kernel(const float *__restrict__ x, long long x_stride, long long n_frames, int hop,
-                         float *__restrict__ rows, long long rows_stride_c, long long rows_stride_f,
-                         const float2 *__restrict__ win2, const float2 *__restrict__ tw32,
-                         const float2 *__restrict__ comb, const float2 *__restrict__ post,
-                         long long total_items, int vec_ok, const ScreenRows scr) {
-    stft_multi_body<R, kModeScreen>(x, x_stride, n_frames, hop, rows, rows_stride_c, rows_stride_f, win2, tw32,
-                                    comb, post, total_items, vec_ok, scr);
-}
-
 // ------------------------------------------------------------------------------------------
 // N = 64 Q, Q in {1, 2, 4, 8, 16, 32} (64 .. 2048 points): ONE WARP PER G = 32/Q FRAMES.
 // M = N/2 = 32 Q.  Lane t holds z_g[32 n1 + t] (n1 < Q) of each of the G frames in register g*Q + n1,
@@ -392,26 +371,23 @@ stft_multi_screen_kernel(const float *__restrict__ x, long long x_stride, long l
 // aligned frames are staged by the TMA engine; smaller Q run two CTAs of 8 warps per SM.
 template <int Q> __host__ __device__ constexpr int small_warps() { return Q == 32 ? 16 : 8; }
 template <int Q> __host__ __device__ constexpr int small_ctas_per_sm() { return Q == 32 ? 1 : 2; }
-template <int Q>
-constexpr size_t small_smem() {
-    // window, twiddle and split tables, the warps' tiles and (Q = 32) the warps' mbarriers
-    return sizeof(float2) * (32 * Q + 32 * Q + 16 * Q + (size_t)small_warps<Q>() * TILE) +
-           (Q == 32 ? sizeof(unsigned long long) * small_warps<Q>() : 0);
-}
-
 // kModeScreen: the warp's G columns go to its tile, free again after the transpose; with TMA the tile
 // already holds the next frame by then, so each warp has a column buffer of its own after the mbarriers.
-template <int Q, bool TMA>
-constexpr size_t small_screen_smem() {
-    return small_smem<Q>() + (TMA ? sizeof(float) * (size_t)small_warps<Q>() * (32 * Q + 1) : 0);
+template <int Q, int MODE, bool TMA>
+constexpr size_t small_smem() {
+    // window, twiddle and split tables, the warps' tiles, (Q = 32) the warps' mbarriers and
+    // (kModeScreen with TMA) the warps' column buffers
+    return sizeof(float2) * (32 * Q + 32 * Q + 16 * Q + (size_t)small_warps<Q>() * TILE) +
+           (Q == 32 ? sizeof(unsigned long long) * small_warps<Q>() : 0) +
+           (MODE == kModeScreen && TMA ? sizeof(float) * (size_t)small_warps<Q>() * (32 * Q + 1) : 0);
 }
 
 template <int Q, int MODE, bool TMA>
-__device__ __forceinline__ void
-stft_small_body(const float *__restrict__ x, long long x_stride, long long n_frames, int hop,
-                float *__restrict__ out, long long out_stride_c, long long out_stride_f,
-                const float2 *__restrict__ win2, const float2 *__restrict__ tw,
-                const float2 *__restrict__ post, long long total_items, int vec_ok, const ScreenRows &scr) {
+__global__ void __launch_bounds__(small_warps<Q>() * 32, small_ctas_per_sm<Q>())
+stft_small_kernel(const float *__restrict__ x, long long x_stride, long long n_frames, int hop,
+                  float *__restrict__ out, long long out_stride_c, long long out_stride_f,
+                  const float2 *__restrict__ win2, const float2 *__restrict__ tw,
+                  const float2 *__restrict__ post, long long total_items, int vec_ok, const ScreenRows scr) {
     static_assert(!TMA || Q == 32, "TMA staging is for one frame per warp");
     constexpr int G = 32 / Q, M = 32 * Q, N = 2 * M, WARPS = small_warps<Q>();
     extern __shared__ float2 smem[];
@@ -563,27 +539,6 @@ stft_small_body(const float *__restrict__ x, long long x_stride, long long n_fra
     }
 }
 
-template <int Q, int MODE, bool TMA>
-__global__ void __launch_bounds__(small_warps<Q>() * 32, small_ctas_per_sm<Q>())
-stft_small_kernel(const float *__restrict__ x, long long x_stride, long long n_frames, int hop,
-                  float *__restrict__ out, long long out_stride_c, long long out_stride_f,
-                  const float2 *__restrict__ win2, const float2 *__restrict__ tw,
-                  const float2 *__restrict__ post, long long total_items, int vec_ok) {
-    stft_small_body<Q, MODE, TMA>(x, x_stride, n_frames, hop, out, out_stride_c, out_stride_f, win2, tw, post,
-                                  total_items, vec_ok, ScreenRows{});
-}
-
-template <int Q, bool TMA>
-__global__ void __launch_bounds__(small_warps<Q>() * 32, small_ctas_per_sm<Q>())
-stft_small_screen_kernel(const float *__restrict__ x, long long x_stride, long long n_frames, int hop,
-                         float *__restrict__ rows, long long rows_stride_c, long long rows_stride_f,
-                         const float2 *__restrict__ win2, const float2 *__restrict__ tw,
-                         const float2 *__restrict__ post, long long total_items, int vec_ok,
-                         const ScreenRows scr) {
-    stft_small_body<Q, kModeScreen, TMA>(x, x_stride, n_frames, hop, rows, rows_stride_c, rows_stride_f, win2, tw,
-                                         post, total_items, vec_ok, scr);
-}
-
 // ------------------------------------------------------------------------------------------
 // N = 4096 / 8192, 8-byte aligned input: the stft_multi_kernel decomposition (R warps per frame, each a
 // 1024-point complex FFT of a decimated sequence, then a radix-R combine + split step) rebuilt
@@ -627,13 +582,13 @@ __device__ __forceinline__ float2 post_lookup(const float2 *s_post, int kk, int 
 }
 
 template <int R, int MODE>
-__device__ __forceinline__ void
-stft_large_body(const float *__restrict__ x, long long x_stride, long long n_frames, int hop,
-                float *__restrict__ out, long long out_stride_c, long long out_stride_f,
-                const float2 *__restrict__ win2, const float4 *__restrict__ wlane,
-                const float2 *__restrict__ tw32, const float2 *__restrict__ comb,
-                const float2 *__restrict__ post, long long total_items, const HannA &hann_a,
-                const ScreenRows &scr) {
+__global__ void __launch_bounds__(large_warps<R, MODE>() * 32, 1)
+stft_large_kernel(const float *__restrict__ x, long long x_stride, long long n_frames, int hop,
+                  float *__restrict__ out, long long out_stride_c, long long out_stride_f,
+                  const float2 *__restrict__ win2, const float4 *__restrict__ wlane,
+                  const float2 *__restrict__ tw32, const float2 *__restrict__ comb,
+                  const float2 *__restrict__ post, long long total_items,
+                  const __grid_constant__ HannA hann_a, const ScreenRows scr) {
     // STAG: 8-byte shared accesses are served per half-warp; the 16/R elements a half-warp sends to
     // each of the R tiles must fall on different banks
     constexpr int LARGE_WARPS = large_warps<R, MODE>();
@@ -720,30 +675,6 @@ stft_large_body(const float *__restrict__ x, long long x_stride, long long n_fra
     }
 }
 
-template <int R, int MODE>
-__global__ void __launch_bounds__(large_warps<R, MODE>() * 32, 1)
-stft_large_kernel(const float *__restrict__ x, long long x_stride, long long n_frames, int hop,
-                  float *__restrict__ out, long long out_stride_c, long long out_stride_f,
-                  const float2 *__restrict__ win2, const float4 *__restrict__ wlane,
-                  const float2 *__restrict__ tw32, const float2 *__restrict__ comb,
-                  const float2 *__restrict__ post, long long total_items,
-                  const __grid_constant__ HannA hann_a) {
-    stft_large_body<R, MODE>(x, x_stride, n_frames, hop, out, out_stride_c, out_stride_f, win2, wlane, tw32, comb,
-                             post, total_items, hann_a, ScreenRows{});
-}
-
-template <int R>
-__global__ void __launch_bounds__(large_warps<R, kModeScreen>() * 32, 1)
-stft_large_screen_kernel(const float *__restrict__ x, long long x_stride, long long n_frames, int hop,
-                         float *__restrict__ rows, long long rows_stride_c, long long rows_stride_f,
-                         const float2 *__restrict__ win2, const float4 *__restrict__ wlane,
-                         const float2 *__restrict__ tw32, const float2 *__restrict__ comb,
-                         const float2 *__restrict__ post, long long total_items,
-                         const __grid_constant__ HannA hann_a, const ScreenRows scr) {
-    stft_large_body<R, kModeScreen>(x, x_stride, n_frames, hop, rows, rows_stride_c, rows_stride_f, win2, wlane,
-                                    tw32, comb, post, total_items, hann_a, scr);
-}
-
 // ------------------------------------------------------------------------------------------
 // Generic path: one CTA per frame, Stockham autosort in shared memory.
 __device__ __forceinline__ void stockham_radix4(const float2 *__restrict__ in,
@@ -771,15 +702,15 @@ __device__ __forceinline__ void stockham_radix4(const float2 *__restrict__ in,
     }
 }
 
-// SCREEN: the column goes to the buffer the FFT does not end in, and the frame's rows to out.
-template <bool SCREEN>
-__device__ __forceinline__ void stft_generic_body(const float *__restrict__ x, long long x_stride,
-                                                  long long n_frames, int hop, float *__restrict__ out,
-                                                  long long out_stride_c, long long out_stride_f,
-                                                  const float *__restrict__ win,
-                                                  const float2 *__restrict__ tw,
-                                                  const float2 *__restrict__ post, int mode, int n_fft,
-                                                  int log2m, const ScreenRows &scr) {
+// kModeScreen: the column goes to the buffer the FFT does not end in, and the frame's rows to out.
+template <int MODE>
+__global__ void stft_generic_kernel(const float *__restrict__ x, long long x_stride,
+                                    long long n_frames, int hop, float *__restrict__ out,
+                                    long long out_stride_c, long long out_stride_f,
+                                    const float *__restrict__ win,
+                                    const float2 *__restrict__ tw,
+                                    const float2 *__restrict__ post, int n_fft, int log2m,
+                                    const ScreenRows scr) {
     extern __shared__ float2 smem[];
     const int M = n_fft >> 1;
     float2 *buf0 = smem;
@@ -815,7 +746,7 @@ __device__ __forceinline__ void stft_generic_body(const float *__restrict__ x, l
     }
     // `in` now holds Z[0..M)
     const float scale = 1.0f / (4.0f * (float)n_fft * (float)n_fft);
-    float *o = SCREEN ? reinterpret_cast<float *>(ob) : out + c * out_stride_c + f * out_stride_f;
+    float *o = MODE == kModeScreen ? reinterpret_cast<float *>(ob) : out + c * out_stride_c + f * out_stride_f;
     for (int k = tid; k <= M / 2; k += nthreads) {
         const float2 z = in[k];
         const float2 zp = in[(M - k) & (M - 1)];
@@ -824,49 +755,33 @@ __device__ __forceinline__ void stft_generic_body(const float *__restrict__ x, l
         const float2 T = cmul(O, post[k]);
         const float2 X = cadd(E, T);
         const float2 Y = csub(E, T);
-        const float p1 = fmaf(X.x, X.x, X.y * X.y), p2 = fmaf(Y.x, Y.x, Y.y * Y.y);
-        if (mode == FRT_STFT_POWER) {
-            o[k] = finish<FRT_STFT_POWER>(p1, scale);
-            o[M - k] = finish<FRT_STFT_POWER>(p2, scale);
-        } else {
-            o[k] = finish<FRT_STFT_LOGPOWER>(p1, scale);
-            o[M - k] = finish<FRT_STFT_LOGPOWER>(p2, scale);
-        }
+        o[k] = finish<MODE>(fmaf(X.x, X.x, X.y * X.y), scale);
+        o[M - k] = finish<MODE>(fmaf(Y.x, Y.x, Y.y * Y.y), scale);
     }
-    if constexpr (SCREEN) {
+    if constexpr (MODE == kModeScreen) {
         __syncthreads();
         write_rows(o, out + c * out_stride_c + f * out_stride_f, scr, tid, nthreads);
     }
 }
 
-__global__ void stft_generic_kernel(const float *__restrict__ x, long long x_stride,
-                                    long long n_frames, int hop, float *__restrict__ out,
-                                    long long out_stride_c, long long out_stride_f,
-                                    const float *__restrict__ win,
-                                    const float2 *__restrict__ tw,
-                                    const float2 *__restrict__ post, int mode, int n_fft,
-                                    int log2m) {
-    stft_generic_body<false>(x, x_stride, n_frames, hop, out, out_stride_c, out_stride_f, win, tw, post, mode,
-                             n_fft, log2m, ScreenRows{});
+// the tw table and the R tiles (+ kModeScreen: the frame's column)
+template <int R, int MODE>
+constexpr size_t multi_smem() {
+    return sizeof(float2) * (1024 + (size_t)R * TILE) + (MODE == kModeScreen ? sizeof(float) * (1024 * R + 1) : 0);
+}
+// kModeScreen: no more CTAs per SM than its 228 KB hold (1 KB of each CTA's is reserved)
+template <int R, int MODE>
+constexpr long long multi_ctas_per_sm() {
+    constexpr long long n = R == 8 ? 2 : (R == 4 ? 4 : 8);
+    return MODE == kModeScreen ? std::min<long long>(n, (228 * 1024) / (multi_smem<R, MODE>() + 1024)) : n;
 }
 
-__global__ void stft_generic_screen_kernel(const float *__restrict__ x, long long x_stride,
-                                           long long n_frames, int hop, float *__restrict__ rows,
-                                           long long rows_stride_c, long long rows_stride_f,
-                                           const float *__restrict__ win, const float2 *__restrict__ tw,
-                                           const float2 *__restrict__ post, int n_fft, int log2m,
-                                           const ScreenRows scr) {
-    stft_generic_body<true>(x, x_stride, n_frames, hop, rows, rows_stride_c, rows_stride_f, win, tw, post,
-                            FRT_STFT_LOGPOWER, n_fft, log2m, scr);
-}
-
-size_t multi_smem(int r) { return sizeof(float2) * (1024 + (size_t)r * TILE); }
-
-// calls launch with the mode (FRT_STFT_POWER / FRT_STFT_LOGPOWER) as a compile-time constant
+// calls launch with the output (FRT_STFT_POWER, FRT_STFT_LOGPOWER or kModeScreen) as a compile-time constant
 template <class F>
 int with_mode(int mode, F &&launch) {
     if (mode == FRT_STFT_POWER) return launch(std::integral_constant<int, FRT_STFT_POWER>());
-    return launch(std::integral_constant<int, FRT_STFT_LOGPOWER>());
+    if (mode == FRT_STFT_LOGPOWER) return launch(std::integral_constant<int, FRT_STFT_LOGPOWER>());
+    return launch(std::integral_constant<int, kModeScreen>());
 }
 
 // how far every frame's first sample is aligned: 2 = 16 bytes, 1 = 8 bytes, 0 = 4 bytes
@@ -883,7 +798,7 @@ struct Frames {
     int hop;
     float *out;
     long long osc, osf, total;
-    int mode, vec_ok;
+    int mode, align;   // align: frame_alignment of the frames
     cudaStream_t st;
     ScreenRows scr;   // kModeScreen
 };
@@ -894,58 +809,42 @@ int launch_small(frt_ctx *h, const StftPlan &pl, const Frames &a) {
     const long long max_blocks = (long long)small_ctas_per_sm<Q>() * h->sm_count;
     long long blocks = ((a.total + G - 1) / G + WARPS - 1) / WARPS;
     if (blocks > max_blocks) blocks = max_blocks;
-    const float2 *w2 = reinterpret_cast<const float2 *>(pl.win_dev.get());
-    if (a.mode == kModeScreen)
-        return frt_launch(h, stft_small_screen_kernel<Q, TMA>, (unsigned)blocks, WARPS * 32, small_screen_smem<Q, TMA>(),
-                          a.st, a.x, a.x_stride, a.n_frames, a.hop, a.out, a.osc, a.osf, w2, pl.tw_dev.get(),
-                          pl.post_dev.get(), a.total, a.vec_ok, a.scr);
     return with_mode(a.mode, [&](auto m) {
-        return frt_launch(h, stft_small_kernel<Q, decltype(m)::value, TMA>, (unsigned)blocks, WARPS * 32,
-                          small_smem<Q>(), a.st, a.x, a.x_stride, a.n_frames, a.hop, a.out, a.osc, a.osf, w2,
-                          pl.tw_dev.get(), pl.post_dev.get(), a.total, a.vec_ok);
+        constexpr int MODE = decltype(m)::value;
+        return frt_launch(h, stft_small_kernel<Q, MODE, TMA>, (unsigned)blocks, WARPS * 32, small_smem<Q, MODE, TMA>(),
+                          a.st, a.x, a.x_stride, a.n_frames, a.hop, a.out, a.osc, a.osf,
+                          reinterpret_cast<const float2 *>(pl.win_dev.get()), pl.tw_dev.get(), pl.post_dev.get(),
+                          a.total, a.align >= 1, a.scr);
     });
 }
 template <int R>
 int launch_large(frt_ctx *h, const StftPlan &pl, const Frames &a) {
-    const int NG = (a.mode == kModeScreen ? large_warps<R, kModeScreen>() : large_warps<R, FRT_STFT_POWER>()) / R;
-    long long blocks = (a.total + NG - 1) / NG;
-    if (blocks > h->sm_count) blocks = h->sm_count;
     HannA ha;
     const double theta = 2.0 * 3.14159265358979323846 / (double)(2048 * R - 1);
     for (int n1 = 0; n1 < 32; n1++) {
         const double a = theta * 64.0 * R * n1;
         ha.v[n1] = make_float2((float)(0.5 * cos(a)), (float)(0.5 * sin(a)));
     }
-    if (a.mode == kModeScreen)
-        return frt_launch(h, stft_large_screen_kernel<R>, (unsigned)blocks, large_warps<R, kModeScreen>() * 32,
-                          large_smem<R, kModeScreen>(), a.st, a.x, a.x_stride, a.n_frames, a.hop, a.out, a.osc,
-                          a.osf, reinterpret_cast<const float2 *>(pl.win_dev.get()), pl.wlane_dev.get(),
-                          pl.tw_dev.get(), pl.comb_dev.get(), pl.post_dev.get(), a.total, ha, a.scr);
     return with_mode(a.mode, [&](auto m) {
-        constexpr int MODE = decltype(m)::value;
+        constexpr int MODE = decltype(m)::value, NG = large_warps<R, MODE>() / R;
+        long long blocks = (a.total + NG - 1) / NG;
+        if (blocks > h->sm_count) blocks = h->sm_count;
         return frt_launch(h, stft_large_kernel<R, MODE>, (unsigned)blocks, large_warps<R, MODE>() * 32,
                           large_smem<R, MODE>(), a.st, a.x, a.x_stride, a.n_frames, a.hop, a.out, a.osc, a.osf,
                           reinterpret_cast<const float2 *>(pl.win_dev.get()), pl.wlane_dev.get(), pl.tw_dev.get(),
-                          pl.comb_dev.get(), pl.post_dev.get(), a.total, ha);
+                          pl.comb_dev.get(), pl.post_dev.get(), a.total, ha, a.scr);
     });
 }
 template <int R>
 int launch_multi(frt_ctx *h, const StftPlan &pl, const Frames &a) {
-    long long per_sm = R == 8 ? 2 : (R == 4 ? 4 : 8);
-    const size_t screen_smem = multi_smem(R) + sizeof(float) * (1024 * R + 1);
-    // kModeScreen: as many CTAs per SM as its 228 KB hold (1 KB of each CTA's is reserved)
-    if (a.mode == kModeScreen) per_sm = std::min<long long>(per_sm, (228 * 1024) / (screen_smem + 1024));
-    long long blocks = (long long)h->sm_count * per_sm;
-    if (blocks > a.total) blocks = a.total;
-    const float2 *w2 = reinterpret_cast<const float2 *>(pl.win_dev.get());
-    if (a.mode == kModeScreen)
-        return frt_launch(h, stft_multi_screen_kernel<R>, (unsigned)blocks, 32 * R, screen_smem, a.st, a.x,
-                          a.x_stride, a.n_frames, a.hop, a.out, a.osc, a.osf, w2, pl.tw_dev.get(), pl.comb_dev.get(),
-                          pl.post_dev.get(), a.total, a.vec_ok, a.scr);
     return with_mode(a.mode, [&](auto m) {
-        return frt_launch(h, stft_multi_kernel<R, decltype(m)::value>, (unsigned)blocks, 32 * R, multi_smem(R),
-                          a.st, a.x, a.x_stride, a.n_frames, a.hop, a.out, a.osc, a.osf, w2, pl.tw_dev.get(),
-                          pl.comb_dev.get(), pl.post_dev.get(), a.total, a.vec_ok);
+        constexpr int MODE = decltype(m)::value;
+        long long blocks = (long long)h->sm_count * multi_ctas_per_sm<R, MODE>();
+        if (blocks > a.total) blocks = a.total;
+        return frt_launch(h, stft_multi_kernel<R, MODE>, (unsigned)blocks, 32 * R, multi_smem<R, MODE>(), a.st, a.x,
+                          a.x_stride, a.n_frames, a.hop, a.out, a.osc, a.osf,
+                          reinterpret_cast<const float2 *>(pl.win_dev.get()), pl.tw_dev.get(), pl.comb_dev.get(),
+                          pl.post_dev.get(), a.total, a.align >= 1, a.scr);
     });
 }
 
@@ -1043,32 +942,9 @@ extern "C" int frt_stft_window(frt_handle h, float *window_host) {
     return FRT_OK;
 }
 
-static int stft_dispatch(frt_ctx *h, const StftPlan &pl, const Frames &a);
-
-extern "C" int frt_stft_process(frt_handle h, const float *x_dev, int64_t x_stride,
-                                int n_channels, int64_t n_frames, int hop, float *out_dev,
-                                int64_t out_stride_c, int64_t out_stride_f, int mode,
-                                void *stream) {
-    if (!h) return FRT_EINVAL;
-    DeviceGuard g(h->device);
-    if (!h->stft) return frt_fail(h, FRT_ESTATE, "frt_stft_process: call frt_stft_plan first");
-    const StftPlan &pl = *h->stft;
-    FRT_CHECK_ARG(h, n_channels >= 0 && n_frames >= 0, "negative shape");
-    FRT_CHECK_ARG(h, hop >= 1, "hop must be >= 1");
-    FRT_CHECK_ARG(h, mode == FRT_STFT_POWER || mode == FRT_STFT_LOGPOWER, "unknown mode");
-    if (n_channels == 0 || n_frames == 0) return FRT_OK;   // empty input: nothing to do
-    FRT_CHECK_ARG(h, x_dev != nullptr && out_dev != nullptr, "NULL buffer");
-    const int nbins = pl.n_fft / 2 + 1;
-    FRT_CHECK_ARG(h, out_stride_f >= nbins, "out_stride_f smaller than n_fft/2+1");
-    const long long total = (long long)n_channels * n_frames;
-    const Frames a{x_dev, x_stride, n_frames, hop, out_dev, out_stride_c, out_stride_f, total,
-                   mode, frame_alignment(x_dev, x_stride, hop) >= 1, (cudaStream_t)stream, ScreenRows{}};
-    return stft_dispatch(h, pl, a);
-}
-
 // the kernel family for the plan's size and the frames' alignment, for every output mode
 static int stft_dispatch(frt_ctx *h, const StftPlan &pl, const Frames &a) {
-    const int N = pl.n_fft, align = frame_alignment(a.x, a.x_stride, a.hop);
+    const int N = pl.n_fft;
     if (N >= 64 && N <= 2048) {
         switch (N / 64) {
             case 1: return launch_small<1>(h, pl, a);
@@ -1077,11 +953,11 @@ static int stft_dispatch(frt_ctx *h, const StftPlan &pl, const Frames &a) {
             case 8: return launch_small<8>(h, pl, a);
             case 16: return launch_small<16>(h, pl, a);
             default:   // 16-byte aligned frames: the TMA engine stages them (cp.async.bulk)
-                if (align == 2) return launch_small<32, true>(h, pl, a);
+                if (a.align == 2) return launch_small<32, true>(h, pl, a);
                 return launch_small<32>(h, pl, a);
         }
     }
-    if ((N == 4096 || N == 8192) && a.vec_ok) {
+    if ((N == 4096 || N == 8192) && a.align >= 1) {
         if (N == 4096) return launch_large<2>(h, pl, a);
         return launch_large<4>(h, pl, a);
     }
@@ -1095,13 +971,43 @@ static int stft_dispatch(frt_ctx *h, const StftPlan &pl, const Frames &a) {
     int threads = M / 4;
     if (threads < 32) threads = 32;
     if (threads > 512) threads = 512;
-    if (a.mode == kModeScreen)
-        return frt_launch(h, stft_generic_screen_kernel, (unsigned)a.total, threads, sizeof(float2) * 2 * M, a.st,
-                          a.x, a.x_stride, a.n_frames, a.hop, a.out, a.osc, a.osf, pl.win_dev.get(), pl.tw_dev.get(),
-                          pl.post_dev.get(), N, ilog2(M), a.scr);
-    return frt_launch(h, stft_generic_kernel, (unsigned)a.total, threads, sizeof(float2) * 2 * M, a.st, a.x,
-                      a.x_stride, a.n_frames, a.hop, a.out, a.osc, a.osf, pl.win_dev.get(),
-                      pl.tw_dev.get(), pl.post_dev.get(), a.mode, N, ilog2(M));
+    return with_mode(a.mode, [&](auto m) {
+        return frt_launch(h, stft_generic_kernel<decltype(m)::value>, (unsigned)a.total, threads,
+                          sizeof(float2) * 2 * M, a.st, a.x, a.x_stride, a.n_frames, a.hop, a.out, a.osc, a.osf,
+                          pl.win_dev.get(), pl.tw_dev.get(), pl.post_dev.get(), N, ilog2(M), a.scr);
+    });
+}
+
+// What frt_stft_process and frt_stft_screen_rows (mode kModeScreen) share, in order: the plan, the shape
+// and hop checks, the entry point's own check on its other scalars (bad_args: why they are refused, or
+// NULL), nothing to do on empty input, the buffers (tables_ok: the entry point's own ones are set), room
+// for a frame's bins or screen rows at out_stride_f, and the launch.
+static int stft_call(frt_ctx *h, const char *fn, const float *x, int64_t x_stride, int n_channels,
+                     int64_t n_frames, int hop, float *out, int64_t out_stride_c, int64_t out_stride_f, int mode,
+                     const ScreenRows &scr, const char *bad_args, bool tables_ok, void *stream) {
+    if (!h->stft) return frt_fail(h, FRT_ESTATE, "%s: call frt_stft_plan first", fn);
+    const StftPlan &pl = *h->stft;
+    FRT_CHECK_ARG(h, n_channels >= 0 && n_frames >= 0, "negative shape");
+    FRT_CHECK_ARG(h, hop >= 1, "hop must be >= 1");
+    if (bad_args) return frt_fail(h, FRT_EINVAL, "%s", bad_args);
+    if (n_channels == 0 || n_frames == 0) return FRT_OK;   // empty input: nothing to do
+    FRT_CHECK_ARG(h, x && out && tables_ok, "NULL buffer");
+    FRT_CHECK_ARG(h, out_stride_f >= (mode == kModeScreen ? scr.height : pl.n_fft / 2 + 1),
+                  "frame stride smaller than a frame's bins or screen rows");
+    const Frames a{x, x_stride, n_frames, hop, out, out_stride_c, out_stride_f, (long long)n_channels * n_frames,
+                   mode, frame_alignment(x, x_stride, hop), (cudaStream_t)stream, scr};
+    return stft_dispatch(h, pl, a);
+}
+
+extern "C" int frt_stft_process(frt_handle h, const float *x_dev, int64_t x_stride,
+                                int n_channels, int64_t n_frames, int hop, float *out_dev,
+                                int64_t out_stride_c, int64_t out_stride_f, int mode,
+                                void *stream) {
+    if (!h) return FRT_EINVAL;
+    DeviceGuard g(h->device);
+    const bool known = mode == FRT_STFT_POWER || mode == FRT_STFT_LOGPOWER;
+    return stft_call(h, "frt_stft_process", x_dev, x_stride, n_channels, n_frames, hop, out_dev, out_stride_c,
+                     out_stride_f, mode, ScreenRows{}, known ? nullptr : "unknown mode", true, stream);
 }
 
 extern "C" int frt_stft_screen_rows(frt_handle h, const float *x_dev, int64_t x_stride, int n_channels,
@@ -1111,18 +1017,10 @@ extern "C" int frt_stft_screen_rows(frt_handle h, const float *x_dev, int64_t x_
                                     void *stream) {
     if (!h) return FRT_EINVAL;
     DeviceGuard g(h->device);
-    if (!h->stft) return frt_fail(h, FRT_ESTATE, "frt_stft_screen_rows: call frt_stft_plan first");
-    FRT_CHECK_ARG(h, n_channels >= 0 && n_frames >= 0 && height >= 1, "bad shape");
-    FRT_CHECK_ARG(h, hop >= 1, "hop must be >= 1");
-    FRT_CHECK_ARG(h, spec_max != spec_min, "empty dB range");
-    if (n_channels == 0 || n_frames == 0) return FRT_OK;   // empty input: nothing to do
-    FRT_CHECK_ARG(h, x_dev && row_i0_dev && row_t_dev && rows_dev, "NULL buffer");
-    FRT_CHECK_ARG(h, rows_stride_f >= height, "rows_stride_f smaller than height");
-    ScreenRows scr{weight_dev, row_i0_dev, row_t_dev, spec_min, 1.0f / (spec_max - spec_min), height};
-    const Frames a{x_dev, x_stride, n_frames, hop, rows_dev, rows_stride_c, rows_stride_f,
-                   (long long)n_channels * n_frames, kModeScreen, frame_alignment(x_dev, x_stride, hop) >= 1,
-                   (cudaStream_t)stream, scr};
-    return stft_dispatch(h, *h->stft, a);
+    const char *bad = height < 1 ? "height must be >= 1" : (spec_max == spec_min ? "empty dB range" : nullptr);
+    const ScreenRows scr{weight_dev, row_i0_dev, row_t_dev, spec_min, 1.0f / (spec_max - spec_min), height};
+    return stft_call(h, "frt_stft_screen_rows", x_dev, x_stride, n_channels, n_frames, hop, rows_dev, rows_stride_c,
+                     rows_stride_f, kModeScreen, scr, bad, row_i0_dev && row_t_dev, stream);
 }
 
 extern "C" int frt_stft_process_host(frt_handle h, const float *x_host, int64_t x_stride,

@@ -202,50 +202,36 @@ class SpectrogramDisplay:
             self._old = torch.zeros((self.n_channels, self.height), dtype=torch.float32, device=device)
 
     def push(self, db, stream=None):
-        import torch
-        if db.dim() != 3 or db.shape[0] != self.n_channels or db.shape[2] != len(self.freq):
-            raise ValueError("db must be [%d, F, %d]" % (self.n_channels, len(self.freq)))
-        if not db.is_contiguous():
-            raise ValueError("db must be a contiguous CUDA float32 tensor")
-        _lib.check_tensor(self, db, "db")
-        C, F, nb = db.shape
-        with _lib.call_stream(db.device, stream) as sp:
-            self._ensure(db.device)
-            cols, a = self.index.push(F)
-            n_out = len(cols)
-            pixels = torch.empty((C, self.height, n_out), dtype=torch.int32, device=db.device)
-            if F == 0:
-                return pixels
-            cols_d = _upload(cols, db.device) if n_out else None
-            a_d = _upload(a.astype(np.float32), db.device) if n_out else None
-            T = self._tables
-            self.handle.call("frt_display_columns", _lib._ptr(db), int(F * nb), int(nb), int(C), int(F),
-                             int(nb), _lib._ptr(T["w"]), c_float(self.spec_min), c_float(self.spec_max),
-                             _lib._ptr(T["i0"]), _lib._ptr(T["t"]), int(self.height), _lib._ptr(cols_d),
-                             _lib._ptr(a_d), int(n_out), _lib._ptr(self._old), _lib._ptr(T["lut"]),
-                             _lib._ptr(pixels) if n_out else None, sp)
-        return pixels
+        return self._push("frt_display_columns", db, "db", len(self.freq), stream, lambda T: (
+            _lib._ptr(T["w"]), c_float(self.spec_min), c_float(self.spec_max), _lib._ptr(T["i0"]), _lib._ptr(T["t"]),
+            int(self.height)))
 
     def push_rows(self, rows, stream=None):
         """``push`` for rows already on the screen grid: rows [C, F, height] contiguous CUDA float32,
         made with this object's current ``tables`` and dB range."""
+        return self._push("frt_display_rows", rows, "rows", self.height, stream, lambda T: ())
+
+    def _push(self, fn, x, name, width, stream, table_args):
+        """What push and push_rows share: x [C, F, width] is checked, the time resampler advances by F
+        columns and ``fn`` (frt_display_columns or frt_display_rows) draws them, with ``table_args(tables)``
+        between the input's shape and the resampler's arguments."""
         import torch
-        if rows.dim() != 3 or rows.shape[0] != self.n_channels or rows.shape[2] != self.height:
-            raise ValueError("rows must be [%d, F, %d]" % (self.n_channels, self.height))
-        if not rows.is_contiguous():
-            raise ValueError("rows must be a contiguous CUDA float32 tensor")
-        _lib.check_tensor(self, rows, "rows")
-        C, F, H = rows.shape
-        with _lib.call_stream(rows.device, stream) as sp:
-            self._ensure(rows.device)
+        if x.dim() != 3 or x.shape[0] != self.n_channels or x.shape[2] != width:
+            raise ValueError("%s must be [%d, F, %d]" % (name, self.n_channels, width))
+        if not x.is_contiguous():
+            raise ValueError("%s must be a contiguous CUDA float32 tensor" % name)
+        _lib.check_tensor(self, x, name)
+        C, F, W = x.shape
+        with _lib.call_stream(x.device, stream) as sp:
+            self._ensure(x.device)
             cols, a = self.index.push(F)
             n_out = len(cols)
-            pixels = torch.empty((C, H, n_out), dtype=torch.int32, device=rows.device)
+            pixels = torch.empty((C, self.height, n_out), dtype=torch.int32, device=x.device)
             if F == 0:
                 return pixels
-            cols_d = _upload(cols, rows.device) if n_out else None
-            a_d = _upload(a.astype(np.float32), rows.device) if n_out else None
-            self.handle.call("frt_display_rows", _lib._ptr(rows), int(F * H), int(H), int(C), int(F), int(H),
+            cols_d = _upload(cols, x.device) if n_out else None
+            a_d = _upload(a.astype(np.float32), x.device) if n_out else None
+            self.handle.call(fn, _lib._ptr(x), int(F * W), int(W), int(C), int(F), int(W), *table_args(self._tables),
                              _lib._ptr(cols_d), _lib._ptr(a_d), int(n_out), _lib._ptr(self._old),
                              _lib._ptr(self._tables["lut"]), _lib._ptr(pixels) if n_out else None, sp)
         return pixels
