@@ -48,6 +48,7 @@ extern "C" int frt_create(int device, frt_handle *out) {
     if (!h) return frt_fail(nullptr, FRT_ENOMEM, "frt_create: out of host memory");
     h->device = device;
     h->sm_count = prop.multiProcessorCount;
+    h->smem_optin = prop.sharedMemPerBlockOptin;
     *out = h;
     return FRT_OK;
 }

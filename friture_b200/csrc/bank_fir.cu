@@ -276,6 +276,13 @@ extern "C" int frt_firbank_plan(frt_handle h, int n_channels, int bands_per_octa
     FRT_CHECK_ARG(h, n_octaves >= 1 && n_octaves <= FIR_MAX_OCT, "n_octaves must be in [1, 10]");
     FRT_CHECK_ARG(h, n_taps >= 2 && n_taps <= 1024, "n_taps must be in [2, 1024]");
     FRT_CHECK_ARG(h, fir_band && fir_dec, "NULL tap table");
+    // the taps, the histories and two stage buffers live in one CTA's shared memory: a bank that does
+    // not fit even at its shortest block, 2^(n_octaves-1), cannot run at all
+    const size_t need = FirSmem(n_taps, bands_per_octave, n_octaves, 1 << (n_octaves - 1)).total;
+    if (need > h->smem_optin)
+        return frt_fail(h, FRT_EINVAL,
+                        "frt_firbank_plan: the bank needs %zu bytes of shared memory at its shortest block, "
+                        "the device allows %zu per block", need, h->smem_optin);
     PlanPtr<FirPlan> pl(new (std::nothrow) FirPlan());
     if (!pl) return frt_fail(h, FRT_ENOMEM, "out of host memory");
     pl->n_channels = n_channels;
@@ -333,6 +340,15 @@ extern "C" int frt_firbank_set_smoothing(frt_handle h, const double *alphas, con
     return FRT_OK;
 }
 
+// Shared memory of one CTA at a block length; fir_bank_kernel declares no static shared memory.
+static int fir_check_block(frt_handle h, const FirPlan *pl, int block, const char *fn) {
+    const size_t need = FirSmem(pl->L, pl->bpo, pl->n_oct, block).total;
+    if (need > h->smem_optin)
+        return frt_fail(h, FRT_EINVAL, "%s: a block of %d samples needs %zu bytes of shared memory, the device "
+                        "allows %zu per block", fn, block, need, h->smem_optin);
+    return FRT_OK;
+}
+
 static int fir_launch(frt_handle h, FirPlan *pl, FirArgs &a, void *stream) {
     a.L = pl->L;
     a.bpo = pl->bpo;
@@ -363,6 +379,7 @@ extern "C" int frt_firbank_process(frt_handle h, const float *x_dev, int64_t x_s
     long long need = 0;
     for (int j = 0; j < pl->n_oct; j++) need += (long long)pl->bpo * (n_samples >> j);
     FRT_CHECK_ARG(h, y_stride >= need, "y_stride smaller than the ragged output size");
+    if (int rc = fir_check_block(h, pl, n_samples, "frt_firbank_process")) return rc;
     FirArgs a = {};
     a.x = x_dev;
     a.x_stride = x_stride;
@@ -392,6 +409,7 @@ extern "C" int frt_firbank_levels(frt_handle h, const float *x_dev, int64_t x_st
         FRT_CHECK_ARG(h, (block >> j) <= (8192 >> j), "block longer than the smoothing kernel");
     FRT_CHECK_ARG(h, x_dev && levels_dev, "NULL buffer");
     FRT_CHECK_ARG(h, x_stride >= (int64_t)block * n_blocks, "x_stride smaller than block*n_blocks");
+    if (int rc = fir_check_block(h, pl, block, "frt_firbank_levels")) return rc;
     FirArgs a = {};
     a.x = x_dev;
     a.x_stride = x_stride;

@@ -175,6 +175,7 @@ int gcc_long_phat_pairs(frt_ctx *h, const float *x_dev, int64_t stride, const Gc
 struct frt_ctx {
     int device = 0;
     int sm_count = 0;
+    size_t smem_optin = 0;            // cudaDeviceProp::sharedMemPerBlockOptin of the device
     int64_t launches = 0;
     std::string err;
     std::map<int, StftPlan> stft_cache;  // every size planned so far
@@ -240,9 +241,11 @@ int frt_launch(frt_ctx *h, void (*kernel)(Params...), dim3 grid, dim3 block, siz
                Args &&...args) {
     if (smem > FRT_SMEM_NO_OPT_IN) {
         const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess)
+        if (e != cudaSuccess) {
+            cudaGetLastError();   // the runtime also keeps it as the last error: the next launch must not see it
             return frt_fail(h, FRT_ECUDA, "cudaFuncSetAttribute(%zu bytes of dynamic shared memory) failed: %s",
                             smem, cudaGetErrorString(e));
+        }
     }
     kernel<<<grid, block, smem, st>>>(std::forward<Args>(args)...);
     const cudaError_t e = cudaGetLastError();

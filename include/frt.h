@@ -152,7 +152,13 @@ int frt_bank_set_state(frt_handle h, const float *z_host, const float *ema_host)
  * n_taps-1 inputs of every stage.  Parity mode; the IIR bank above is the throughput path.
  *   fir_band [bands_per_octave][n_taps], fir_dec [n_taps]  (float64 taps)
  *   process: n_samples <= 4096 and a multiple of 2^(n_octaves-1); y_dev ragged as in frt_bank_process
- * plan and reset zero the filter history and the smoothed levels of frt_firbank_levels.          */
+ * plan and reset zero the filter history and the smoothed levels of frt_firbank_levels.
+ * One CTA per channel holds the taps, every stage's history and two stage buffers in shared memory:
+ *     8 ((bpo+1) n_taps) + 4 (n_octaves (n_taps-1) + 2 round4(n_taps) + 1.5 block) bytes, about,
+ * which must fit the device's opt-in limit per block (227 KiB on an H100).  frt_firbank_plan refuses
+ * (FRT_EINVAL) a bank that does not fit at its shortest block, 2^(n_octaves-1); process and levels
+ * refuse a block that does not fit, before any launch and with the plan's state unchanged.  The
+ * library's 512-tap tables fit at every block (153 728 bytes at most: bpo 24, 10 octaves, 4096).  */
 int frt_firbank_plan(frt_handle h, int n_channels, int bands_per_octave, int n_octaves, int n_taps,
                      const double *fir_band, const double *fir_dec);
 int frt_firbank_reset(frt_handle h);
