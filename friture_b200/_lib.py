@@ -103,6 +103,12 @@ SIGNATURES = {
     "frt_spectrum_reduce_dual_ticks": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int,
                                                c_int, c_int, c_int, c_float, c_void_p, c_void_p,
                                                c_void_p, c_void_p, c_void_p, c_void_p]),
+    "frt_spectrum_frames": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int64, c_int, c_void_p, c_int,
+                                    c_float, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_void_p,
+                                    c_void_p, c_void_p]),
+    "frt_spectrum_frames_dual": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int64, c_int,
+                                         c_void_p, c_int, c_float, c_void_p, c_void_p, c_void_p, c_int64,
+                                         c_int64, c_void_p, c_void_p, c_void_p]),
     "frt_plot_curves": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int, c_int, c_int, c_double,
                                 c_double, c_double, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                 c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),

@@ -295,6 +295,46 @@ __device__ __forceinline__ float screen_value(const float *__restrict__ col, con
     return fmaf(t, b - a, a);
 }
 
+// ---- the spectrum widget's per-bin arithmetic, shared by the reduction kernels (reduce.cu) and the
+// STFT kernels' smoothing output (stft.cu), so that both produce the same bits.
+//
+// One frame of exponential smoothing, s <- alpha x + (1-alpha) s (friture/signal/exp_smoothing.py:59-107),
+// as s + alpha (x - s) in double.  In float32, (1-alpha) rounded biases the fixed point by about
+// eps/alpha, and rounding every frame walks s off by about eps/sqrt(alpha): 1e-4 and 4e-6 of the peak at
+// N = 32, T = 5 s (alpha = 3.5e-5).  The callers round s to float32 once per tick.
+__device__ __forceinline__ double smooth_step(double s, float x, double a) { return fma(a, (double)x - s, s); }
+
+// dB of one smoothed bin, 10 log10(sp + 1e-30) + weight (friture/spectrum.py:95-101,171).  The product
+// and the sum are rounded separately, as the widget's NumPy does.
+__device__ __forceinline__ float db_single(float sp, const float *__restrict__ weight, int k) {
+    float v = __fmul_rn(kLog10Scale, lg2_fast(sp + 1e-30f));
+    if (weight) v = __fadd_rn(v, __ldg(weight + k));
+    return v;
+}
+
+// The transfer function 10 log10(sp2 + 1e-30) - 10 log10(sp1 + 1e-30) (spectrum.py:168-169), as the
+// log of the ratio in double: two float32 dB values near -160 dB carry an ulp of 1.5e-5 dB each, and a
+// silent reference against a loud measurement gives a ratio past the float32 range (1e10 / 1e-30).
+__device__ __forceinline__ float db_dual(float sp1, float sp2) {
+    return (float)(10.0 * log10(((double)sp2 + 1e-30) / ((double)sp1 + 1e-30)));
+}
+
+// Term k of the 3-harmonic product spectrum of the float32 smoothed power sp (spectrum.py:103-123), in
+// double: a float32 product of three quiet bins (power 1e-16) underflows to 0 and the arg-max falls to
+// index 0.  T is float (a stored row) or double (a row of float32 values held in double).
+template <class T>
+__device__ __forceinline__ double hps_term(const T *sp, int k) {
+    return __dmul_rn(__dmul_rn((double)sp[k], (double)sp[2 * k]), (double)sp[3 * k]);
+}
+
+// The first arg-max: the larger value, the lower index on a tie.
+__device__ __forceinline__ void argmax_merge(double &best, int &besti, double ob, int oi) {
+    if (ob > best || (ob == best && oi < besti)) {
+        best = ob;
+        besti = oi;
+    }
+}
+
 // cp.async: global -> shared copies that bypass the registers, waited for by commit group
 __device__ __forceinline__ unsigned smem_u32(const void *p) {
     return (unsigned)__cvta_generic_to_shared(p);

@@ -10,13 +10,6 @@
 
 namespace {
 
-__device__ __forceinline__ void argmax_merge(double &best, int &besti, double ob, int oi) {
-    if (ob > best || (ob == best && oi < besti)) {
-        best = ob;
-        besti = oi;
-    }
-}
-
 __device__ int block_argmax(double best, int besti, double *s_val, int *s_idx) {
     for (int o = 16; o > 0; o >>= 1) {
         const double ob = __shfl_xor_sync(0xffffffffu, best, o);
@@ -45,22 +38,19 @@ __device__ int block_argmax(double best, int besti, double *s_val, int *s_idx) {
     return s_idx[32];
 }
 
-// s <- alpha x + (1-alpha) s  (exp_smoothing.py:59-107), as s + alpha (x - s) in double across
-// n_frames frames of one bin of NCH channels side by side (their loads in flight together).
+// smooth_step across n_frames frames of one bin of NCH channels side by side (their loads in flight
+// together).
 template <int NCH>
 __device__ __forceinline__ void smooth_frames(const float *const (&p)[NCH], long long stride_f,
                                               int n_frames, double a, double (&s)[NCH]) {
     for (int f = 0; f < n_frames; f++) {
 #pragma unroll
         for (int i = 0; i < NCH; i++)
-            s[i] = fma(a, (double)__ldg(p[i] + (size_t)f * stride_f) - s[i], s[i]);
+            s[i] = smooth_step(s[i], __ldg(p[i] + (size_t)f * stride_f), a);
     }
 }
 
-// One tick of smooth_frames; the carried states d are read and written back rounded to float32.  In
-// float32, (1-alpha) rounded biases the fixed point by about eps/alpha, and rounding every frame walks
-// s off by about eps/sqrt(alpha): 1e-4 and 4e-6 of the peak at N = 32, T = 5 s (alpha = 3.5e-5).
-// Here s is rounded once per tick.
+// One tick of smooth_frames; the carried states d are read and written back rounded to float32.
 template <int NCH>
 __device__ __forceinline__ void smooth_bin(const float *const (&p)[NCH], long long stride_f,
                                            int n_frames, double a, float *const (&d)[NCH],
@@ -76,30 +66,13 @@ __device__ __forceinline__ void smooth_bin(const float *const (&p)[NCH], long lo
     }
 }
 
-// dB of one smoothed bin, 10 log10(sp + 1e-30) + weight (spectrum.py:95-101,171).  The product and
-// the sum are rounded separately, as the widget's NumPy does.
-__device__ __forceinline__ float db_single(float sp, const float *__restrict__ weight, int k) {
-    float v = __fmul_rn(kLog10Scale, lg2_fast(sp + 1e-30f));
-    if (weight) v = __fadd_rn(v, __ldg(weight + k));
-    return v;
-}
-
-// The transfer function 10 log10(sp2 + 1e-30) - 10 log10(sp1 + 1e-30) (spectrum.py:168-169), as the
-// log of the ratio in double: two float32 dB values near -160 dB carry an ulp of 1.5e-5 dB each, and a
-// silent reference against a loud measurement gives a ratio past the float32 range (1e10 / 1e-30).
-__device__ __forceinline__ float db_dual(float sp1, float sp2) {
-    return (float)(10.0 * log10(((double)sp2 + 1e-30) / ((double)sp1 + 1e-30)));
-}
-
-// The first arg-max of the harmonic product spectrum of sp[0 .. nbins), 3 harmonics
-// (spectrum.py:103-123), in double: a float32 product of three quiet bins (power 1e-16) underflows to
-// 0 and the arg-max falls to index 0.
+// The first arg-max of the harmonic product spectrum of sp[0 .. nbins), 3 harmonics (hps_term).
 __device__ __forceinline__ int hps_argmax(const float *sp, int nbins, double *s_val, int *s_idx) {
     const int h = nbins / 3;
     double bestp = -INFINITY;
     int besti = 0x7fffffff;
     for (int k = threadIdx.x; k < h; k += blockDim.x) {
-        const double r = (double)sp[k] * sp[2 * k] * sp[3 * k];
+        const double r = hps_term(sp, k);
         if (r > bestp) {
             bestp = r;
             besti = k;

@@ -128,9 +128,22 @@ __host__ __device__ constexpr int brevq(int r) {
     return o;
 }
 
+// Fourth output of the STFT kernels (frt_spectrum_frames / _dual): each frame's power column goes
+// straight into the spectrum widget's smoothing (smooth_step) and is never stored.  kModeSmoothDual
+// transforms a (reference, measurement) pair per channel and smooths both.
+constexpr int kModeScreen = 2;
+constexpr int kModeSmooth = 3;
+constexpr int kModeSmoothDual = 4;
+// the smoothed states per channel: 0 for the other outputs
+__host__ __device__ constexpr int smooth_nch(int mode) {
+    return mode == kModeSmooth ? 1 : (mode == kModeSmoothDual ? 2 : 0);
+}
+
 template <int MODE>
 __device__ __forceinline__ float finish(float mag2, float scale) {
-    // mag2*scale = |X|^2/N^2 (audioproc.py:49-50); log mode: spectrogram.py:119-125
+    // mag2*scale = |X|^2/N^2 (audioproc.py:49-50); log mode: spectrogram.py:119-125.  The smoothing
+    // output rounds the product on its own, so that no contraction reaches into the smoothing.
+    if (smooth_nch(MODE)) return __fmul_rn(mag2, scale);
     if (MODE == FRT_STFT_POWER) return mag2 * scale;
     return kLog10Scale * lg2_fast(fmaf(mag2, scale, kEps));
 }
@@ -139,9 +152,7 @@ __device__ __forceinline__ float finish(float mag2, float scale) {
 // FRT_STFT_LOGPOWER computes it, stays in shared memory and only its `height` screen rows are written,
 // row r = screen_value of the column (what display_kernel computes from a stored column).  Every kernel
 // family takes the output as its MODE template argument and the screen tables as its last parameter,
-// which the other two modes leave unused (launched as ScreenRows{}).
-constexpr int kModeScreen = 2;
-
+// which the other modes leave unused (launched as ScreenRows{}).
 struct ScreenRows {
     const float *weight;   // [nbins] dB or NULL
     const int *i0;         // [height] bin index of each row, 0 <= i0 <= nbins - 2
@@ -156,6 +167,146 @@ __device__ __forceinline__ void write_rows(const float *s_col, float *__restrict
                                            int i, int n) {
     for (int r = i; r < s.height; r += n)
         rows[r] = screen_value<true>(s_col, s.weight, __ldg(s.i0 + r), __ldg(s.t + r), s.spec_min, s.inv_range);
+}
+
+// The smoothing outputs' arguments (the other modes launch with SmoothTicks{}).  Channel c's frames are
+// those of frt_stft_process; in kModeSmoothDual frame f of its measurement row starts at
+// x2 + c x_stride + f hop.  A slot walks its channel's frames as items i = NCH f + j in order (j = 1:
+// the measurement), every item's power column going into state j.
+struct SmoothTicks {
+    const float *x2;
+    const int *tick_end;   // [n_ticks] the frame at which each tick ends, strictly ascending
+    int n_ticks, n_channels;
+    float alpha;
+    float *disp[2];        // [C][nbins] carried states, float32
+    const float *weight;   // [nbins] dB or NULL (kModeSmooth)
+    float *db;             // row r of channel c at db + c db_sc + r db_sr, or NULL
+    long long db_sc, db_sr;
+    int *imax, *ipitch;    // [n_ticks][C]
+};
+
+// One slot of a smoothing output: n threads (t = 0..n-1, whole warps) walk one channel's frames in
+// order, its NCH states in shared memory in double (st: [NCH][nb]).  A state is read from disp once at
+// the channel's start and written once at its end, and each tick end rounds it to float32, writes the
+// tick's dB row and its two arg-maxes, as spectrum_reduce_kernel does for one tick.  s_val / s_idx:
+// [n/32] scratch of the arg-maxes when the slot has more than one warp; sync() is the slot's barrier.
+template <int NCH, class Sync>
+struct Smoother {
+    const SmoothTicks &sm;
+    double *st;
+    double *s_val;
+    int *s_idx;
+    int nb, t, n;
+    Sync sync;
+    double a;
+    long long c = 0;
+    int r = 0;
+
+    __device__ Smoother(const SmoothTicks &sm_, double *st_, double *s_val_, int *s_idx_, int nb_, int t_, int n_,
+                        Sync sync_)
+        : sm(sm_), st(st_), s_val(s_val_), s_idx(s_idx_), nb(nb_), t(t_), n(n_), sync(sync_), a(sm_.alpha) {}
+
+    __device__ void begin(long long ch) {
+        c = ch;
+        r = 0;
+        for (int j = 0; j < NCH; j++)
+            for (int k = t; k < nb; k += n) st[j * nb + k] = sm.disp[j][(size_t)c * nb + k];
+        sync();
+    }
+    __device__ __forceinline__ void add(int j, int k, float p) { st[j * nb + k] = smooth_step(st[j * nb + k], p, a); }
+    // after item i of the channel, every thread's adds made: the end of a tick?
+    __device__ __forceinline__ void after(long long i) {
+        if (i % NCH == NCH - 1 && r < sm.n_ticks && i / NCH + 1 == __ldg(sm.tick_end + r)) tick();
+    }
+    __device__ void end() {
+        sync();
+        for (int j = 0; j < NCH; j++)
+            for (int k = t; k < nb; k += n) sm.disp[j][(size_t)c * nb + k] = (float)st[j * nb + k];
+    }
+
+    // the slot's first arg-max, in every thread
+    __device__ int argmax(double best, int besti) {
+        for (int o = 16; o > 0; o >>= 1) {
+            const double ob = __shfl_xor_sync(0xffffffffu, best, o);
+            const int oi = __shfl_xor_sync(0xffffffffu, besti, o);
+            argmax_merge(best, besti, ob, oi);
+        }
+        if (n > 32) {
+            sync();
+            if ((t & 31) == 0) {
+                s_val[t >> 5] = best;
+                s_idx[t >> 5] = besti;
+            }
+            sync();
+            best = -INFINITY;
+            besti = 0x7fffffff;
+            for (int w = 0; w < n / 32; w++) argmax_merge(best, besti, s_val[w], s_idx[w]);
+        }
+        return besti;
+    }
+
+    __device__ void tick() {
+        sync();   // every bin has had the tick's frames
+        float best = -INFINITY;
+        int besti = 0x7fffffff;
+        for (int k = t; k < nb; k += n) {
+            const float v = (float)st[k];
+            st[k] = v;
+            float d;
+            if constexpr (NCH == 2) {
+                const float v2 = (float)st[nb + k];
+                st[nb + k] = v2;
+                d = db_dual(v, v2);
+            } else {
+                d = db_single(v, sm.weight, k);
+            }
+            if (sm.db) sm.db[c * sm.db_sc + r * sm.db_sr + k] = d;
+            if (d > best) {   // on the float32 value, as spectrum_reduce_kernel
+                best = d;
+                besti = k;
+            }
+        }
+        const int imax = argmax(best, besti);     // spectrum.py:175
+        sync();   // every bin of state 0 is rounded
+        double bp = -INFINITY;
+        int bpi = 0x7fffffff;
+        for (int k = t; k < nb / 3; k += n) {
+            const double h = hps_term(st, k);
+            if (h > bp) {
+                bp = h;
+                bpi = k;
+            }
+        }
+        const int ipitch = argmax(bp, bpi);       // spectrum.py:180
+        if (t == 0) {
+            sm.imax[(size_t)r * sm.n_channels + c] = imax;
+            sm.ipitch[(size_t)r * sm.n_channels + c] = ipitch;
+        }
+        r++;
+        sync();   // the states are read before the next frame's adds
+    }
+};
+
+// shared memory of one slot's states and arg-max scratch (warps: the slot's)
+template <int MODE>
+__host__ __device__ constexpr size_t smooth_slot_bytes(int nbins, int warps) {
+    return smooth_nch(MODE)
+               ? (sizeof(double) * smooth_nch(MODE) * nbins + (sizeof(double) + sizeof(int)) * warps + 15) / 16 * 16
+               : 0;
+}
+template <int NCH, class Sync>
+__device__ Smoother<NCH, Sync> slot_smoother(const SmoothTicks &sm, void *slot_smem, int nb, int t, int n, Sync sync) {
+    double *st = reinterpret_cast<double *>(slot_smem);
+    double *s_val = st + NCH * nb;
+    return Smoother<NCH, Sync>(sm, st, s_val, reinterpret_cast<int *>(s_val + n / 32), nb, t, n, sync);
+}
+
+// frame f of channel c (in the smoothing outputs: item f of the channel)
+template <int MODE>
+__device__ __forceinline__ const float *frame_at(const float *x, const SmoothTicks &sm, long long x_stride, int hop,
+                                                 long long c, long long f) {
+    if constexpr (MODE == kModeSmoothDual) return ((f & 1) ? sm.x2 : x) + c * x_stride + (f >> 1) * hop;
+    else return x + c * x_stride + f * hop;
 }
 
 // ---- TMA bulk copy (cp.async.bulk, SASS UBLKCP) + mbarrier helpers ------------------------------
@@ -259,9 +410,10 @@ template <> __device__ __forceinline__ void combine<8>(float2 (&t)[8]) {
 
 // The R-warp kernels' last stage: radix-R combine of the R natural-order tiles Z_w and the split
 // step of every bin of the frame, by thread t of the frame's 32 R threads.  comb(w, k0) and post(kk)
-// read W_M^(w k0) and U[kk] from wherever the kernel keeps those tables.
-template <int R, int MODE, class Comb, class Post>
-__device__ __forceinline__ void combine_split(float *__restrict__ o, const float2 *tiles, Comb comb,
+// read W_M^(w k0) and U[kk] from wherever the kernel keeps those tables.  The bins go to o, or in the
+// smoothing outputs to add(k, power): a bin's value is the last one o would hold (bin M/2 is split twice).
+template <int R, int MODE, class Comb, class Post, class Add>
+__device__ __forceinline__ void combine_split(float *__restrict__ o, Add add, const float2 *tiles, Comb comb,
                                               Post post, int t, float scale) {
     constexpr int M = 1024 * R;
     auto load_group = [&](int k0, float2(&g)[R]) {
@@ -276,8 +428,13 @@ __device__ __forceinline__ void combine_split(float *__restrict__ o, const float
         const float2 T = cmul(O, post(kk));
         const float2 X = cadd(E, T);
         const float2 Y = csub(E, T);
-        o[kk] = finish<MODE>(fmaf(X.x, X.x, X.y * X.y), scale);
-        o[M - kk] = finish<MODE>(fmaf(Y.x, Y.x, Y.y * Y.y), scale);
+        if constexpr (smooth_nch(MODE)) {
+            if (kk != M - kk) add(kk, finish<MODE>(fmaf(X.x, X.x, X.y * X.y), scale));
+            add(M - kk, finish<MODE>(fmaf(Y.x, Y.x, Y.y * Y.y), scale));
+        } else {
+            o[kk] = finish<MODE>(fmaf(X.x, X.x, X.y * X.y), scale);
+            o[M - kk] = finish<MODE>(fmaf(Y.x, Y.x, Y.y * Y.y), scale);
+        }
     };
     for (int k0 = 1 + t; k0 < 512; k0 += 32 * R) {
         float2 A[R], B[R];
@@ -301,15 +458,16 @@ __device__ __forceinline__ void combine_split(float *__restrict__ o, const float
     }
 }
 
-// kModeScreen: the frame's column goes to s_col, after the tiles, and its rows to out.
+// kModeScreen: the frame's column goes to s_col, after the tiles, and its rows to out.  Smoothing
+// outputs: one CTA per channel, its states after the tiles.
 template <int R, int MODE>
 __global__ void __launch_bounds__(32 * R)
 stft_multi_kernel(const float *__restrict__ x, long long x_stride, long long n_frames, int hop,
                   float *__restrict__ out, long long out_stride_c, long long out_stride_f,
                   const float2 *__restrict__ win2, const float2 *__restrict__ tw32,
                   const float2 *__restrict__ comb, const float2 *__restrict__ post,
-                  long long total_items, int vec_ok, const ScreenRows scr) {
-    constexpr int M = 1024 * R, N = 2 * M;
+                  long long total_items, int vec_ok, const ScreenRows scr, const SmoothTicks sm) {
+    constexpr int M = 1024 * R, N = 2 * M, NCH = smooth_nch(MODE);
     extern __shared__ float2 smem[];
     float2 *s_tw = smem;                       // [32][32] W_1024^(k1 t)
     float2 *s_tiles = s_tw + 1024;             // R padded tiles
@@ -319,10 +477,8 @@ stft_multi_kernel(const float *__restrict__ x, long long x_stride, long long n_f
     for (int i = tid; i < 1024; i += blockDim.x) s_tw[i] = tw32[i];
     __syncthreads();
     const float scale = 1.0f / (4.0f * (float)N * (float)N);
-    for (long long item = blockIdx.x; item < total_items; item += gridDim.x) {
-        const long long c = item / n_frames;
-        const long long f = item - c * n_frames;
-        const float *p = x + c * x_stride + f * hop;
+    // the frame at p into the natural-order tiles, for the combine
+    auto transform = [&](const float *p) {
         float2 v[32];
 #pragma unroll
         for (int n1 = 0; n1 < 32; n1++) {
@@ -342,18 +498,40 @@ stft_multi_kernel(const float *__restrict__ x, long long x_stride, long long n_f
 #pragma unroll
         for (int r = 0; r < 32; r++) s_x[lane + 32 * brev5(r)] = v[r];   // natural order
         __syncthreads();
-
-        auto comb_at = [=](int w, int k0) { return __ldg(comb + (w - 1) * 1024 + k0); };
-        auto post_at = [=](int kk) { return __ldg(post + kk); };
-        if constexpr (MODE == kModeScreen) {
-            combine_split<R, MODE>(s_col, s_tiles, comb_at, post_at, tid, scale);
-            __syncthreads();
-            // s_col is rewritten only after the next frame's tile barrier
-            write_rows(s_col, out + c * out_stride_c + f * out_stride_f, scr, tid, 32 * R);
-        } else {
-            combine_split<R, MODE>(out + c * out_stride_c + f * out_stride_f, s_tiles, comb_at, post_at, tid,
-                                   scale);
-            __syncthreads();
+    };
+    auto comb_at = [=](int w, int k0) { return __ldg(comb + (w - 1) * 1024 + k0); };
+    auto post_at = [=](int kk) { return __ldg(post + kk); };
+    if constexpr (NCH > 0) {
+        auto sync = [] { __syncthreads(); };
+        auto s = slot_smoother<NCH>(sm, s_tiles + R * TILE, M + 1, tid, 32 * R, sync);
+        for (long long c = blockIdx.x; c < sm.n_channels; c += gridDim.x) {
+            s.begin(c);
+            for (long long i = 0; i < NCH * n_frames; i++) {
+                transform(frame_at<MODE>(x, sm, x_stride, hop, c, i));
+                const int j = (int)(i % NCH);
+                combine_split<R, MODE>(nullptr, [&](int k, float p) { s.add(j, k, p); }, s_tiles, comb_at, post_at,
+                                       tid, scale);
+                __syncthreads();
+                s.after(i);
+            }
+            s.end();
+        }
+    } else {
+        for (long long item = blockIdx.x; item < total_items; item += gridDim.x) {
+            const long long c = item / n_frames;
+            const long long f = item - c * n_frames;
+            transform(x + c * x_stride + f * hop);
+            auto no_add = [](int, float) {};
+            if constexpr (MODE == kModeScreen) {
+                combine_split<R, MODE>(s_col, no_add, s_tiles, comb_at, post_at, tid, scale);
+                __syncthreads();
+                // s_col is rewritten only after the next frame's tile barrier
+                write_rows(s_col, out + c * out_stride_c + f * out_stride_f, scr, tid, 32 * R);
+            } else {
+                combine_split<R, MODE>(out + c * out_stride_c + f * out_stride_f, no_add, s_tiles, comb_at, post_at,
+                                       tid, scale);
+                __syncthreads();
+            }
         }
     }
 }
@@ -369,27 +547,37 @@ stft_multi_kernel(const float *__restrict__ x, long long x_stride, long long n_f
 // G frames.
 // Q = 32 (N = 2048, one frame per warp) runs one CTA of 16 warps per SM, and with TMA its 16-byte
 // aligned frames are staged by the TMA engine; smaller Q run two CTAs of 8 warps per SM.
-template <int Q> __host__ __device__ constexpr int small_warps() { return Q == 32 ? 16 : 8; }
-template <int Q> __host__ __device__ constexpr int small_ctas_per_sm() { return Q == 32 ? 1 : 2; }
+// Smoothing outputs: one warp per channel, its states after the mbarriers.  At Q = 32 a lane adds the
+// bins it splits (the same ones in every frame); smaller Q write the warp's G columns to its tile, as
+// kModeScreen does, and add them in frame order.  Q = 32 runs 8 warps there, for the states' room.
+template <int Q, int MODE = FRT_STFT_POWER> __host__ __device__ constexpr int small_warps() {
+    return Q == 32 ? (smooth_nch(MODE) ? 8 : 16) : 8;
+}
+template <int Q, int MODE = FRT_STFT_POWER> __host__ __device__ constexpr int small_ctas_per_sm() {
+    return Q == 32 || smooth_nch(MODE) ? 1 : 2;
+}
 // kModeScreen: the warp's G columns go to its tile, free again after the transpose; with TMA the tile
 // already holds the next frame by then, so each warp has a column buffer of its own after the mbarriers.
 template <int Q, int MODE, bool TMA>
 constexpr size_t small_smem() {
-    // window, twiddle and split tables, the warps' tiles, (Q = 32) the warps' mbarriers and
-    // (kModeScreen with TMA) the warps' column buffers
-    return sizeof(float2) * (32 * Q + 32 * Q + 16 * Q + (size_t)small_warps<Q>() * TILE) +
-           (Q == 32 ? sizeof(unsigned long long) * small_warps<Q>() : 0) +
-           (MODE == kModeScreen && TMA ? sizeof(float) * (size_t)small_warps<Q>() * (32 * Q + 1) : 0);
+    // window, twiddle and split tables, the warps' tiles, (Q = 32) the warps' mbarriers,
+    // (kModeScreen with TMA) the warps' column buffers and (smoothing) the warps' states
+    constexpr int W = small_warps<Q, MODE>();
+    return sizeof(float2) * (32 * Q + 32 * Q + 16 * Q + (size_t)W * TILE) +
+           (Q == 32 ? sizeof(unsigned long long) * W : 0) +
+           (MODE == kModeScreen && TMA ? sizeof(float) * (size_t)W * (32 * Q + 1) : 0) +
+           W * smooth_slot_bytes<MODE>(32 * Q + 1, 1);
 }
 
 template <int Q, int MODE, bool TMA>
-__global__ void __launch_bounds__(small_warps<Q>() * 32, small_ctas_per_sm<Q>())
+__global__ void __launch_bounds__(small_warps<Q, MODE>() * 32, small_ctas_per_sm<Q, MODE>())
 stft_small_kernel(const float *__restrict__ x, long long x_stride, long long n_frames, int hop,
                   float *__restrict__ out, long long out_stride_c, long long out_stride_f,
                   const float2 *__restrict__ win2, const float2 *__restrict__ tw,
-                  const float2 *__restrict__ post, long long total_items, int vec_ok, const ScreenRows scr) {
+                  const float2 *__restrict__ post, long long total_items, int vec_ok, const ScreenRows scr,
+                  const SmoothTicks sm) {
     static_assert(!TMA || Q == 32, "TMA staging is for one frame per warp");
-    constexpr int G = 32 / Q, M = 32 * Q, N = 2 * M, WARPS = small_warps<Q>();
+    constexpr int G = 32 / Q, M = 32 * Q, N = 2 * M, WARPS = small_warps<Q, MODE>(), NCH = smooth_nch(MODE);
     extern __shared__ float2 smem[];
     float2 *s_win = smem;              // [M]     (w[2n], w[2n+1])
     float2 *s_tw = s_win + M;          // [Q][32] W_M^(k1 t)
@@ -403,138 +591,270 @@ stft_small_kernel(const float *__restrict__ x, long long x_stride, long long n_f
     for (int i = threadIdx.x; i < 16 * Q; i += blockDim.x) s_post[i] = post[i];
     __syncthreads();
 
-    // contiguous range of frames per warp, a multiple of G long
-    // (consecutive frames of a channel stay on one SM, so the overlapping part of each frame is
-    // re-read from L1/L2, not HBM)
-    const long long warps_total = (long long)gridDim.x * WARPS;
-    const long long gw = (long long)blockIdx.x * WARPS + warp;
-    long long per = (total_items + warps_total - 1) / warps_total;
-    per = (per + G - 1) / G * G;
-    long long item = gw * per;
-    long long item_end = item + per;
-    if (item_end > total_items) item_end = total_items;
-    const float scale = 1.0f / (4.0f * (float)N * (float)N);
-    const int k1 = lane & (Q - 1), gsel = lane / Q;
-    const int src_lane = (lane - k1) + ((Q - k1) & (Q - 1));
-
-    long long c = (item < item_end) ? item / n_frames : 0;
-    long long f = item - c * n_frames;
-    // TMA: each frame's 8 KB are fetched by the TMA engine (cp.async.bulk) into the warp's tile
-    // while the frame before it is in its second FFT pass and split step, so no warp ever waits on
-    // a global load with its registers tied up.  The first frame is fetched here, each next one
-    // once the transpose has freed the tile.
-    unsigned long long *bar = reinterpret_cast<unsigned long long *>(s_post + 16 * Q + WARPS * TILE) + warp;
-    unsigned parity = 0;
-    if (TMA) {
-        if (lane == 0) mbar_init(bar, 1);
-        fence_proxy_async();
-        __syncwarp();
-        if (lane == 0 && item < item_end) {
-            mbar_expect_tx(bar, N * 4);
-            bulk_g2s(s_x, x + c * x_stride + f * hop, N * 4, bar);
+    // Smoothing outputs: warp gw walks channels gw, gw + warps_total, ..; its items are a channel's frames
+    // (kModeSmoothDual: reference and measurement in turn, frame_at).  The other outputs keep the loop below
+    // to themselves, so that their code is what it was before this output existed.
+    if constexpr (NCH > 0) {
+        const long long warps_total = (long long)gridDim.x * WARPS;
+        const float scale = 1.0f / (4.0f * (float)N * (float)N);
+        const int k1 = lane & (Q - 1), gsel = lane / Q;
+        const int src_lane = (lane - k1) + ((Q - k1) & (Q - 1));
+        unsigned long long *bar = reinterpret_cast<unsigned long long *>(s_post + 16 * Q + WARPS * TILE) + warp;
+        unsigned char *states = reinterpret_cast<unsigned char *>(bar - warp + (Q == 32 ? WARPS : 0));
+        auto s = slot_smoother<NCH>(sm, states + warp * smooth_slot_bytes<MODE>(M + 1, 1), M + 1, lane, 32,
+                                    [] { __syncwarp(); });
+        unsigned parity = 0;
+        if (TMA) {
+            if (lane == 0) mbar_init(bar, 1);
+            fence_proxy_async();
+            __syncwarp();
         }
-    }
-    for (; item < item_end; item += G) {
-        float2 v[32];
-        long long myc = 0, myf = 0;
-        bool myok = false;
-#pragma unroll
-        for (int g = 0; g < G; g++) {
-            const bool ok = item + g < item_end;
-            const float *p = x + c * x_stride + f * hop;
-            if (g == gsel) {
-                myc = c;
-                myf = f;
-                myok = ok;
+        const long long nv = NCH * n_frames;
+        for (long long ch = (long long)blockIdx.x * WARPS + warp; ch < sm.n_channels; ch += warps_total) {
+            s.begin(ch);
+            long long f = 0;   // the next item to load
+            if (TMA && lane == 0) {
+                mbar_expect_tx(bar, N * 4);
+                bulk_g2s(s_x, frame_at<MODE>(x, sm, x_stride, hop, ch, 0), N * 4, bar);
             }
-            if (TMA) {
-                mbar_wait(bar, parity);
-                parity ^= 1;
+            for (long long item = 0; item < nv; item += G) {
+                float2 v[32];
+                long long myf = 0;
+                bool myok = false;
 #pragma unroll
-                for (int n1 = 0; n1 < 32; n1++) v[n1] = s_x[32 * n1 + lane];
-                __syncwarp();   // every lane has its samples before the tile is reused for the exchange
-            } else if (ok && vec_ok) {
+                for (int g = 0; g < G; g++, f++) {
+                    const bool ok = f < nv;
+                    const float *p = frame_at<MODE>(x, sm, x_stride, hop, ch, f);
+                    if (g == gsel) {
+                        myf = f;
+                        myok = ok;
+                    }
+                    if (TMA) {
+                        mbar_wait(bar, parity);
+                        parity ^= 1;
 #pragma unroll
-                for (int n1 = 0; n1 < Q; n1++)
-                    v[g * Q + n1] = __ldg(reinterpret_cast<const float2 *>(p) + 32 * n1 + lane);
-            } else if (ok) {
+                        for (int n1 = 0; n1 < 32; n1++) v[n1] = s_x[32 * n1 + lane];
+                        __syncwarp();   // every lane has its samples before the tile is reused for the exchange
+                    } else if (ok && vec_ok) {
+#pragma unroll
+                        for (int n1 = 0; n1 < Q; n1++)
+                            v[g * Q + n1] = __ldg(reinterpret_cast<const float2 *>(p) + 32 * n1 + lane);
+                    } else if (ok) {
+#pragma unroll
+                        for (int n1 = 0; n1 < Q; n1++) {
+                            v[g * Q + n1].x = __ldg(p + 64 * n1 + 2 * lane);
+                            v[g * Q + n1].y = __ldg(p + 64 * n1 + 2 * lane + 1);
+                        }
+                    } else {
+#pragma unroll
+                        for (int n1 = 0; n1 < Q; n1++) v[g * Q + n1] = make_float2(0.0f, 0.0f);
+                    }
+                }
 #pragma unroll
                 for (int n1 = 0; n1 < Q; n1++) {
-                    v[g * Q + n1].x = __ldg(p + 64 * n1 + 2 * lane);
-                    v[g * Q + n1].y = __ldg(p + 64 * n1 + 2 * lane + 1);
+                    const float2 w = s_win[32 * n1 + lane];
+#pragma unroll
+                    for (int g = 0; g < G; g++) v[g * Q + n1] = f2_mul(v[g * Q + n1], w);
                 }
-            } else {
+                dft_groups<Q>(v);
+                twiddle_transpose<Q>(v, s_tw, s_x, lane);
+                if (TMA && f < nv) {   // the tile is free: fetch the next item into it
+                    fence_proxy_async();
+                    if (lane == 0) {
+                        mbar_expect_tx(bar, N * 4);
+                        bulk_g2s(s_x, frame_at<MODE>(x, sm, x_stride, hop, ch, f), N * 4, bar);
+                    }
+                }
+                dft32(v);   // v[r] = Z_g[k1 + Q*brev5(r)] of this lane's (g, k1)
+
+                // G = 1: the lane's bins go straight into state j; G > 1: frame g's column to the tile
+                constexpr bool direct = G == 1;
+                const int j = (int)(myf % NCH);
+                float *o = reinterpret_cast<float *>(s_x) + gsel * (M + 1);
 #pragma unroll
-                for (int n1 = 0; n1 < Q; n1++) v[g * Q + n1] = make_float2(0.0f, 0.0f);
+                for (int m = 0; m < 16; m++) {
+                    const float2 z = v[brev5(m)];
+                    const float2 other = v[brev5(31 - m)];
+                    float2 zp;
+                    zp.x = __shfl_sync(0xffffffffu, other.x, src_lane);
+                    zp.y = __shfl_sync(0xffffffffu, other.y, src_lane);
+                    if (k1 == 0) zp = (m == 0) ? v[0] : v[brev5(32 - m)];
+                    const float2 E = make_float2(z.x + zp.x, z.y - zp.y);
+                    const float2 O = make_float2(z.x - zp.x, z.y + zp.y);
+                    const int k = k1 + Q * m;
+                    const float2 T = cmul(O, s_post[k]);
+                    const float2 X = cadd(E, T);
+                    const float2 Y = csub(E, T);
+                    const float p1 = finish<MODE>(fmaf(X.x, X.x, X.y * X.y), scale);
+                    const float p2 = finish<MODE>(fmaf(Y.x, Y.x, Y.y * Y.y), scale);
+                    if (myok) {
+                        if constexpr (direct) {
+                            s.add(j, k, p1);
+                            s.add(j, M - k, p2);
+                        } else {
+                            o[k] = p1;
+                            o[M - k] = p2;
+                        }
+                    }
+                }
+                if (k1 == 0 && myok) {
+                    const float2 z = v[brev5(16)];   // bin M/2: X = conj(Z)
+                    const float p = finish<MODE>(4.0f * fmaf(z.x, z.x, z.y * z.y), scale);
+                    if constexpr (direct) s.add(j, M / 2, p);
+                    else o[M / 2] = p;
+                }
+                __syncwarp();   // every add, or the warp's G columns, complete
+                if constexpr (direct) {
+                    s.after(myf);
+                } else {
+                    const float *s_col = reinterpret_cast<const float *>(s_x);
+#pragma unroll 1
+                    for (int g = 0; g < G; g++) {   // in frame order; a lane adds the same bins every time
+                        const long long fg = item + g;
+                        if (fg >= nv) break;
+                        const int jg = (int)(fg % NCH);
+                        for (int k = lane; k <= M; k += 32) s.add(jg, k, s_col[g * (M + 1) + k]);
+                        s.after(fg);
+                    }
+                    __syncwarp();   // every lane is done with the columns before the tile is written again
+                }
             }
-            if (++f == n_frames) {
-                f = 0;
-                c++;
-            }
+            s.end();
         }
-#pragma unroll
-        for (int n1 = 0; n1 < Q; n1++) {
-            const float2 w = s_win[32 * n1 + lane];
-#pragma unroll
-            for (int g = 0; g < G; g++) v[g * Q + n1] = f2_mul(v[g * Q + n1], w);
-        }
-        dft_groups<Q>(v);   // v[g*Q + r] = sum_n1 z_g[32 n1 + t] W_Q^(n1 k1), k1 = brevq<Q>(r)
-        twiddle_transpose<Q>(v, s_tw, s_x, lane);
-        if (TMA && item + 1 < item_end) {   // the tile is free: fetch the next frame, (c, f), into it
+    } else {
+        // contiguous range of frames per warp, a multiple of G long
+        // (consecutive frames of a channel stay on one SM, so the overlapping part of each frame is
+        // re-read from L1/L2, not HBM)
+        const long long warps_total = (long long)gridDim.x * WARPS;
+        const long long gw = (long long)blockIdx.x * WARPS + warp;
+        long long per = (total_items + warps_total - 1) / warps_total;
+        per = (per + G - 1) / G * G;
+        long long item = gw * per;
+        long long item_end = item + per;
+        if (item_end > total_items) item_end = total_items;
+        const float scale = 1.0f / (4.0f * (float)N * (float)N);
+        const int k1 = lane & (Q - 1), gsel = lane / Q;
+        const int src_lane = (lane - k1) + ((Q - k1) & (Q - 1));
+
+        long long c = (item < item_end) ? item / n_frames : 0;
+        long long f = item - c * n_frames;
+        // TMA: each frame's 8 KB are fetched by the TMA engine (cp.async.bulk) into the warp's tile
+        // while the frame before it is in its second FFT pass and split step, so no warp ever waits on
+        // a global load with its registers tied up.  The first frame is fetched here, each next one
+        // once the transpose has freed the tile.
+        unsigned long long *bar = reinterpret_cast<unsigned long long *>(s_post + 16 * Q + WARPS * TILE) + warp;
+        unsigned parity = 0;
+        if (TMA) {
+            if (lane == 0) mbar_init(bar, 1);
             fence_proxy_async();
-            if (lane == 0) {
+            __syncwarp();
+            if (lane == 0 && item < item_end) {
                 mbar_expect_tx(bar, N * 4);
                 bulk_g2s(s_x, x + c * x_stride + f * hop, N * 4, bar);
             }
         }
-        dft32(v);   // v[r] = Z_g[k1 + Q*brev5(r)] of this lane's (g, k1)
+        for (; item < item_end; item += G) {
+            float2 v[32];
+            long long myc = 0, myf = 0;
+            bool myok = false;
+#pragma unroll
+            for (int g = 0; g < G; g++) {
+                const bool ok = item + g < item_end;
+                const float *p = x + c * x_stride + f * hop;
+                if (g == gsel) {
+                    myc = c;
+                    myf = f;
+                    myok = ok;
+                }
+                if (TMA) {
+                    mbar_wait(bar, parity);
+                    parity ^= 1;
+#pragma unroll
+                    for (int n1 = 0; n1 < 32; n1++) v[n1] = s_x[32 * n1 + lane];
+                    __syncwarp();   // every lane has its samples before the tile is reused for the exchange
+                } else if (ok && vec_ok) {
+#pragma unroll
+                    for (int n1 = 0; n1 < Q; n1++)
+                        v[g * Q + n1] = __ldg(reinterpret_cast<const float2 *>(p) + 32 * n1 + lane);
+                } else if (ok) {
+#pragma unroll
+                    for (int n1 = 0; n1 < Q; n1++) {
+                        v[g * Q + n1].x = __ldg(p + 64 * n1 + 2 * lane);
+                        v[g * Q + n1].y = __ldg(p + 64 * n1 + 2 * lane + 1);
+                    }
+                } else {
+#pragma unroll
+                    for (int n1 = 0; n1 < Q; n1++) v[g * Q + n1] = make_float2(0.0f, 0.0f);
+                }
+                if (++f == n_frames) {
+                    f = 0;
+                    c++;
+                }
+            }
+#pragma unroll
+            for (int n1 = 0; n1 < Q; n1++) {
+                const float2 w = s_win[32 * n1 + lane];
+#pragma unroll
+                for (int g = 0; g < G; g++) v[g * Q + n1] = f2_mul(v[g * Q + n1], w);
+            }
+            dft_groups<Q>(v);   // v[g*Q + r] = sum_n1 z_g[32 n1 + t] W_Q^(n1 k1), k1 = brevq<Q>(r)
+            twiddle_transpose<Q>(v, s_tw, s_x, lane);
+            if (TMA && item + 1 < item_end) {   // the tile is free: fetch the next frame, (c, f), into it
+                fence_proxy_async();
+                if (lane == 0) {
+                    mbar_expect_tx(bar, N * 4);
+                    bulk_g2s(s_x, x + c * x_stride + f * hop, N * 4, bar);
+                }
+            }
+            dft32(v);   // v[r] = Z_g[k1 + Q*brev5(r)] of this lane's (g, k1)
 
-        float *o;
-        if constexpr (MODE == kModeScreen) {
-            float *s_col = reinterpret_cast<float *>(s_x);
-            if (TMA)
-                s_col = reinterpret_cast<float *>(reinterpret_cast<unsigned long long *>(s_post + 16 * Q + WARPS * TILE) +
-                                                  WARPS) + warp * (M + 1);
-            o = s_col + gsel * (M + 1);
-        } else {
-            o = out + myc * out_stride_c + myf * out_stride_f;
-        }
-#pragma unroll
-        for (int m = 0; m < 16; m++) {
-            const float2 z = v[brev5(m)];
-            const float2 other = v[brev5(31 - m)];
-            float2 zp;
-            zp.x = __shfl_sync(0xffffffffu, other.x, src_lane);
-            zp.y = __shfl_sync(0xffffffffu, other.y, src_lane);
-            if (k1 == 0) zp = (m == 0) ? v[0] : v[brev5(32 - m)];
-            const float2 E = make_float2(z.x + zp.x, z.y - zp.y);
-            const float2 O = make_float2(z.x - zp.x, z.y + zp.y);
-            const int k = k1 + Q * m;
-            const float2 T = cmul(O, s_post[k]);
-            const float2 X = cadd(E, T);
-            const float2 Y = csub(E, T);
-            const float p1 = fmaf(X.x, X.x, X.y * X.y);
-            const float p2 = fmaf(Y.x, Y.x, Y.y * Y.y);
-            if (myok) {
-                o[k] = finish<MODE>(p1, scale);
-                o[M - k] = finish<MODE>(p2, scale);
+            float *o;
+            if constexpr (MODE == kModeScreen) {
+                float *s_col = reinterpret_cast<float *>(s_x);
+                if (TMA)
+                    s_col = reinterpret_cast<float *>(reinterpret_cast<unsigned long long *>(s_post + 16 * Q + WARPS * TILE) +
+                                                      WARPS) + warp * (M + 1);
+                o = s_col + gsel * (M + 1);
+            } else {
+                o = out + myc * out_stride_c + myf * out_stride_f;
             }
-        }
-        if (k1 == 0 && myok) {
-            const float2 z = v[brev5(16)];   // bin M/2: X = conj(Z)
-            o[M / 2] = finish<MODE>(4.0f * fmaf(z.x, z.x, z.y * z.y), scale);
-        }
-        if constexpr (MODE == kModeScreen) {
-            __syncwarp();   // the warp's G columns are complete
-            const float *s_col = o - gsel * (M + 1);
 #pragma unroll
-            for (int g = 0; g < G; g++) {   // frame g's (channel, frame) from the lanes that hold it
-                const long long cg = __shfl_sync(0xffffffffu, myc, g * Q);
-                const long long fg = __shfl_sync(0xffffffffu, myf, g * Q);
-                if (__shfl_sync(0xffffffffu, (int)myok, g * Q))
-                    write_rows(s_col + g * (M + 1), out + cg * out_stride_c + fg * out_stride_f, scr, lane, 32);
+            for (int m = 0; m < 16; m++) {
+                const float2 z = v[brev5(m)];
+                const float2 other = v[brev5(31 - m)];
+                float2 zp;
+                zp.x = __shfl_sync(0xffffffffu, other.x, src_lane);
+                zp.y = __shfl_sync(0xffffffffu, other.y, src_lane);
+                if (k1 == 0) zp = (m == 0) ? v[0] : v[brev5(32 - m)];
+                const float2 E = make_float2(z.x + zp.x, z.y - zp.y);
+                const float2 O = make_float2(z.x - zp.x, z.y + zp.y);
+                const int k = k1 + Q * m;
+                const float2 T = cmul(O, s_post[k]);
+                const float2 X = cadd(E, T);
+                const float2 Y = csub(E, T);
+                const float p1 = fmaf(X.x, X.x, X.y * X.y);
+                const float p2 = fmaf(Y.x, Y.x, Y.y * Y.y);
+                if (myok) {
+                    o[k] = finish<MODE>(p1, scale);
+                    o[M - k] = finish<MODE>(p2, scale);
+                }
             }
-            __syncwarp();   // every lane is done with the columns before the tile is written again
+            if (k1 == 0 && myok) {
+                const float2 z = v[brev5(16)];   // bin M/2: X = conj(Z)
+                o[M / 2] = finish<MODE>(4.0f * fmaf(z.x, z.x, z.y * z.y), scale);
+            }
+            if constexpr (MODE == kModeScreen) {
+                __syncwarp();   // the warp's G columns are complete
+                const float *s_col = o - gsel * (M + 1);
+#pragma unroll
+                for (int g = 0; g < G; g++) {   // frame g's (channel, frame) from the lanes that hold it
+                    const long long cg = __shfl_sync(0xffffffffu, myc, g * Q);
+                    const long long fg = __shfl_sync(0xffffffffu, myf, g * Q);
+                    if (__shfl_sync(0xffffffffu, (int)myok, g * Q))
+                        write_rows(s_col + g * (M + 1), out + cg * out_stride_c + fg * out_stride_f, scr, lane, 32);
+                }
+                __syncwarp();   // every lane is done with the columns before the tile is written again
+            }
         }
     }
 }
@@ -557,17 +877,25 @@ stft_small_kernel(const float *__restrict__ x, long long x_stride, long long n_f
 // kModeScreen: each frame group's column goes to a buffer of its own after the tiles (the tiles are read
 // until the split step ends).  At R = 4 sixteen warps' tiles, tables and four such buffers exceed the
 // 227 KB a CTA may hold, so that instantiation runs twelve warps (three frame groups).
+// Smoothing outputs: one frame group per channel, its states after the tiles, each thread adding the bins
+// it splits (the same ones in every frame).  A group's states take 16 KB (R = 2) or 32 KB (R = 4) per
+// channel of the pair, so these run eight warps, and four (one group) at R = 4 in kModeSmoothDual.
 template <int R, int MODE>
-__host__ __device__ constexpr int large_warps() { return (MODE == kModeScreen && R == 4) ? 12 : 16; }
+__host__ __device__ constexpr int large_warps() {
+    if (smooth_nch(MODE)) return (R == 4 && MODE == kModeSmoothDual) ? 4 : 8;
+    return (MODE == kModeScreen && R == 4) ? 12 : 16;
+}
 struct HannA {
     float2 v[32];     // (0.5 cos(theta 64 R n1), 0.5 sin(theta 64 R n1))
 };
 template <int R, int MODE>
 constexpr size_t large_smem() {
-    // tw [1024] + comb [R-1][1024] + post [512 R + 1 -> even] + tiles (+ kModeScreen: the groups' columns)
+    // tw [1024] + comb [R-1][1024] + post [512 R + 1 -> even] + tiles (+ kModeScreen: the groups' columns;
+    // smoothing: the groups' states)
     constexpr int W = large_warps<R, MODE>();
     return sizeof(float2) * (1024 + 1024 * (R - 1) + 512 * R + 2 + (size_t)W * TILE) +
-           (MODE == kModeScreen ? sizeof(float) * (size_t)(W / R) * (1024 * R + 1) : 0);
+           (MODE == kModeScreen ? sizeof(float) * (size_t)(W / R) * (1024 * R + 1) : 0) +
+           (W / R) * smooth_slot_bytes<MODE>(1024 * R + 1, R);
 }
 
 __device__ __forceinline__ void group_barrier(int id, int nthreads) {
@@ -588,11 +916,11 @@ stft_large_kernel(const float *__restrict__ x, long long x_stride, long long n_f
                   const float2 *__restrict__ win2, const float4 *__restrict__ wlane,
                   const float2 *__restrict__ tw32, const float2 *__restrict__ comb,
                   const float2 *__restrict__ post, long long total_items,
-                  const __grid_constant__ HannA hann_a, const ScreenRows scr) {
+                  const __grid_constant__ HannA hann_a, const ScreenRows scr, const SmoothTicks sm) {
     // STAG: 8-byte shared accesses are served per half-warp; the 16/R elements a half-warp sends to
     // each of the R tiles must fall on different banks
     constexpr int LARGE_WARPS = large_warps<R, MODE>();
-    constexpr int M = 1024 * R, N = 2 * M, NG = LARGE_WARPS / R, GT = 32 * R, STAG = 16 / R;
+    constexpr int M = 1024 * R, N = 2 * M, NG = LARGE_WARPS / R, GT = 32 * R, STAG = 16 / R, NCH = smooth_nch(MODE);
     extern __shared__ float2 smem[];
     float2 *s_tw = smem;                          // [32][32] W_1024^(k1 t)
     float2 *s_comb = s_tw + 1024;                 // [R-1][1024] W_M^(w k0)
@@ -610,68 +938,90 @@ stft_large_kernel(const float *__restrict__ x, long long x_stride, long long n_f
 
     const long long groups_total = (long long)gridDim.x * NG;
     const long long gg = (long long)blockIdx.x * NG + grp;
-    const long long per = (total_items + groups_total - 1) / groups_total;
-    long long item = gg * per;
-    long long item_end = item + per;
-    if (item_end > total_items) item_end = total_items;
     const float scale = 1.0f / (4.0f * (float)N * (float)N);
-    long long c = (item < item_end) ? item / n_frames : 0;
-    long long f = item - c * n_frames;
     const float4 wb = wlane[w * 32 + lane];       // cos B (e = 0, 1), sin B (e = 0, 1)
     const float2 wcb = make_float2(wb.x, wb.y), wsb = make_float2(wb.z, wb.w);
     // (w[n], w[n+1]) of register blocks 0 and 31: z index R (32 n1 + lane) + w
     const float2 wfirst = __ldg(win2 + R * lane + w), wlast = __ldg(win2 + R * (32 * 31 + lane) + w);
 
     auto fetch = [&](long long cc, long long ff) {
-        const float2 *p2 = reinterpret_cast<const float2 *>(x + cc * x_stride + ff * hop);
+        const float2 *p2 = reinterpret_cast<const float2 *>(frame_at<MODE>(x, sm, x_stride, hop, cc, ff));
 #pragma unroll 8
         for (int e = gtid; e < M; e += GT) {
             const int ww = e % R, i = e / R;
             cp_async8(s_tiles + ww * TILE + ww * STAG + i, p2 + e);
         }
     };
-    if (item < item_end) fetch(c, f);
-    for (; item < item_end; item++) {
-        cp_async_commit();
-        cp_async_wait<0>();
-        group_barrier(1 + grp, GT);          // the whole frame has landed
-        float2 v[32];
+    // items [item, item_end), the first one frame f of channel c, nf frames (smoothing: items) per channel;
+    // s: the group's Smoother in the smoothing outputs
+    auto run = [&](long long item, long long item_end, long long c, long long f, long long nf, auto &s) {
+        if (item < item_end) fetch(c, f);
+        for (; item < item_end; item++) {
+            cp_async_commit();
+            cp_async_wait<0>();
+            group_barrier(1 + grp, GT);          // the whole frame has landed
+            float2 v[32];
 #pragma unroll
-        for (int n1 = 0; n1 < 32; n1++) v[n1] = s_x[w * STAG + 32 * n1 + lane];
-        __syncwarp();                        // inputs are in registers: the tile becomes the exchange buffer
+            for (int n1 = 0; n1 < 32; n1++) v[n1] = s_x[w * STAG + 32 * n1 + lane];
+            __syncwarp();                        // inputs are in registers: the tile becomes the exchange buffer
 #pragma unroll
-        for (int n1 = 0; n1 < 32; n1++) {
-            float2 wv;
-            if (n1 == 0) {
-                wv = wfirst;
-            } else if (n1 == 31) {
-                wv = wlast;
-            } else {
-                const float ca = hann_a.v[n1].x, sa = hann_a.v[n1].y;
-                wv = f2_fma(make_float2(-ca, -ca), wcb, make_float2(0.5f, 0.5f));
-                wv = f2_fma(make_float2(sa, sa), wsb, wv);
+            for (int n1 = 0; n1 < 32; n1++) {
+                float2 wv;
+                if (n1 == 0) {
+                    wv = wfirst;
+                } else if (n1 == 31) {
+                    wv = wlast;
+                } else {
+                    const float ca = hann_a.v[n1].x, sa = hann_a.v[n1].y;
+                    wv = f2_fma(make_float2(-ca, -ca), wcb, make_float2(0.5f, 0.5f));
+                    wv = f2_fma(make_float2(sa, sa), wsb, wv);
+                }
+                v[n1] = f2_mul(v[n1], wv);
             }
-            v[n1] = f2_mul(v[n1], wv);
-        }
-        dft32(v);
-        twiddle_transpose<32>(v, s_tw, s_x, lane);
-        dft32(v);   // v[r] = Z_w[lane + 32*brev5(r)]
+            dft32(v);
+            twiddle_transpose<32>(v, s_tw, s_x, lane);
+            dft32(v);   // v[r] = Z_w[lane + 32*brev5(r)]
 #pragma unroll
-        for (int r = 0; r < 32; r++) s_x[lane + 32 * brev5(r)] = v[r];   // natural order
-        group_barrier(1 + grp, GT);
+            for (int r = 0; r < 32; r++) s_x[lane + 32 * brev5(r)] = v[r];   // natural order
+            group_barrier(1 + grp, GT);
 
-        float *rows = out + c * out_stride_c + f * out_stride_f;
-        combine_split<R, MODE>(MODE == kModeScreen ? s_col : rows, s_tiles,
-                               [=](int w, int k0) { return s_comb[(w - 1) * 1024 + k0]; },
-                               [=](int kk) { return post_lookup(s_post, kk, M / 2); }, gtid, scale);
-        if (++f == n_frames) {
-            f = 0;
-            c++;
+            float *rows = out + c * out_stride_c + f * out_stride_f;
+            [[maybe_unused]] const long long myf = f;
+            auto add = [&](int k, float p) {
+                if constexpr (NCH > 0) s.add((int)(myf % NCH), k, p);
+            };
+            combine_split<R, MODE>(MODE == kModeScreen ? s_col : rows, add, s_tiles,
+                                   [=](int w, int k0) { return s_comb[(w - 1) * 1024 + k0]; },
+                                   [=](int kk) { return post_lookup(s_post, kk, M / 2); }, gtid, scale);
+            if (++f == nf) {
+                f = 0;
+                c++;
+            }
+            group_barrier(1 + grp, GT);          // every Z_w has been read: the tiles are free again
+            if (item + 1 < item_end) fetch(c, f);
+            // (the group's column is written again only after the next frame's first barrier)
+            if constexpr (MODE == kModeScreen) write_rows(s_col, rows, scr, gtid, GT);
+            if constexpr (NCH > 0) s.after(myf);
         }
-        group_barrier(1 + grp, GT);          // every Z_w has been read: the tiles are free again
-        if (item + 1 < item_end) fetch(c, f);
-        // (the group's column is written again only after the next frame's first barrier)
-        if constexpr (MODE == kModeScreen) write_rows(s_col, rows, scr, gtid, GT);
+    };
+    if constexpr (NCH > 0) {
+        unsigned char *slot = reinterpret_cast<unsigned char *>(s_tiles_all + (size_t)LARGE_WARPS * TILE) +
+                              grp * smooth_slot_bytes<MODE>(M + 1, R);
+        auto s = slot_smoother<NCH>(sm, slot, M + 1, gtid, GT, [grp] { group_barrier(1 + grp, GT); });
+        const long long nv = NCH * n_frames;
+        for (long long ch = gg; ch < sm.n_channels; ch += groups_total) {
+            s.begin(ch);
+            run(ch * nv, (ch + 1) * nv, ch, 0, nv, s);
+            s.end();
+        }
+    } else {
+        const long long per = (total_items + groups_total - 1) / groups_total;
+        const long long item = gg * per;
+        long long item_end = item + per;
+        if (item_end > total_items) item_end = total_items;
+        const long long c = (item < item_end) ? item / n_frames : 0;
+        int none = 0;
+        run(item, item_end, c, item - c * n_frames, n_frames, none);
     }
 }
 
@@ -703,6 +1053,7 @@ __device__ __forceinline__ void stockham_radix4(const float2 *__restrict__ in,
 }
 
 // kModeScreen: the column goes to the buffer the FFT does not end in, and the frame's rows to out.
+// Smoothing outputs: one CTA per channel, its states after the two buffers.
 template <int MODE>
 __global__ void stft_generic_kernel(const float *__restrict__ x, long long x_stride,
                                     long long n_frames, int hop, float *__restrict__ out,
@@ -710,77 +1061,112 @@ __global__ void stft_generic_kernel(const float *__restrict__ x, long long x_str
                                     const float *__restrict__ win,
                                     const float2 *__restrict__ tw,
                                     const float2 *__restrict__ post, int n_fft, int log2m,
-                                    const ScreenRows scr) {
+                                    const ScreenRows scr, const SmoothTicks sm) {
     extern __shared__ float2 smem[];
+    constexpr int NCH = smooth_nch(MODE);
     const int M = n_fft >> 1;
     float2 *buf0 = smem;
     float2 *buf1 = smem + M;
     const int tid = threadIdx.x, nthreads = blockDim.x;
-    const long long item = blockIdx.x;
-    const long long c = item / n_frames;
-    const long long f = item - c * n_frames;
-    const float *p = x + c * x_stride + f * hop;
-
-    for (int n = tid; n < M; n += nthreads)
-        buf0[n] = make_float2(__ldg(p + 2 * n) * __ldg(win + 2 * n),
-                              __ldg(p + 2 * n + 1) * __ldg(win + 2 * n + 1));
-    __syncthreads();
-
-    float2 *in = buf0, *ob = buf1;
-    int Ns = 1;
-    if (log2m & 1) {   // one radix-2 pass first (no twiddles at Ns = 1)
-        const int halfm = M >> 1;
-        for (int j = tid; j < halfm; j += nthreads) {
-            const float2 a = in[j], b = in[j + halfm];
-            ob[2 * j] = cadd(a, b);
-            ob[2 * j + 1] = csub(a, b);
-        }
-        __syncthreads();
-        float2 *t = in; in = ob; ob = t;
-        Ns = 2;
-    }
-    for (; Ns < M; Ns <<= 2) {
-        stockham_radix4(in, ob, tw, M, Ns, tid, nthreads);
-        __syncthreads();
-        float2 *t = in; in = ob; ob = t;
-    }
-    // `in` now holds Z[0..M)
     const float scale = 1.0f / (4.0f * (float)n_fft * (float)n_fft);
-    float *o = MODE == kModeScreen ? reinterpret_cast<float *>(ob) : out + c * out_stride_c + f * out_stride_f;
-    for (int k = tid; k <= M / 2; k += nthreads) {
-        const float2 z = in[k];
-        const float2 zp = in[(M - k) & (M - 1)];
-        const float2 E = make_float2(z.x + zp.x, z.y - zp.y);
-        const float2 O = make_float2(z.x - zp.x, z.y + zp.y);
-        const float2 T = cmul(O, post[k]);
-        const float2 X = cadd(E, T);
-        const float2 Y = csub(E, T);
-        o[k] = finish<MODE>(fmaf(X.x, X.x, X.y * X.y), scale);
-        o[M - k] = finish<MODE>(fmaf(Y.x, Y.x, Y.y * Y.y), scale);
-    }
-    if constexpr (MODE == kModeScreen) {
+
+    // the frame at p: `in` then holds Z[0..M) and `ob` is free
+    auto transform = [&](const float *p, float2 *&in, float2 *&ob) {
+        for (int n = tid; n < M; n += nthreads)
+            buf0[n] = make_float2(__ldg(p + 2 * n) * __ldg(win + 2 * n),
+                                  __ldg(p + 2 * n + 1) * __ldg(win + 2 * n + 1));
         __syncthreads();
-        write_rows(o, out + c * out_stride_c + f * out_stride_f, scr, tid, nthreads);
+
+        in = buf0;
+        ob = buf1;
+        int Ns = 1;
+        if (log2m & 1) {   // one radix-2 pass first (no twiddles at Ns = 1)
+            const int halfm = M >> 1;
+            for (int j = tid; j < halfm; j += nthreads) {
+                const float2 a = in[j], b = in[j + halfm];
+                ob[2 * j] = cadd(a, b);
+                ob[2 * j + 1] = csub(a, b);
+            }
+            __syncthreads();
+            float2 *t = in; in = ob; ob = t;
+            Ns = 2;
+        }
+        for (; Ns < M; Ns <<= 2) {
+            stockham_radix4(in, ob, tw, M, Ns, tid, nthreads);
+            __syncthreads();
+            float2 *t = in; in = ob; ob = t;
+        }
+    };
+    // the split step: bins k and M - k to store(k, |X|^2, |Y|^2), k <= M/2
+    auto split = [&](const float2 *in, auto store) {
+        for (int k = tid; k <= M / 2; k += nthreads) {
+            const float2 z = in[k];
+            const float2 zp = in[(M - k) & (M - 1)];
+            const float2 E = make_float2(z.x + zp.x, z.y - zp.y);
+            const float2 O = make_float2(z.x - zp.x, z.y + zp.y);
+            const float2 T = cmul(O, post[k]);
+            const float2 X = cadd(E, T);
+            const float2 Y = csub(E, T);
+            store(k, fmaf(X.x, X.x, X.y * X.y), fmaf(Y.x, Y.x, Y.y * Y.y));
+        }
+    };
+    if constexpr (NCH > 0) {
+        auto s = slot_smoother<NCH>(sm, smem + 2 * M, M + 1, tid, nthreads, [] { __syncthreads(); });
+        const long long c = blockIdx.x;
+        s.begin(c);
+        for (long long i = 0; i < NCH * n_frames; i++) {
+            float2 *in, *ob;
+            transform(frame_at<MODE>(x, sm, x_stride, hop, c, i), in, ob);
+            const int j = (int)(i % NCH);
+            split(in, [&](int k, float pX, float pY) {   // bin M/2 is split twice: its second value counts
+                if (k != M - k) s.add(j, k, finish<MODE>(pX, scale));
+                s.add(j, M - k, finish<MODE>(pY, scale));
+            });
+            __syncthreads();   // `in` is read before the next frame is written
+            s.after(i);
+        }
+        s.end();
+    } else {
+        const long long item = blockIdx.x;
+        const long long c = item / n_frames;
+        const long long f = item - c * n_frames;
+        float2 *in, *ob;
+        transform(x + c * x_stride + f * hop, in, ob);
+        float *o = MODE == kModeScreen ? reinterpret_cast<float *>(ob) : out + c * out_stride_c + f * out_stride_f;
+        split(in, [&](int k, float pX, float pY) {
+            o[k] = finish<MODE>(pX, scale);
+            o[M - k] = finish<MODE>(pY, scale);
+        });
+        if constexpr (MODE == kModeScreen) {
+            __syncthreads();
+            write_rows(o, out + c * out_stride_c + f * out_stride_f, scr, tid, nthreads);
+        }
     }
 }
 
-// the tw table and the R tiles (+ kModeScreen: the frame's column)
+// the tw table and the R tiles (+ kModeScreen: the frame's column; smoothing: the channel's states)
 template <int R, int MODE>
 constexpr size_t multi_smem() {
-    return sizeof(float2) * (1024 + (size_t)R * TILE) + (MODE == kModeScreen ? sizeof(float) * (1024 * R + 1) : 0);
+    return sizeof(float2) * (1024 + (size_t)R * TILE) + (MODE == kModeScreen ? sizeof(float) * (1024 * R + 1) : 0) +
+           smooth_slot_bytes<MODE>(1024 * R + 1, R);
 }
-// kModeScreen: no more CTAs per SM than its 228 KB hold (1 KB of each CTA's is reserved)
+// kModeScreen and smoothing: no more CTAs per SM than its 228 KB hold (1 KB of each CTA's is reserved)
 template <int R, int MODE>
 constexpr long long multi_ctas_per_sm() {
     constexpr long long n = R == 8 ? 2 : (R == 4 ? 4 : 8);
-    return MODE == kModeScreen ? std::min<long long>(n, (228 * 1024) / (multi_smem<R, MODE>() + 1024)) : n;
+    return MODE == kModeScreen || smooth_nch(MODE)
+               ? std::min<long long>(n, (228 * 1024) / (multi_smem<R, MODE>() + 1024))
+               : n;
 }
 
-// calls launch with the output (FRT_STFT_POWER, FRT_STFT_LOGPOWER or kModeScreen) as a compile-time constant
+// calls launch with the output (FRT_STFT_POWER, FRT_STFT_LOGPOWER, kModeScreen, kModeSmooth or
+// kModeSmoothDual) as a compile-time constant
 template <class F>
 int with_mode(int mode, F &&launch) {
     if (mode == FRT_STFT_POWER) return launch(std::integral_constant<int, FRT_STFT_POWER>());
     if (mode == FRT_STFT_LOGPOWER) return launch(std::integral_constant<int, FRT_STFT_LOGPOWER>());
+    if (mode == kModeSmooth) return launch(std::integral_constant<int, kModeSmooth>());
+    if (mode == kModeSmoothDual) return launch(std::integral_constant<int, kModeSmoothDual>());
     return launch(std::integral_constant<int, kModeScreen>());
 }
 
@@ -790,8 +1176,9 @@ int frame_alignment(const float *x, long long x_stride, int hop) {
     return (((uintptr_t)x & 7) == 0) && ((x_stride & 1) == 0) && ((hop & 1) == 0);
 }
 
-// one frt_stft_process / frt_stft_screen_rows call: total = channels x frames items, frame f of
-// channel c at x + c x_stride + f hop, its spectrum (or, kModeScreen, its rows) at out + c osc + f osf
+// one frt_stft_process / frt_stft_screen_rows / frt_spectrum_frames(_dual) call: total = channels x
+// frames items, frame f of channel c at x + c x_stride + f hop, its spectrum (or, kModeScreen, its rows)
+// at out + c osc + f osf
 struct Frames {
     const float *x;
     long long x_stride, n_frames;
@@ -801,20 +1188,21 @@ struct Frames {
     int mode, align;   // align: frame_alignment of the frames
     cudaStream_t st;
     ScreenRows scr;   // kModeScreen
+    SmoothTicks sm;   // smoothing
 };
 
 template <int Q, bool TMA = false>
 int launch_small(frt_ctx *h, const StftPlan &pl, const Frames &a) {
-    constexpr int G = 32 / Q, WARPS = small_warps<Q>();
-    const long long max_blocks = (long long)small_ctas_per_sm<Q>() * h->sm_count;
-    long long blocks = ((a.total + G - 1) / G + WARPS - 1) / WARPS;
-    if (blocks > max_blocks) blocks = max_blocks;
     return with_mode(a.mode, [&](auto m) {
-        constexpr int MODE = decltype(m)::value;
+        constexpr int MODE = decltype(m)::value, G = 32 / Q, WARPS = small_warps<Q, MODE>();
+        const long long max_blocks = (long long)small_ctas_per_sm<Q, MODE>() * h->sm_count;
+        const long long slots = smooth_nch(MODE) ? a.sm.n_channels : (a.total + G - 1) / G;
+        long long blocks = (slots + WARPS - 1) / WARPS;
+        if (blocks > max_blocks) blocks = max_blocks;
         return frt_launch(h, stft_small_kernel<Q, MODE, TMA>, (unsigned)blocks, WARPS * 32, small_smem<Q, MODE, TMA>(),
                           a.st, a.x, a.x_stride, a.n_frames, a.hop, a.out, a.osc, a.osf,
                           reinterpret_cast<const float2 *>(pl.win_dev.get()), pl.tw_dev.get(), pl.post_dev.get(),
-                          a.total, a.align >= 1, a.scr);
+                          a.total, a.align >= 1, a.scr, a.sm);
     });
 }
 template <int R>
@@ -827,24 +1215,26 @@ int launch_large(frt_ctx *h, const StftPlan &pl, const Frames &a) {
     }
     return with_mode(a.mode, [&](auto m) {
         constexpr int MODE = decltype(m)::value, NG = large_warps<R, MODE>() / R;
-        long long blocks = (a.total + NG - 1) / NG;
+        const long long slots = smooth_nch(MODE) ? a.sm.n_channels : a.total;
+        long long blocks = (slots + NG - 1) / NG;
         if (blocks > h->sm_count) blocks = h->sm_count;
         return frt_launch(h, stft_large_kernel<R, MODE>, (unsigned)blocks, large_warps<R, MODE>() * 32,
                           large_smem<R, MODE>(), a.st, a.x, a.x_stride, a.n_frames, a.hop, a.out, a.osc, a.osf,
                           reinterpret_cast<const float2 *>(pl.win_dev.get()), pl.wlane_dev.get(), pl.tw_dev.get(),
-                          pl.comb_dev.get(), pl.post_dev.get(), a.total, ha, a.scr);
+                          pl.comb_dev.get(), pl.post_dev.get(), a.total, ha, a.scr, a.sm);
     });
 }
 template <int R>
 int launch_multi(frt_ctx *h, const StftPlan &pl, const Frames &a) {
     return with_mode(a.mode, [&](auto m) {
         constexpr int MODE = decltype(m)::value;
+        const long long slots = smooth_nch(MODE) ? a.sm.n_channels : a.total;
         long long blocks = (long long)h->sm_count * multi_ctas_per_sm<R, MODE>();
-        if (blocks > a.total) blocks = a.total;
+        if (blocks > slots) blocks = slots;
         return frt_launch(h, stft_multi_kernel<R, MODE>, (unsigned)blocks, 32 * R, multi_smem<R, MODE>(), a.st, a.x,
                           a.x_stride, a.n_frames, a.hop, a.out, a.osc, a.osf,
                           reinterpret_cast<const float2 *>(pl.win_dev.get()), pl.tw_dev.get(), pl.comb_dev.get(),
-                          pl.post_dev.get(), a.total, a.align >= 1, a.scr);
+                          pl.post_dev.get(), a.total, a.align >= 1, a.scr, a.sm);
     });
 }
 
@@ -972,9 +1362,12 @@ static int stft_dispatch(frt_ctx *h, const StftPlan &pl, const Frames &a) {
     if (threads < 32) threads = 32;
     if (threads > 512) threads = 512;
     return with_mode(a.mode, [&](auto m) {
-        return frt_launch(h, stft_generic_kernel<decltype(m)::value>, (unsigned)a.total, threads,
-                          sizeof(float2) * 2 * M, a.st, a.x, a.x_stride, a.n_frames, a.hop, a.out, a.osc, a.osf,
-                          pl.win_dev.get(), pl.tw_dev.get(), pl.post_dev.get(), N, ilog2(M), a.scr);
+        constexpr int MODE = decltype(m)::value;
+        const long long blocks = smooth_nch(MODE) ? a.sm.n_channels : a.total;   // smoothing: one per channel
+        return frt_launch(h, stft_generic_kernel<MODE>, (unsigned)blocks, threads,
+                          sizeof(float2) * 2 * M + smooth_slot_bytes<MODE>(M + 1, threads / 32), a.st, a.x,
+                          a.x_stride, a.n_frames, a.hop, a.out, a.osc, a.osf, pl.win_dev.get(), pl.tw_dev.get(),
+                          pl.post_dev.get(), N, ilog2(M), a.scr, a.sm);
     });
 }
 
@@ -995,7 +1388,7 @@ static int stft_call(frt_ctx *h, const char *fn, const float *x, int64_t x_strid
     FRT_CHECK_ARG(h, out_stride_f >= (mode == kModeScreen ? scr.height : pl.n_fft / 2 + 1),
                   "frame stride smaller than a frame's bins or screen rows");
     const Frames a{x, x_stride, n_frames, hop, out, out_stride_c, out_stride_f, (long long)n_channels * n_frames,
-                   mode, frame_alignment(x, x_stride, hop), (cudaStream_t)stream, scr};
+                   mode, frame_alignment(x, x_stride, hop), (cudaStream_t)stream, scr, SmoothTicks{}};
     return stft_dispatch(h, pl, a);
 }
 
@@ -1021,6 +1414,55 @@ extern "C" int frt_stft_screen_rows(frt_handle h, const float *x_dev, int64_t x_
     const ScreenRows scr{weight_dev, row_i0_dev, row_t_dev, spec_min, 1.0f / (spec_max - spec_min), height};
     return stft_call(h, "frt_stft_screen_rows", x_dev, x_stride, n_channels, n_frames, hop, rows_dev, rows_stride_c,
                      rows_stride_f, kModeScreen, scr, bad, row_i0_dev && row_t_dev, stream);
+}
+
+// frt_spectrum_frames and _dual (mode kModeSmooth / kModeSmoothDual; x2 and disp2 NULL in kModeSmooth): the
+// checks, nothing to do on empty input, and the launch of the plan's kernel family.
+static int spectrum_frames_call(frt_ctx *h, const char *fn, int mode, const float *x, const float *x2,
+                                int64_t x_stride, int n_channels, int64_t n_frames, int hop, const int *tick_end,
+                                int n_ticks, float alpha, float *disp, float *disp2, const float *weight, float *db,
+                                int64_t db_stride_c, int64_t db_stride_r, int *imax, int *ipitch, void *stream) {
+    if (!h->stft) return frt_fail(h, FRT_ESTATE, "%s: call frt_stft_plan first", fn);
+    const int nbins = h->stft->n_fft / 2 + 1;
+    const bool dual = mode == kModeSmoothDual;
+    FRT_CHECK_ARG(h, n_channels >= 0 && n_frames >= 0, "negative shape");
+    FRT_CHECK_ARG(h, hop >= 1, "hop must be >= 1");
+    FRT_CHECK_ARG(h, alpha > 0.f && alpha <= 1.f, "alpha must be in (0, 1]");
+    FRT_CHECK_ARG(h, n_ticks >= 0 && n_ticks <= n_frames && (n_ticks > 0 || n_frames == 0),
+                  "n_ticks must be in 1..n_frames");
+    if (n_channels == 0 || n_frames == 0) return FRT_OK;   // empty input: nothing to do
+    FRT_CHECK_ARG(h, x && tick_end && disp && imax && ipitch && (!dual || (x2 && disp2)), "NULL buffer");
+    FRT_CHECK_ARG(h, !db || (db_stride_r >= nbins && db_stride_c >= 0), "dB row stride smaller than a row's bins");
+    const SmoothTicks sm{x2,     tick_end, n_ticks, n_channels,  alpha,       {disp, disp2},
+                         weight, db,       db_stride_c, db_stride_r, imax,  ipitch};
+    int align = frame_alignment(x, x_stride, hop);
+    if (dual) align = std::min(align, frame_alignment(x2, x_stride, hop));
+    const Frames a{x,    x_stride, n_frames, hop, nullptr, 0, 0, (long long)n_channels * n_frames,
+                   mode, align,    (cudaStream_t)stream,   ScreenRows{}, sm};
+    return stft_dispatch(h, *h->stft, a);
+}
+
+extern "C" int frt_spectrum_frames(frt_handle h, const float *x_dev, int64_t x_stride, int n_channels,
+                                   int64_t n_frames, int hop, const int *tick_end_dev, int n_ticks, float alpha,
+                                   float *disp_dev, const float *weight_dev, float *db_dev, int64_t db_stride_c,
+                                   int64_t db_stride_r, int *imax_dev, int *ipitch_dev, void *stream) {
+    if (!h) return FRT_EINVAL;
+    DeviceGuard g(h->device);
+    return spectrum_frames_call(h, "frt_spectrum_frames", kModeSmooth, x_dev, nullptr, x_stride, n_channels, n_frames,
+                                hop, tick_end_dev, n_ticks, alpha, disp_dev, nullptr, weight_dev, db_dev, db_stride_c,
+                                db_stride_r, imax_dev, ipitch_dev, stream);
+}
+
+extern "C" int frt_spectrum_frames_dual(frt_handle h, const float *x1_dev, const float *x2_dev, int64_t x_stride,
+                                        int n_pairs, int64_t n_frames, int hop, const int *tick_end_dev, int n_ticks,
+                                        float alpha, float *disp1_dev, float *disp2_dev, float *db_dev,
+                                        int64_t db_stride_c, int64_t db_stride_r, int *imax_dev, int *ipitch_dev,
+                                        void *stream) {
+    if (!h) return FRT_EINVAL;
+    DeviceGuard g(h->device);
+    return spectrum_frames_call(h, "frt_spectrum_frames_dual", kModeSmoothDual, x1_dev, x2_dev, x_stride, n_pairs,
+                                n_frames, hop, tick_end_dev, n_ticks, alpha, disp1_dev, disp2_dev, nullptr, db_dev,
+                                db_stride_c, db_stride_r, imax_dev, ipitch_dev, stream);
 }
 
 extern "C" int frt_stft_process_host(frt_handle h, const float *x_host, int64_t x_stride,

@@ -16,20 +16,26 @@ import numpy as np
 
 from . import _lib
 from .audioproc import FRAMES_PER_BUFFER, SAMPLING_RATE, audioproc, frame_count
+from .stream import StreamFramer
 
 DEFAULT_FFT_SIZE = 8192        # friture/spectrum_settings.py:27 (2**7 * 32 ... the widget default)
 DEFAULT_RESPONSE_TIME = 0.025  # friture/spectrum_settings.py
 OVERLAP = 0.75                 # friture/spectrum.py:66
 MAX_FRAMES_PER_TICK = 8192     # the frames one tick may smooth (the reference's 8192-tap kernel)
+STREAM_HISTORY = 16384         # samples handle_new_data keeps before old_index: the largest FFT size
 
 
 @dataclass
 class SpectrumTicks:
-    """``SpectrumAnalyzer.process_ticks``'s outputs, one row per tick: ``db`` CUDA float32
-    [C, R, bins] (None when not requested), ``fmax_hz`` and ``fpitch_hz`` host float64 [R, C]."""
+    """``SpectrumAnalyzer.process_ticks``'s and ``handle_new_data``'s outputs, one row per tick: ``db``
+    CUDA float32 [C, R, bins] (None when not requested), ``fmax_hz`` and ``fpitch_hz`` host float64
+    [R, C].  From ``handle_new_data`` also ``tick`` [R], which buffer of the call each row belongs to,
+    and ``n_frames`` [R], the frames it smoothed (None from ``process_ticks``)."""
     db: object
     fmax_hz: np.ndarray
     fpitch_hz: np.ndarray
+    tick: np.ndarray = None
+    n_frames: np.ndarray = None
 
 
 class SpectrumAnalyzer:
@@ -44,6 +50,10 @@ class SpectrumAnalyzer:
         self._disp = None
         self._disp2 = None
         self._w_dev = None
+        self._framer = None      # handle_new_data's stream, created by its first call
+        self._pairs = None       # whether that stream is [C, 2, n]
+        self.minfreq = 20.       # friture/spectrum_settings.py defaults
+        self.maxfreq = SAMPLING_RATE / 2
         self.setfftsize(fft_size)
 
     # -- the widget's setters ---------------------------------------------------------------
@@ -56,6 +66,8 @@ class SpectrumAnalyzer:
         self.setweighting(self.weighting)
         self._disp = None                                            # update_display_buffers, :224-226
         self._disp2 = None
+        if self._framer is not None:                                 # old_index is kept
+            self._framer.set_geometry(self.fft_size, self.hop)
 
     def setresponsetime(self, response_time):
         # spectrum.py:196-218: the newest n = T*fs/hop frames carry 65 % of the weight
@@ -74,6 +86,25 @@ class SpectrumAnalyzer:
     def setdualchannels(self, dual_enabled):
         """spectrum.py:286-293: changes the mode only; both smoothed states are kept."""
         self.dual_channels = bool(dual_enabled)
+
+    def setminfreq(self, minfreq):
+        self.setMinMaxFreq(minfreq, self.maxfreq)
+
+    def setmaxfreq(self, maxfreq):
+        self.setMinMaxFreq(self.minfreq, maxfreq)
+
+    def setMinMaxFreq(self, minfreq, maxfreq):
+        """spectrum.py:228-249: restarts both smoothed states.  The frequency axis stays: the reference's
+        audioproc.set_maxfreq only rebuilds it when the FFT size changes (audioproc.py:83-96)."""
+        self.minfreq = minfreq
+        self.maxfreq = maxfreq
+        self._disp = None                                            # update_display_buffers
+        self._disp2 = None
+
+    @property
+    def old_index(self):
+        """The widget's old_index: where the next frame of ``handle_new_data``'s stream ends."""
+        return self._framer.old_index if self._framer is not None else 0
 
     # -- one tick ----------------------------------------------------------------------------
     def process(self, x, stream=None):
@@ -191,6 +222,108 @@ class SpectrumAnalyzer:
                             self._disp2.mul_(decay)
             _, fmax, fpitch = self._indices_to_hz(None, imax, ipitch)
             return SpectrumTicks(db, fmax, fpitch)
+
+    # -- the widget's stream ----------------------------------------------------------------------
+    def handle_new_data(self, chunk, buffer=None, want_db=True, stream=None):
+        """``Spectrum_Widget.handle_new_data`` (friture/spectrum.py:125-184) over a stream pushed in
+        chunks: CUDA float32 [C, n], or [C, 2, n] with row 0 the reference and row 1 the measurement;
+        the first chunk's shape fixes the stream's.  Frames of ``fft_size`` samples end at
+        ``old_index``, which then advances by the hop (zeros before the stream starts).  ``buffer=None``:
+        the chunk is one widget tick; ``buffer=b``: it is n/b ticks of b samples each, the same bits as
+        n/b calls.  Returns a ``SpectrumTicks`` with one row per tick that had frames (the widget draws
+        nothing on the others), ``tick`` and ``n_frames`` saying which and how many.  Each frame's power
+        column goes straight into the smoothing on chip (``frt_spectrum_frames``); the rows, indices
+        and states are the same bits as ``process`` on the frames each tick cut.  Refusals happen
+        before the stream or the states change."""
+        import torch
+        _lib.check_tensor(self.proc, chunk, "chunk")
+        if chunk.dim() not in (2, 3) or (chunk.dim() == 3 and chunk.shape[1] != 2):
+            raise ValueError("chunk must be [C, n] or [C, 2, n], got %s" % (tuple(chunk.shape),))
+        if chunk.shape[0] != self.n_channels:
+            raise ValueError("chunk must have %d channels" % self.n_channels)
+        pairs = chunk.dim() == 3
+        if self._pairs is not None and pairs != self._pairs:
+            raise ValueError("the stream is %s; this chunk is not" % ("[C, 2, n]" if self._pairs else "[C, n]"))
+        ends, ticks = self.stream_ticks(chunk.shape[-1], buffer)
+        C = self.n_channels
+        rows_in = 2 * C if pairs else C
+        x = chunk.reshape(rows_in, chunk.shape[-1])
+        dual = pairs and self.dual_channels
+        nb = self.fft_size // 2 + 1
+        dev = chunk.device
+        with _lib.call_stream(dev, stream) as sp:
+            if self._framer is None:
+                self._framer = StreamFramer(rows_in, self.fft_size, self.hop, dev, capacity=2 * STREAM_HISTORY,
+                                            history=STREAM_HISTORY)
+                self._pairs = pairs
+            fr = self._framer
+            fr.push(x)
+            view, F = fr.take()
+            R = len(ends)
+            db = torch.empty((C, R, nb), dtype=torch.float32, device=dev) if want_db else None
+            imax = torch.empty((R, C), dtype=torch.int32, device=dev)
+            ipitch = torch.empty((R, C), dtype=torch.int32, device=dev)
+            if F:
+                if self._disp is None:
+                    self._disp = torch.zeros((C, nb), dtype=torch.float32, device=dev)
+                if dual and self._disp2 is None:
+                    self._disp2 = torch.zeros((C, nb), dtype=torch.float32, device=dev)
+                if not dual and self._w_dev is None:
+                    self._w_dev = torch.from_numpy(np.ascontiguousarray(self.w, dtype=np.float32)).to(dev)
+                # the tick ends go up from pinned memory without waiting for the stream
+                ends_host = torch.from_numpy(ends.astype(np.int32))
+                if dev.type == "cuda":
+                    ends_host = ends_host.pin_memory()
+                ends_dev = ends_host.to(dev, non_blocking=True)
+                h = self.proc.handle
+                h.call("frt_stft_plan", int(self.fft_size))
+                pitch = int(view.stride(0))
+                db_strides = (int(R * nb), int(nb))
+                if dual:
+                    p1 = view.data_ptr()
+                    h.call("frt_spectrum_frames_dual", _lib._ptr(p1), _lib._ptr(p1 + 4 * pitch), 2 * pitch, C,
+                           int(F), int(self.hop), _lib._ptr(ends_dev), int(R), c_float(self.alpha),
+                           _lib._ptr(self._disp), _lib._ptr(self._disp2), _lib._ptr(db), *db_strides,
+                           _lib._ptr(imax), _lib._ptr(ipitch), sp)
+                else:
+                    # [C, 2, n]: the reference rows only
+                    h.call("frt_spectrum_frames", _lib._ptr(view), 2 * pitch if pairs else pitch, C, int(F),
+                           int(self.hop), _lib._ptr(ends_dev), int(R), c_float(self.alpha),
+                           _lib._ptr(self._disp), _lib._ptr(self._w_dev) if self.weighting else None,
+                           _lib._ptr(db), *db_strides, _lib._ptr(imax), _lib._ptr(ipitch), sp)
+                    if self._disp2 is not None:
+                        # process's decay of the unfilled second state, once per tick
+                        for nf in np.diff(ends, prepend=0):
+                            self._disp2.mul_((1. - self.alpha) ** int(nf))
+            _, fmax, fpitch = self._indices_to_hz(None, imax, ipitch)
+            return SpectrumTicks(db, fmax, fpitch, ticks, np.diff(ends, prepend=0))
+
+    def stream_ticks(self, n, buffer=None):
+        """(ends, ticks) of a ``handle_new_data`` call of n samples per row: the frame index at which
+        each tick with frames ends (counted from the call's first frame) and which buffer of the call
+        it is, from the widget's framing (friture/spectrum.py:128-155); nothing changes.  Raises
+        FrtValueError for a buffer that does not divide n or a tick of more than 8192 frames."""
+        n = int(n)
+        if buffer is not None and (isinstance(buffer, (bool, np.bool_)) or
+                                   not isinstance(buffer, (int, np.integer)) or buffer < 1):
+            raise _lib.FrtValueError(_lib.FRT_EINVAL, "buffer must be a positive integer, got %r" % (buffer,))
+        b = n if buffer is None else int(buffer)
+        if n == 0:
+            return np.zeros(0, np.int64), np.zeros(0, np.int64)
+        if n % b:
+            raise _lib.FrtValueError(_lib.FRT_EINVAL, "%d samples are not a whole number of %d-sample buffers"
+                                     % (n, b))
+        offset = self._framer.offset if self._framer is not None else 0
+        # old_index advances by whole hops while offset - old_index >= hop, so after buffer t the frames
+        # cut so far are floor((offset_t - old_index) / hop)
+        avail = offset + b * np.arange(1, n // b + 1, dtype=np.int64) - self.old_index
+        cum = np.maximum(avail, 0) // self.hop
+        per = np.diff(cum, prepend=0)
+        if per.max() > MAX_FRAMES_PER_TICK:
+            raise _lib.FrtValueError(_lib.FRT_EINVAL, "a tick of %d frames exceeds the reference's %d-tap kernel"
+                                     % (per.max(), MAX_FRAMES_PER_TICK))
+        ticks = np.flatnonzero(per)
+        return cum[ticks], ticks
 
     def _indices_to_hz(self, db, imax, ipitch):
         # on the call's stream, which is current: the reads wait for the kernel that writes them

@@ -347,6 +347,39 @@ int frt_spectrum_reduce_dual_ticks(frt_handle h, const float *power1_dev, const 
                                    float *disp1_dev, float *disp2_dev, float *db_dev,
                                    int *fmax_idx_dev, int *pitch_idx_dev, void *stream);
 
+/* The spectrum widget's ticks straight from the frames (friture/spectrum.py:125-184): frame f of
+ * channel c, x_dev[c*x_stride + f*hop .. + n_fft) with the frt_stft_plan'ed size, is transformed to its
+ * FRT_STFT_POWER column, which stays on chip and goes straight into the smoothing of
+ * frt_spectrum_reduce; a channel's frames are smoothed in order.  Tick r ends at frame
+ * tick_end_dev[r] (exclusive): tick_end_dev is int32 [n_ticks] on the device, strictly ascending,
+ * tick_end_dev[n_ticks-1] == n_frames, at most 8192 frames per tick (the reference's 8192-tap kernel).
+ * The library does not read it on the host: an array that breaks these rules gives rows that mean
+ * nothing, not a fault.  At each tick's end the state is rounded to float32 and the tick's outputs
+ * are written:
+ *   db_dev[c*db_stride_c + r*db_stride_r + k] = 10*log10(sp + 1e-30) + weight[k] (db_dev may be NULL),
+ *   imax_dev[r*C + c] its first arg-max, ipitch_dev[r*C + c] the harmonic-product arg-max.
+ * Rows, indices and disp_dev afterwards are the same bits as frt_stft_process(FRT_STFT_POWER) on the
+ * same frames followed by frt_spectrum_reduce one tick at a time.  disp_dev [C][n_fft/2+1] is read
+ * once and written once; weight_dev [n_fft/2+1] dB or NULL.  Needs hop >= 1, alpha in (0, 1],
+ * 1 <= n_ticks <= n_frames and, with db_dev, db_stride_r >= n_fft/2+1; n_channels == 0 or
+ * n_frames == 0 is a no-op.  No workspace.                                                        */
+int frt_spectrum_frames(frt_handle h, const float *x_dev, int64_t x_stride, int n_channels,
+                        int64_t n_frames, int hop, const int *tick_end_dev, int n_ticks, float alpha,
+                        float *disp_dev, const float *weight_dev, float *db_dev, int64_t db_stride_c,
+                        int64_t db_stride_r, int *imax_dev, int *ipitch_dev, void *stream);
+
+/* frt_spectrum_frames in the dual-channel measurement mode (friture/spectrum.py:125-184 with
+ * dual_channels set): pair p's reference frames start at x1_dev + p*x_stride + f*hop, its
+ * measurement frames at x2_dev + p*x_stride + f*hop; both are smoothed (disp1_dev, disp2_dev
+ * [P][n_fft/2+1]), the dB row is the transfer function of frt_spectrum_reduce_dual and the pitch
+ * comes from the reference.  The same bits as frt_stft_process(FRT_STFT_POWER) on both rows followed
+ * by frt_spectrum_reduce_dual one tick at a time.  Checks as frt_spectrum_frames.                  */
+int frt_spectrum_frames_dual(frt_handle h, const float *x1_dev, const float *x2_dev, int64_t x_stride,
+                             int n_pairs, int64_t n_frames, int hop, const int *tick_end_dev,
+                             int n_ticks, float alpha, float *disp1_dev, float *disp2_dev,
+                             float *db_dev, int64_t db_stride_c, int64_t db_stride_r, int *imax_dev,
+                             int *ipitch_dev, void *stream);
+
 /* ---------------------------------------------------------------- plotted curves and peak hold
  * The last numeric step of the spectrum and octave widgets: SpectrumPlotWidget.setdata and
  * compute_peaks (friture/spectrumPlotWidget.py:122-200), HistPlot.setdata and compute_peaks
