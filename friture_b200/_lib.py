@@ -300,8 +300,40 @@ def device_rows(owner, x, name):
     return x, _row_stride(x.shape, x.stride(0))
 
 
-def host_rows(x):
-    """Host twin of ``device_rows`` for a float32 NumPy array or CPU tensor [C, T] or [T]."""
+def _host_float32(x):
+    """True for a float32 NumPy array or CPU torch tensor."""
+    import numpy as np
+    if isinstance(x, np.ndarray):
+        return x.dtype == np.float32
+    import torch
+    return isinstance(x, torch.Tensor) and x.dtype == torch.float32 and x.device.type == "cpu"
+
+def _elem_strides(x):
+    return tuple(x.stride()) if hasattr(x, "data_ptr") else tuple(s // 4 for s in x.strides)
+
+
+def host_rows(x, name="x"):
+    """Host twin of ``device_rows``: ``x`` as [C, T] and its row stride in floats, once it is checked
+    to be a float32 NumPy array or CPU tensor [C, T] or [T], contiguous along time.  The library
+    reads it at that stride as float32, so any other layout would be read as different samples."""
+    if not _host_float32(x):
+        raise ValueError("%s must be a float32 NumPy array or CPU tensor" % name)
     if x.ndim == 1:
         x = x[None, :]
-    return x, _row_stride(x.shape, x.stride(0) if hasattr(x, "data_ptr") else x.strides[0] // 4)
+    if x.ndim != 2:
+        raise ValueError("%s must be [C, T], contiguous along time" % name)
+    if not hasattr(x, "data_ptr") and any(s % 4 for s in x.strides):
+        raise ValueError("%s must be [C, T], contiguous along time" % name)
+    s0, s1 = _elem_strides(x)
+    if (x.shape[1] > 1 and s1 != 1) or (x.shape[0] > 1 and s0 < x.shape[1]):
+        raise ValueError("%s must be [C, T], contiguous along time" % name)
+    return x, _row_stride(x.shape, s0)
+
+
+def check_host_out(out, shape, name):
+    """Raise ValueError unless ``out`` is a C-contiguous float32 NumPy array or CPU tensor of exactly
+    ``shape``: the library writes it densely at the pitch that shape implies."""
+    if (not _host_float32(out) or tuple(out.shape) != tuple(shape)
+            or not (out.is_contiguous() if hasattr(out, "data_ptr") else out.flags.c_contiguous)):
+        raise ValueError("%s must be a contiguous float32 NumPy array or CPU tensor of shape %s"
+                         % (name, tuple(shape)))

@@ -22,6 +22,16 @@ from .audioproc import audioproc, frame_count
 from .octavefilters import Octave_Filters
 
 
+def bank_block_ok(block, n_octaves):
+    """Whether the filterbank kernels can run blocks of ``block`` samples with ``n_octaves`` octaves
+    (csrc/bank.cu, frt_bank_check_block): a multiple of 256 samples, and the longest of the 1024, 512
+    and 256-sample tiles that divides it still even at the last of the halving stages."""
+    if block <= 0 or block % 256:
+        return False
+    tile = next(t for t in (1024, 512, 256) if block % t == 0)
+    return (tile >> (n_octaves - 1)) >= 1
+
+
 class ChannelAnalyzer:
     def __init__(self, n_channels, fft_size=2048, hop=1024, bandsperoctave=3, n_octaves=10,
                  response_time=1.0, weighting=None, device=None):
@@ -30,6 +40,10 @@ class ChannelAnalyzer:
         self.handle = Handle(self.device.index)
         self.n_channels = int(n_channels)
         self.fft_size, self.hop = int(fft_size), int(hop)
+        if not bank_block_ok(self.hop, n_octaves):
+            raise ValueError("hop %d is not a filterbank block for %d octaves: it must be a multiple of 256 "
+                             "samples whose longest tile of 1024, 512 or 256 that divides it holds %d samples"
+                             % (self.hop, n_octaves, 1 << (n_octaves - 1)))
         self.nbins = self.fft_size // 2 + 1
         self.proc = audioproc(self.handle)
         self.proc.set_fftsize(self.fft_size)
@@ -71,8 +85,13 @@ class ChannelAnalyzer:
         F, B = self.frames(T), self.blocks(T)
         if spec is None:
             spec = torch.empty((C, F, self.nbins), dtype=torch.float32, device=x.device)
+        elif (not isinstance(spec, torch.Tensor) or spec.device != x.device or spec.dtype != torch.float32
+              or tuple(spec.shape) != (C, F, self.nbins) or not spec.is_contiguous()):
+            raise ValueError("spec must be a contiguous float32 tensor of shape %s on %s"
+                             % ((C, F, self.nbins), x.device))
         if bands is None:
             bands = torch.empty((C, B, self.nbands), dtype=torch.float32, device=x.device)
+        self._check_bands(x, bands)     # both outputs are checked before either kernel is queued
         if not overlap:
             self.proc.stft(x, hop=self.hop, log=True, out=spec)
             self._bank(x, bands)
@@ -89,10 +108,22 @@ class ChannelAnalyzer:
         cur.wait_stream(s_bank)
         return spec, bands
 
+    def _check_bands(self, x, bands):
+        """The bank writes channel c, block b of every channel at bands + c*stride(0) + b*nbands."""
+        x, _ = _lib.device_rows(self, x, "x")
+        C, T = x.shape
+        B = self.blocks(T)
+        _lib.check_tensor(self, bands, "bands")
+        if (bands.device != x.device or bands.dim() != 3 or tuple(bands.shape) != (C, B, self.nbands)
+                or (B > 0 and bands.stride(2) != 1) or (B > 1 and bands.stride(1) != self.nbands)):
+            raise ValueError("bands must be [C, n_samples/hop, nbands] = %s on %s, with stride(2) == 1 and "
+                             "stride(1) == nbands" % ((C, B, self.nbands), x.device))
+
     def _bank(self, x, bands):
+        self._check_bands(x, bands)
         x, x_stride = _lib.device_rows(self, x, "x")
-        self.bank._ensure_plan(x.shape[0])
-        B = bands.shape[1]
+        C, B = x.shape[0], bands.shape[1]
+        self.bank._ensure_plan(C)
         with _lib.call_stream(x.device) as sp:
             self.handle.call("frt_bank_process_strided", _lib._ptr(x), x_stride, int(self.hop), int(B),
                              _lib._ptr(bands), int(bands.stride(0)), 1, sp)
@@ -102,15 +133,19 @@ class ChannelAnalyzer:
         """x_host: CPU float32 tensor / array [C, n_samples] (pinned memory for full PCIe speed).
         Outputs are written into the given CPU tensors (allocated pinned when omitted)."""
         import torch
+        if getattr(x_host, "ndim", None) != 2:
+            raise ValueError("x_host must be [C, n_samples]")
+        x_host, x_stride = _lib.host_rows(x_host, "x_host")
         C, T = x_host.shape
         F, B = self.frames(T), self.blocks(T)
         if spec_host is None:
             spec_host = torch.empty((C, F, self.nbins), dtype=torch.float32, pin_memory=True)
         if bands_host is None:
             bands_host = torch.empty((C, B, self.nbands), dtype=torch.float32, pin_memory=True)
+        _lib.check_host_out(spec_host, (C, F, self.nbins), "spec_host")
+        _lib.check_host_out(bands_host, (C, B, self.nbands), "bands_host")
         self.proc._ensure_plan()
         self.bank._ensure_plan(C)
-        _, x_stride = _lib.host_rows(x_host)
         self.handle.call("frt_combined_process_host", _lib._ptr(x_host), x_stride, int(C), int(T),
                          int(self.hop), _lib._ptr(spec_host), _lib._ptr(bands_host), int(self.nbands), 1)
         return spec_host, bands_host
@@ -152,6 +187,7 @@ class ChannelAnalyzer:
         fc = F // n_chunks
         if bands is None:
             bands = torch.empty((C, B, self.nbands), dtype=torch.float32, device=x.device)
+        self._check_bands(x, bands)
         cur = torch.cuda.current_stream(x.device)
         s_stft, s_bank, s_comm = self._side_streams()
         for s in (s_stft, s_bank, s_comm):

@@ -121,9 +121,10 @@ class audioproc():
         C, T = x.shape
         nf = frame_count(T, self.fft_size, hop)
         nb = self.fft_size // 2 + 1
-        if out is not None and (tuple(out.shape) != (C, nf, nb) or out.dtype != torch.float32
+        if out is not None and (not isinstance(out, torch.Tensor) or out.device != x.device
+                                or tuple(out.shape) != (C, nf, nb) or out.dtype != torch.float32
                                 or not out.is_contiguous()):
-            raise ValueError("out must be a contiguous float32 tensor of shape %s" % ((C, nf, nb),))
+            raise ValueError("out must be a contiguous float32 tensor of shape %s on %s" % ((C, nf, nb), x.device))
         with _lib.call_stream(x.device, stream) as sp:
             if out is None:
                 out = torch.empty((C, nf, nb), dtype=torch.float32, device=x.device)
@@ -145,7 +146,9 @@ class audioproc():
         C, T = x.shape
         nf = frame_count(T, self.fft_size, hop)
         nb = self.fft_size // 2 + 1
-        if out is None:
+        if out is not None:
+            _lib.check_host_out(out, (C, nf, nb), "out")
+        else:
             if is_torch:
                 import torch
                 out = torch.empty((C, nf, nb), dtype=torch.float32, pin_memory=x.is_pinned())

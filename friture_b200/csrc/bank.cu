@@ -706,6 +706,17 @@ static int bank_process_impl(frt_handle h, const float *x_dev, int64_t x_stride,
                              int n_blocks, float *energies_dev, int64_t e_stride, float *y_dev,
                              int64_t y_stride, int db, void *stream);
 
+// the chunk-scan kernels' tile: the longest of 1024, 512 and 256 samples that divides the block
+static int bank_tile(int block) { return (block % 1024 == 0) ? 1024 : ((block % 512 == 0) ? 512 : 256); }
+
+int frt_bank_check_block(frt_ctx *h, const BankPlan *pl, int block) {
+    // blocks must stay even-length at every stage (decimate.py:41 restarts the [::2] phase
+    // on every call), i.e. block % 2^(n_oct-1) == 0; the kernel tiles are 256/512/1024
+    FRT_CHECK_ARG(h, block > 0 && block % 256 == 0, "block must be a multiple of 256 samples");
+    FRT_CHECK_ARG(h, (bank_tile(block) >> (pl->params.n_oct - 1)) >= 1, "block too short for this many octaves");
+    return FRT_OK;
+}
+
 extern "C" int frt_bank_process(frt_handle h, const float *x_dev, int64_t x_stride, int block,
                                 int n_blocks, float *energies_dev, float *y_dev,
                                 int64_t y_stride, int db, void *stream) {
@@ -738,13 +749,10 @@ static int bank_process_impl(frt_handle h, const float *x_dev, int64_t x_stride,
     const BankParams &P = pl->params;
     FRT_CHECK_ARG(h, n_blocks >= 0 && block >= 0, "negative shape");
     if (n_blocks == 0 || block == 0) return FRT_OK;   // empty chunk: octavespectrum.py:94-95
-    // blocks must stay even-length at every stage (decimate.py:41 restarts the [::2] phase
-    // on every call), i.e. block % 2^(n_oct-1) == 0; the kernel tiles are 256/512/1024
-    FRT_CHECK_ARG(h, block % 256 == 0, "block must be a multiple of 256 samples");
+    if (const int rc = frt_bank_check_block(h, pl, block)) return rc;
     FRT_CHECK_ARG(h, x_dev != nullptr, "x_dev is NULL");
     FRT_CHECK_ARG(h, x_stride >= (int64_t)block * n_blocks, "x_stride too small");
-    int tile = (block % 1024 == 0) ? 1024 : ((block % 512 == 0) ? 512 : 256);
-    FRT_CHECK_ARG(h, (tile >> (P.n_oct - 1)) >= 1, "block too short for this many octaves");
+    const int tile = bank_tile(block);
     const long long t_total = (long long)block * n_blocks;
     if (y_dev) {
         long long need = 0;

@@ -80,6 +80,11 @@ struct BankPlan {
     double alphas[BANK_MAX_OCT];
 };
 
+// bank.cu: FRT_EINVAL (with the handle's error message) unless every filterbank kernel can run
+// blocks of `block` samples for this plan; the filterbank and combined entry points refuse such a
+// block before they queue anything
+int frt_bank_check_block(frt_ctx *h, const BankPlan *pl, int block);
+
 // bank_pipe.cu
 void frt_pipe_prepare(BankPlan *pl);
 void frt_pipe_schedule(int n_oct, int logch, long long t_total, int *T /*[BANK_MAX_OCT+1]*/, int *n_steps);

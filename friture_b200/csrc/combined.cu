@@ -5,27 +5,16 @@
 // y**2, exp_smoothed_value, 10*log10 + weighting).  The stream is cut into time segments; the H2D
 // copy of segment s+1, the two kernels of segment s and the D2H copy of segment s-1 overlap.  All channels go through every launch: the filterbank's
 // parallelism is the channel axis.
-#include "frt_internal.cuh"
+#include "bank_internal.cuh"
 
-extern "C" int frt_combined_process_host(frt_handle h, const float *x_host, int64_t x_stride,
-                                         int n_channels, int64_t n_samples, int hop,
-                                         float *spec_host, float *bands_host, int nbands, int db) {
-    if (!h) return FRT_EINVAL;
-    DeviceGuard g(h->device);
-    if (!h->stft) return frt_fail(h, FRT_ESTATE, "frt_combined_process_host: call frt_stft_plan first");
-    if (!h->bank) return frt_fail(h, FRT_ESTATE, "frt_combined_process_host: call frt_bank_plan first");
+// Queues the segments on the staging streams; returns at the first error, with work still queued.
+static int combined_segments(frt_handle h, const float *x_host, int64_t x_stride, int n_channels,
+                             int64_t n_samples, int hop, float *spec_host, float *bands_host, int nbands,
+                             int db) {
     const int N = h->stft->n_fft;
-    FRT_CHECK_ARG(h, n_channels >= 1 && hop >= 256 && n_samples >= 0, "bad shape");
-    FRT_CHECK_ARG(h, n_samples % hop == 0, "n_samples must be a whole number of hops");
-    FRT_CHECK_ARG(h, x_host && spec_host && bands_host, "NULL buffer");
-    FRT_CHECK_ARG(h, x_stride >= n_samples, "x_stride smaller than n_samples");
     const int nbins = N / 2 + 1;
     const int64_t B = n_samples / hop;                                   // filterbank blocks
     const int64_t F = n_samples >= N ? (n_samples - N) / hop + 1 : 0;    // spectrogram columns
-    if (B == 0) return FRT_OK;
-    // the staging streams are non-blocking and wait for nothing: a device call on this handle that is
-    // still queued on any stream (it reads and writes the filterbank state) must finish first
-    FRT_CUDA(h, cudaDeviceSynchronize());
     CombStaging &p = h->comb_host;
     FRT_CUDA(h, p.create());
     FRT_CUDA(h, p.d_x.grow((size_t)n_channels * n_samples));
@@ -84,8 +73,42 @@ extern "C" int frt_combined_process_host(frt_handle h, const float *x_host, int6
     FRT_CUDA(h, cudaStreamWaitEvent(s_out, p.ev_out[last].get(), 0));
     FRT_CUDA(h, cudaMemcpyAsync(bands_host, d_bands, sizeof(float) * (size_t)n_channels * B * nbands,
                                 cudaMemcpyDeviceToHost, s_out));
-    FRT_CUDA(h, cudaStreamSynchronize(s_out));
-    FRT_CUDA(h, cudaStreamSynchronize(s_cmp));
-    FRT_CUDA(h, cudaStreamSynchronize(s_in));
     return FRT_OK;
+}
+
+extern "C" int frt_combined_process_host(frt_handle h, const float *x_host, int64_t x_stride,
+                                         int n_channels, int64_t n_samples, int hop,
+                                         float *spec_host, float *bands_host, int nbands, int db) {
+    if (!h) return FRT_EINVAL;
+    DeviceGuard g(h->device);
+    if (!h->stft) return frt_fail(h, FRT_ESTATE, "frt_combined_process_host: call frt_stft_plan first");
+    if (!h->bank) return frt_fail(h, FRT_ESTATE, "frt_combined_process_host: call frt_bank_plan first");
+    // every refusal comes before the first copy: the bank runs over all of its plan's channels and
+    // writes its plan's bands, so the staging buffers, sized from the arguments, must hold exactly those
+    const BankPlan *pl = h->bank.get();
+    FRT_CHECK_ARG(h, n_channels >= 1 && hop >= 256 && n_samples >= 0, "bad shape");
+    FRT_CHECK_ARG(h, n_channels == pl->n_channels, "n_channels differs from the filterbank plan's channels");
+    FRT_CHECK_ARG(h, nbands == pl->params.n_oct * pl->params.bpo, "nbands differs from the filterbank plan's bands");
+    if (const int rc = frt_bank_check_block(h, pl, hop)) return rc;
+    FRT_CHECK_ARG(h, n_samples % hop == 0, "n_samples must be a whole number of hops");
+    FRT_CHECK_ARG(h, x_stride >= n_samples, "x_stride smaller than n_samples");
+    if (n_samples == 0) return FRT_OK;
+    // a stream shorter than one frame has band levels but no columns: spec_host may then be empty
+    const bool has_columns = n_samples >= h->stft->n_fft;
+    FRT_CHECK_ARG(h, x_host && bands_host && (spec_host || !has_columns), "NULL buffer");
+    // the staging streams are non-blocking and wait for nothing: a device call on this handle that is
+    // still queued on any stream (it reads and writes the filterbank state) must finish first
+    FRT_CUDA(h, cudaDeviceSynchronize());
+    int rc = combined_segments(h, x_host, x_stride, n_channels, n_samples, hop, spec_host, bands_host, nbands, db);
+    // the queued copies read and write the caller's buffers: whatever happened, none is still in
+    // flight when the call returns
+    CombStaging &p = h->comb_host;
+    for (const cudaStream_t s : {p.s_out.get(), p.s_cmp.get(), p.s_in.get()}) {
+        if (!s) continue;
+        const cudaError_t e = cudaStreamSynchronize(s);
+        if (rc == FRT_OK && e != cudaSuccess)
+            rc = frt_fail(h, FRT_ECUDA, "cudaStreamSynchronize failed: %s (%s:%d)", cudaGetErrorString(e),
+                          __FILE__, __LINE__);
+    }
+    return rc;
 }

@@ -188,7 +188,15 @@ int frt_firbank_levels(frt_handle h, const float *x_dev, int64_t x_stride, int b
  * H2D copy, the two kernels and the D2H copies are pipelined over time segments inside the call
  * (bench.py's `e2e`).  n_samples % hop == 0, hop a valid filterbank block;
  *   spec_host  [n_channels][(n_samples - n_fft)/hop + 1][n_fft/2 + 1]
- *   bands_host [n_channels][n_samples/hop][nbands]                                               */
+ *   bands_host [n_channels][n_samples/hop][nbands]
+ * spec_host may be NULL when n_samples < n_fft (no columns, only band levels).
+ * FRT_EINVAL, before any copy or kernel is queued and with the filter state unchanged, unless
+ * n_channels is the bank plan's channel count, nbands its n_octaves * bands_per_octave, and hop a
+ * block the bank runs: a multiple of 256 whose tile (the longest of 1024, 512 and 256 samples that
+ * divides it) holds 2^(n_octaves-1) samples -- so at 10 octaves 768 is refused, 512 and 1536 are not.
+ * Any blocking of the stream gives the same bits as frt_stft_process and frt_bank_process_strided
+ * on the same samples.  The call returns only once none of its copies is still in flight, after an
+ * error too.                                                                                       */
 int frt_combined_process_host(frt_handle h, const float *x_host, int64_t x_stride, int n_channels,
                               int64_t n_samples, int hop, float *spec_host, float *bands_host,
                               int nbands, int db);

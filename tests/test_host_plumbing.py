@@ -50,6 +50,41 @@ def test_host_rows():
         assert tuple(rows.shape) == (C, T) and s == stride and type(s) is int
 
 
+def test_host_rows_rejections():
+    """The library reads host input as float32 rows at the returned stride: anything else is refused."""
+    T = 1000
+    bad = [
+        np.zeros((3, T), np.float64),                      # read as float32 it would be other samples
+        torch.zeros((3, T), dtype=torch.float64),
+        np.zeros((T, 3), np.float32).T,                    # not contiguous along time
+        torch.zeros((T, 3)).t(),
+        np.zeros((2, 3, T), np.float32),                   # not [C, T]
+        np.zeros((3, T), np.float32)[::-1],                # rows overlap / run backwards
+        [[0.0] * T],                                       # not an array
+    ]
+    for x in bad:
+        with pytest.raises(ValueError):
+            _lib.host_rows(x)
+
+
+def test_check_host_out():
+    shape = (2, 3, 5)
+    _lib.check_host_out(np.zeros(shape, np.float32), shape, "out")
+    _lib.check_host_out(torch.zeros(shape), shape, "out")
+    for out in (np.zeros(shape, np.float64), torch.zeros(shape, dtype=torch.float64), np.zeros((2, 4, 5), np.float32),
+                np.zeros((2, 3, 6), np.float32)[..., :5], torch.zeros((2, 5, 3)).transpose(1, 2), [[0.0]]):
+        with pytest.raises(ValueError):
+            _lib.check_host_out(out, shape, "out")
+
+
+def test_bank_block_rule():
+    """ChannelAnalyzer refuses the hops the filterbank kernels refuse (bank.cu, frt_bank_check_block)."""
+    from friture_b200.analyzer import bank_block_ok
+    assert [b for b in range(0, 4097, 128) if bank_block_ok(b, 10)] == [512, 1024, 1536, 2048, 2560, 3072, 3584, 4096]
+    assert [b for b in range(0, 2049, 128) if bank_block_ok(b, 9)] == list(range(256, 2049, 256))
+    assert bank_block_ok(256, 1) and not bank_block_ok(384, 1) and not bank_block_ok(-256, 3)
+
+
 class StandInHandle:
     """The handle's device check, bound to cuda:0 without a GPU."""
     device = 0
