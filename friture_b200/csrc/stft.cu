@@ -556,17 +556,26 @@ template <int Q, int MODE = FRT_STFT_POWER> __host__ __device__ constexpr int sm
 template <int Q, int MODE = FRT_STFT_POWER> __host__ __device__ constexpr int small_ctas_per_sm() {
     return Q == 32 || smooth_nch(MODE) ? 1 : 2;
 }
-// kModeScreen: the warp's G columns go to its tile, free again after the transpose; with TMA the tile
-// already holds the next frame by then, so each warp has a column buffer of its own after the mbarriers.
+// Byte offsets of stft_small_kernel's shared memory; small_smem() is its size.  kModeScreen: the warp's
+// G columns go to its tile, free again after the transpose; with TMA the tile already holds the next
+// frame by then, so each warp has a column buffer of its own after the mbarriers.
+template <int Q, int MODE, bool TMA>
+struct SmallSmem {
+    static constexpr int W = small_warps<Q, MODE>(), M = 32 * Q;
+    static constexpr size_t win = 0;                                    // [M]      (w[2n], w[2n+1])
+    static constexpr size_t tw = win + sizeof(float2) * M;              // [Q][32]  W_M^(k1 t)
+    static constexpr size_t post = tw + sizeof(float2) * M;             // [M/2]    U[k] = -j W_N^k
+    static constexpr size_t tiles = post + sizeof(float2) * (M / 2);    // [W]      padded tiles
+    static constexpr size_t bars = tiles + sizeof(float2) * W * TILE;   // (Q = 32) [W] mbarriers
+    static constexpr size_t cols = bars + (Q == 32 ? sizeof(unsigned long long) * W : 0);   // (kModeScreen, TMA)
+    static constexpr size_t slots = cols + (MODE == kModeScreen && TMA ? sizeof(float) * W * (M + 1) : 0);
+    static constexpr size_t end = slots + W * smooth_slot_bytes<MODE>(M + 1, 1);   // (smoothing) [W] slots
+    static_assert(tiles % 16 == 0 && TILE * sizeof(float2) % 16 == 0,
+                  "the TMA engine writes each warp's tile in 16-byte units");
+};
 template <int Q, int MODE, bool TMA>
 constexpr size_t small_smem() {
-    // window, twiddle and split tables, the warps' tiles, (Q = 32) the warps' mbarriers,
-    // (kModeScreen with TMA) the warps' column buffers and (smoothing) the warps' states
-    constexpr int W = small_warps<Q, MODE>();
-    return sizeof(float2) * (32 * Q + 32 * Q + 16 * Q + (size_t)W * TILE) +
-           (Q == 32 ? sizeof(unsigned long long) * W : 0) +
-           (MODE == kModeScreen && TMA ? sizeof(float) * (size_t)W * (32 * Q + 1) : 0) +
-           W * smooth_slot_bytes<MODE>(32 * Q + 1, 1);
+    return SmallSmem<Q, MODE, TMA>::end;
 }
 
 template <int Q, int MODE, bool TMA>
@@ -577,13 +586,14 @@ stft_small_kernel(const float *__restrict__ x, long long x_stride, long long n_f
                   const float2 *__restrict__ post, long long total_items, int vec_ok, const ScreenRows scr,
                   const SmoothTicks sm) {
     static_assert(!TMA || Q == 32, "TMA staging is for one frame per warp");
+    using L = SmallSmem<Q, MODE, TMA>;
     constexpr int G = 32 / Q, M = 32 * Q, N = 2 * M, WARPS = small_warps<Q, MODE>(), NCH = smooth_nch(MODE);
     extern __shared__ float2 smem[];
-    float2 *s_win = smem;              // [M]     (w[2n], w[2n+1])
-    float2 *s_tw = s_win + M;          // [Q][32] W_M^(k1 t)
-    float2 *s_post = s_tw + M;         // [M/2]   U[k] = -j W_N^k
+    float2 *s_win = smem + L::win / sizeof(float2);   // every region starts on 8 bytes
+    float2 *s_tw = smem + L::tw / sizeof(float2);
+    float2 *s_post = smem + L::post / sizeof(float2);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    float2 *s_x = s_post + 16 * Q + warp * TILE;   // 16-byte aligned: 80 Q and TILE are even
+    float2 *s_x = smem + L::tiles / sizeof(float2) + warp * TILE;
     for (int i = threadIdx.x; i < M; i += blockDim.x) {
         s_win[i] = win2[i];
         s_tw[i] = tw[i];
@@ -591,24 +601,71 @@ stft_small_kernel(const float *__restrict__ x, long long x_stride, long long n_f
     for (int i = threadIdx.x; i < 16 * Q; i += blockDim.x) s_post[i] = post[i];
     __syncthreads();
 
-    // Smoothing outputs: warp gw walks channels gw, gw + warps_total, ..; its items are a channel's frames
-    // (kModeSmoothDual: reference and measurement in turn, frame_at).  The other outputs keep the loop below
-    // to themselves, so that their code is what it was before this output existed.
-    if constexpr (NCH > 0) {
-        const long long warps_total = (long long)gridDim.x * WARPS;
-        const float scale = 1.0f / (4.0f * (float)N * (float)N);
-        const int k1 = lane & (Q - 1), gsel = lane / Q;
-        const int src_lane = (lane - k1) + ((Q - k1) & (Q - 1));
-        unsigned long long *bar = reinterpret_cast<unsigned long long *>(s_post + 16 * Q + WARPS * TILE) + warp;
-        unsigned char *states = reinterpret_cast<unsigned char *>(bar - warp + (Q == 32 ? WARPS : 0));
-        auto s = slot_smoother<NCH>(sm, states + warp * smooth_slot_bytes<MODE>(M + 1, 1), M + 1, lane, 32,
-                                    [] { __syncwarp(); });
-        unsigned parity = 0;
+    // The steps both loops below take.  TMA: the warp's mbarrier, before the loop's first fetch.
+    unsigned long long *bar = reinterpret_cast<unsigned long long *>(smem + L::bars / sizeof(float2)) + warp;
+    auto init_bar = [&] {
         if (TMA) {
             if (lane == 0) mbar_init(bar, 1);
             fence_proxy_async();
             __syncwarp();
         }
+    };
+    // window, first pass and transpose of the group in v: v[g*Q + r] = sum_n1 z_g[32 n1 + t] W_Q^(n1 k1),
+    // k1 = brevq<Q>(r), then twiddled and transposed; the tile is free again afterwards
+    auto first_pass = [&](float2(&v)[32]) {
+#pragma unroll
+        for (int n1 = 0; n1 < Q; n1++) {
+            const float2 w = s_win[32 * n1 + lane];
+#pragma unroll
+            for (int g = 0; g < G; g++) v[g * Q + n1] = f2_mul(v[g * Q + n1], w);
+        }
+        dft_groups<Q>(v);
+        twiddle_transpose<Q>(v, s_tw, s_x, lane);
+    };
+    // the split step of the lane's bins k = k1 + Q m, their partners M - k and (k1 = 0) bin M/2, after
+    // the second pass: put(k, value of bin k), if the lane's frame exists (ok)
+    auto split = [&](const float2(&v)[32], int k1, int src_lane, float scale, bool ok, auto put) {
+#pragma unroll
+        for (int m = 0; m < 16; m++) {
+            const float2 z = v[brev5(m)];
+            const float2 other = v[brev5(31 - m)];
+            float2 zp;
+            zp.x = __shfl_sync(0xffffffffu, other.x, src_lane);
+            zp.y = __shfl_sync(0xffffffffu, other.y, src_lane);
+            if (k1 == 0) zp = (m == 0) ? v[0] : v[brev5(32 - m)];
+            const float2 E = make_float2(z.x + zp.x, z.y - zp.y);
+            const float2 O = make_float2(z.x - zp.x, z.y + zp.y);
+            const int k = k1 + Q * m;
+            const float2 T = cmul(O, s_post[k]);
+            const float2 X = cadd(E, T);
+            const float2 Y = csub(E, T);
+            const float p1 = fmaf(X.x, X.x, X.y * X.y);
+            const float p2 = fmaf(Y.x, Y.x, Y.y * Y.y);
+            if (ok) {
+                put(k, finish<MODE>(p1, scale));
+                put(M - k, finish<MODE>(p2, scale));
+            }
+        }
+        if (k1 == 0 && ok) {
+            const float2 z = v[brev5(16)];   // bin M/2: X = conj(Z)
+            put(M / 2, finish<MODE>(4.0f * fmaf(z.x, z.x, z.y * z.y), scale));
+        }
+    };
+
+    // Smoothing outputs: warp gw walks channels gw, gw + warps_total, ..; its items are a channel's frames
+    // (kModeSmoothDual: reference and measurement in turn, frame_at).  The other outputs keep the loop below
+    // to themselves, so that their code is what it was before this output existed; both loops call the
+    // steps above.
+    if constexpr (NCH > 0) {
+        const long long warps_total = (long long)gridDim.x * WARPS;
+        const float scale = 1.0f / (4.0f * (float)N * (float)N);
+        const int k1 = lane & (Q - 1), gsel = lane / Q;
+        const int src_lane = (lane - k1) + ((Q - k1) & (Q - 1));
+        unsigned char *slot = reinterpret_cast<unsigned char *>(smem + L::slots / sizeof(float2)) +
+                              warp * smooth_slot_bytes<MODE>(M + 1, 1);
+        auto s = slot_smoother<NCH>(sm, slot, M + 1, lane, 32, [] { __syncwarp(); });
+        unsigned parity = 0;
+        init_bar();
         const long long nv = NCH * n_frames;
         for (long long ch = (long long)blockIdx.x * WARPS + warp; ch < sm.n_channels; ch += warps_total) {
             s.begin(ch);
@@ -650,14 +707,7 @@ stft_small_kernel(const float *__restrict__ x, long long x_stride, long long n_f
                         for (int n1 = 0; n1 < Q; n1++) v[g * Q + n1] = make_float2(0.0f, 0.0f);
                     }
                 }
-#pragma unroll
-                for (int n1 = 0; n1 < Q; n1++) {
-                    const float2 w = s_win[32 * n1 + lane];
-#pragma unroll
-                    for (int g = 0; g < G; g++) v[g * Q + n1] = f2_mul(v[g * Q + n1], w);
-                }
-                dft_groups<Q>(v);
-                twiddle_transpose<Q>(v, s_tw, s_x, lane);
+                first_pass(v);
                 if (TMA && f < nv) {   // the tile is free: fetch the next item into it
                     fence_proxy_async();
                     if (lane == 0) {
@@ -671,38 +721,10 @@ stft_small_kernel(const float *__restrict__ x, long long x_stride, long long n_f
                 constexpr bool direct = G == 1;
                 const int j = (int)(myf % NCH);
                 float *o = reinterpret_cast<float *>(s_x) + gsel * (M + 1);
-#pragma unroll
-                for (int m = 0; m < 16; m++) {
-                    const float2 z = v[brev5(m)];
-                    const float2 other = v[brev5(31 - m)];
-                    float2 zp;
-                    zp.x = __shfl_sync(0xffffffffu, other.x, src_lane);
-                    zp.y = __shfl_sync(0xffffffffu, other.y, src_lane);
-                    if (k1 == 0) zp = (m == 0) ? v[0] : v[brev5(32 - m)];
-                    const float2 E = make_float2(z.x + zp.x, z.y - zp.y);
-                    const float2 O = make_float2(z.x - zp.x, z.y + zp.y);
-                    const int k = k1 + Q * m;
-                    const float2 T = cmul(O, s_post[k]);
-                    const float2 X = cadd(E, T);
-                    const float2 Y = csub(E, T);
-                    const float p1 = finish<MODE>(fmaf(X.x, X.x, X.y * X.y), scale);
-                    const float p2 = finish<MODE>(fmaf(Y.x, Y.x, Y.y * Y.y), scale);
-                    if (myok) {
-                        if constexpr (direct) {
-                            s.add(j, k, p1);
-                            s.add(j, M - k, p2);
-                        } else {
-                            o[k] = p1;
-                            o[M - k] = p2;
-                        }
-                    }
-                }
-                if (k1 == 0 && myok) {
-                    const float2 z = v[brev5(16)];   // bin M/2: X = conj(Z)
-                    const float p = finish<MODE>(4.0f * fmaf(z.x, z.x, z.y * z.y), scale);
-                    if constexpr (direct) s.add(j, M / 2, p);
-                    else o[M / 2] = p;
-                }
+                split(v, k1, src_lane, scale, myok, [&](int k, float p) {
+                    if constexpr (direct) s.add(j, k, p);
+                    else o[k] = p;
+                });
                 __syncwarp();   // every add, or the warp's G columns, complete
                 if constexpr (direct) {
                     s.after(myf);
@@ -742,16 +764,11 @@ stft_small_kernel(const float *__restrict__ x, long long x_stride, long long n_f
         // while the frame before it is in its second FFT pass and split step, so no warp ever waits on
         // a global load with its registers tied up.  The first frame is fetched here, each next one
         // once the transpose has freed the tile.
-        unsigned long long *bar = reinterpret_cast<unsigned long long *>(s_post + 16 * Q + WARPS * TILE) + warp;
         unsigned parity = 0;
-        if (TMA) {
-            if (lane == 0) mbar_init(bar, 1);
-            fence_proxy_async();
-            __syncwarp();
-            if (lane == 0 && item < item_end) {
-                mbar_expect_tx(bar, N * 4);
-                bulk_g2s(s_x, x + c * x_stride + f * hop, N * 4, bar);
-            }
+        init_bar();
+        if (TMA && lane == 0 && item < item_end) {
+            mbar_expect_tx(bar, N * 4);
+            bulk_g2s(s_x, x + c * x_stride + f * hop, N * 4, bar);
         }
         for (; item < item_end; item += G) {
             float2 v[32];
@@ -791,14 +808,7 @@ stft_small_kernel(const float *__restrict__ x, long long x_stride, long long n_f
                     c++;
                 }
             }
-#pragma unroll
-            for (int n1 = 0; n1 < Q; n1++) {
-                const float2 w = s_win[32 * n1 + lane];
-#pragma unroll
-                for (int g = 0; g < G; g++) v[g * Q + n1] = f2_mul(v[g * Q + n1], w);
-            }
-            dft_groups<Q>(v);   // v[g*Q + r] = sum_n1 z_g[32 n1 + t] W_Q^(n1 k1), k1 = brevq<Q>(r)
-            twiddle_transpose<Q>(v, s_tw, s_x, lane);
+            first_pass(v);
             if (TMA && item + 1 < item_end) {   // the tile is free: fetch the next frame, (c, f), into it
                 fence_proxy_async();
                 if (lane == 0) {
@@ -811,38 +821,12 @@ stft_small_kernel(const float *__restrict__ x, long long x_stride, long long n_f
             float *o;
             if constexpr (MODE == kModeScreen) {
                 float *s_col = reinterpret_cast<float *>(s_x);
-                if (TMA)
-                    s_col = reinterpret_cast<float *>(reinterpret_cast<unsigned long long *>(s_post + 16 * Q + WARPS * TILE) +
-                                                      WARPS) + warp * (M + 1);
+                if (TMA) s_col = reinterpret_cast<float *>(smem + L::cols / sizeof(float2)) + warp * (M + 1);
                 o = s_col + gsel * (M + 1);
             } else {
                 o = out + myc * out_stride_c + myf * out_stride_f;
             }
-#pragma unroll
-            for (int m = 0; m < 16; m++) {
-                const float2 z = v[brev5(m)];
-                const float2 other = v[brev5(31 - m)];
-                float2 zp;
-                zp.x = __shfl_sync(0xffffffffu, other.x, src_lane);
-                zp.y = __shfl_sync(0xffffffffu, other.y, src_lane);
-                if (k1 == 0) zp = (m == 0) ? v[0] : v[brev5(32 - m)];
-                const float2 E = make_float2(z.x + zp.x, z.y - zp.y);
-                const float2 O = make_float2(z.x - zp.x, z.y + zp.y);
-                const int k = k1 + Q * m;
-                const float2 T = cmul(O, s_post[k]);
-                const float2 X = cadd(E, T);
-                const float2 Y = csub(E, T);
-                const float p1 = fmaf(X.x, X.x, X.y * X.y);
-                const float p2 = fmaf(Y.x, Y.x, Y.y * Y.y);
-                if (myok) {
-                    o[k] = finish<MODE>(p1, scale);
-                    o[M - k] = finish<MODE>(p2, scale);
-                }
-            }
-            if (k1 == 0 && myok) {
-                const float2 z = v[brev5(16)];   // bin M/2: X = conj(Z)
-                o[M / 2] = finish<MODE>(4.0f * fmaf(z.x, z.x, z.y * z.y), scale);
-            }
+            split(v, k1, src_lane, scale, myok, [&](int k, float p) { o[k] = p; });
             if constexpr (MODE == kModeScreen) {
                 __syncwarp();   // the warp's G columns are complete
                 const float *s_col = o - gsel * (M + 1);

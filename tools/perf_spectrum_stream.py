@@ -7,9 +7,10 @@ frt_spectrum_reduce_ticks), with and without the dB rows.
 
 One call is one second of 512-sample buffers (93 buffers, 47616 samples per channel) at 48 kHz; the
 same chunk is pushed on every call.  process_ticks gets the frames the first call cuts (zeros before
-the stream, as the widget's framing gives), one frame per tick.  The two routes are timed alternately
-in the same run with CUDA events around each whole call (host work and the index reads included),
-median of the rounds, after a warm-up of each.  The byte model is from
+the stream, as the widget's framing gives), one tick per buffer: one frame per tick at N >= 2048,
+512 / hop frames per tick below.  The two routes are timed alternately in the same run with CUDA
+events around each whole call (host work and the index reads included), median of the rounds, after
+a warm-up of each.  The byte model is from
 shapes: HBM bytes a route must move per call beyond reading its input once, over the call's time,
 against the H100 SXM data sheet's 3.35 TB/s.  The card's name and power limit are read in the same run.
 """
@@ -54,20 +55,21 @@ def case(C, N, want_db, rounds):
     stream = SpectrumAnalyzer(C, fft_size=N)
     ticks = SpectrumAnalyzer(C, fft_size=N)
     hop, nb = stream.hop, N // 2 + 1
-    # the frames process_ticks gets: those the first call cuts, one per tick (hop >= 512 here).  Frame f
-    # ends at old_index = f hop, with zeros before the stream starts.
+    per_tick = max(512 // hop, 1)   # frames a 512-sample buffer cuts: 1 for N >= 2048, 512 / hop below
+    # the frames process_ticks gets: those the first call cuts, per_tick per tick.  Frame f ends at
+    # old_index = f hop, with zeros before the stream starts.
     first = stream.handle_new_data(x, buffer=512, want_db=want_db)
     F = int(first.n_frames.sum())
-    assert np.all(first.n_frames == 1)
+    assert np.all(first.n_frames == per_tick)
     frames = torch.cat([torch.zeros(C, N, device="cuda"), x], dim=1)[:, :(F - 1) * hop + N].contiguous()
-    check = SpectrumAnalyzer(C, fft_size=N).process_ticks(frames, frames_per_tick=1, want_db=True)
+    check = SpectrumAnalyzer(C, fft_size=N).process_ticks(frames, frames_per_tick=per_tick, want_db=True)
     assert np.array_equal(check.fmax_hz, first.fmax_hz)     # the same frames, the same peaks
 
     def run_stream():
         return stream.handle_new_data(x, buffer=512, want_db=want_db)
 
     def run_ticks():
-        return ticks.process_ticks(frames, frames_per_tick=1, want_db=want_db)
+        return ticks.process_ticks(frames, frames_per_tick=per_tick, want_db=want_db)
 
     run_stream()
     run_ticks()
@@ -101,7 +103,7 @@ def main():
     print("%5s %6s %3s %7s %10s %10s %7s %12s %12s %8s %8s" % (
         "C", "N", "dB", "frames", "stream ms", "ticks ms", "ratio", "B/ch-frame s", "B/ch-frame t",
         "HBM% s", "HBM% t"))
-    for N in (8192, 2048):
+    for N in (8192, 2048, 1024, 256, 128, 64):
         for want_db in (True, False):
             r = case(args.channels, N, want_db, args.rounds)
             print("%5d %6d %3s %7d %10.3f %10.3f %7.2f %12.0f %12.0f %8.1f %8.1f" % (
