@@ -116,31 +116,34 @@ class SpectrumAnalyzer:
         [C, 2, T] input, dB is the transfer function 10 log10(sp2) - 10 log10(sp1), unweighted, and
         fmax its peak; otherwise dB is 10 log10(sp1) + weighting of row 0.  The pitch always comes
         from row 0 (spectrum.py:180)."""
-        x, dual = self._input(x)
-        if dual:
-            return self._process_dual(x, stream)
         import torch
-        C = x.shape[0]
+        x, dual = self._input(x)
+        C = self.n_channels
         nb = self.fft_size // 2 + 1
-        nf = frame_count(x.shape[1], self.fft_size, self.hop)
-        with _lib.call_stream(x.device, stream) as sp:
-            power = self.proc.stft(x, hop=self.hop, log=False, stream=stream)
-            if self._disp is None:
-                self._disp = torch.zeros((C, nb), dtype=torch.float32, device=x.device)
-            if self._w_dev is None:
-                self._w_dev = torch.from_numpy(np.ascontiguousarray(self.w, dtype=np.float32)).to(x.device)
-            db = torch.empty((C, nb), dtype=torch.float32, device=x.device)
-            imax = torch.empty(C, dtype=torch.int32, device=x.device)
-            ipitch = torch.empty(C, dtype=torch.int32, device=x.device)
-            self.proc.handle.call("frt_spectrum_reduce", _lib._ptr(power), int(nf * nb), int(nb), int(C),
-                                  int(nf), int(nb), c_float(self.alpha), _lib._ptr(self._disp),
-                                  _lib._ptr(self._w_dev) if self.weighting else None, _lib._ptr(db),
-                                  _lib._ptr(imax), _lib._ptr(ipitch), sp)
-            if self._disp2 is not None and nf > 0:
-                # the widget smooths an all-zero second column on every tick it does not fill
-                # (spectrum.py:142,158-159): dispbuffers2 * (1-alpha)^frames
-                self._disp2.mul_((1. - self.alpha) ** nf)
-            return self._indices_to_hz(db, imax, ipitch)
+        nf = frame_count(x.shape[-1], self.fft_size, self.hop)
+        dev = x.device
+        with _lib.call_stream(dev, stream) as sp:
+            rows = x.view(2 * C, x.shape[-1]) if dual else x
+            power = self.proc.stft(rows, hop=self.hop, log=False, stream=stream)
+            self._states(dev, dual)
+            db = torch.empty((C, nb), dtype=torch.float32, device=dev)
+            imax = torch.empty(C, dtype=torch.int32, device=dev)
+            ipitch = torch.empty(C, dtype=torch.int32, device=dev)
+            h = self.proc.handle
+            if dual:
+                # power [2C, nf, nb]: pair c's reference at row 2c, its measurement at row 2c + 1
+                p1 = power.data_ptr() if nf else 0
+                p2 = p1 + 4 * nf * nb if nf else 0
+                h.call("frt_spectrum_reduce_dual", _lib._ptr(p1), _lib._ptr(p2), int(2 * nf * nb), int(nb), int(C),
+                       int(nf), int(nb), c_float(self.alpha), _lib._ptr(self._disp), _lib._ptr(self._disp2),
+                       _lib._ptr(db), _lib._ptr(imax), _lib._ptr(ipitch), sp)
+            else:
+                h.call("frt_spectrum_reduce", _lib._ptr(power), int(nf * nb), int(nb), int(C), int(nf), int(nb),
+                       c_float(self.alpha), _lib._ptr(self._disp),
+                       _lib._ptr(self._w_dev) if self.weighting else None, _lib._ptr(db), _lib._ptr(imax),
+                       _lib._ptr(ipitch), sp)
+                self._decay_unfilled([nf])
+            return (db,) + self._indices_to_hz(imax, ipitch)
 
     def _input(self, x):
         """x as [C, T] or [C, 2, T] and whether it runs in dual mode; [C, 2, T] outside dual mode is
@@ -192,12 +195,7 @@ class SpectrumAnalyzer:
         with _lib.call_stream(dev, stream) as sp:
             rows = x.view(2 * C, x.shape[-1]) if dual else x
             power = self.proc.stft(rows, hop=self.hop, log=False, stream=stream)
-            if self._disp is None:
-                self._disp = torch.zeros((C, nb), dtype=torch.float32, device=dev)
-            if dual and self._disp2 is None:
-                self._disp2 = torch.zeros((C, nb), dtype=torch.float32, device=dev)
-            if not dual and self._w_dev is None:
-                self._w_dev = torch.from_numpy(np.ascontiguousarray(self.w, dtype=np.float32)).to(dev)
+            self._states(dev, dual)
             db = torch.empty((C, R, nb), dtype=torch.float32, device=dev) if want_db else None
             imax = torch.empty((R, C), dtype=torch.int32, device=dev)
             ipitch = torch.empty((R, C), dtype=torch.int32, device=dev)
@@ -215,13 +213,8 @@ class SpectrumAnalyzer:
                            int(R), int(nb), c_float(self.alpha), _lib._ptr(self._disp),
                            _lib._ptr(self._w_dev) if self.weighting else None, _lib._ptr(db),
                            _lib._ptr(imax), _lib._ptr(ipitch), sp)
-                    if self._disp2 is not None:
-                        # process's decay of the unfilled second state, once per tick: each rounds
-                        decay = (1. - self.alpha) ** g
-                        for _ in range(R):
-                            self._disp2.mul_(decay)
-            _, fmax, fpitch = self._indices_to_hz(None, imax, ipitch)
-            return SpectrumTicks(db, fmax, fpitch)
+                    self._decay_unfilled([g] * R)
+            return SpectrumTicks(db, *self._indices_to_hz(imax, ipitch))
 
     # -- the widget's stream ----------------------------------------------------------------------
     def handle_new_data(self, chunk, buffer=None, want_db=True, stream=None):
@@ -264,12 +257,7 @@ class SpectrumAnalyzer:
             imax = torch.empty((R, C), dtype=torch.int32, device=dev)
             ipitch = torch.empty((R, C), dtype=torch.int32, device=dev)
             if F:
-                if self._disp is None:
-                    self._disp = torch.zeros((C, nb), dtype=torch.float32, device=dev)
-                if dual and self._disp2 is None:
-                    self._disp2 = torch.zeros((C, nb), dtype=torch.float32, device=dev)
-                if not dual and self._w_dev is None:
-                    self._w_dev = torch.from_numpy(np.ascontiguousarray(self.w, dtype=np.float32)).to(dev)
+                self._states(dev, dual)
                 # the tick ends go up from pinned memory without waiting for the stream
                 ends_host = torch.from_numpy(ends.astype(np.int32))
                 if dev.type == "cuda":
@@ -291,12 +279,8 @@ class SpectrumAnalyzer:
                            int(self.hop), _lib._ptr(ends_dev), int(R), c_float(self.alpha),
                            _lib._ptr(self._disp), _lib._ptr(self._w_dev) if self.weighting else None,
                            _lib._ptr(db), *db_strides, _lib._ptr(imax), _lib._ptr(ipitch), sp)
-                    if self._disp2 is not None:
-                        # process's decay of the unfilled second state, once per tick
-                        for nf in np.diff(ends, prepend=0):
-                            self._disp2.mul_((1. - self.alpha) ** int(nf))
-            _, fmax, fpitch = self._indices_to_hz(None, imax, ipitch)
-            return SpectrumTicks(db, fmax, fpitch, ticks, np.diff(ends, prepend=0))
+                    self._decay_unfilled(np.diff(ends, prepend=0))
+            return SpectrumTicks(db, *self._indices_to_hz(imax, ipitch), ticks, np.diff(ends, prepend=0))
 
     def stream_ticks(self, n, buffer=None):
         """(ends, ticks) of a ``handle_new_data`` call of n samples per row: the frame index at which
@@ -325,32 +309,30 @@ class SpectrumAnalyzer:
         ticks = np.flatnonzero(per)
         return cum[ticks], ticks
 
-    def _indices_to_hz(self, db, imax, ipitch):
+    def _states(self, dev, dual):
+        """The carried smoothed states, zeros after a restart (the widget's update_display_buffers), and
+        outside dual mode the weighting on the device: whatever of them the coming tick reads and does
+        not have yet."""
+        import torch
+        nb = self.fft_size // 2 + 1
+        if self._disp is None:
+            self._disp = torch.zeros((self.n_channels, nb), dtype=torch.float32, device=dev)
+        if dual and self._disp2 is None:
+            self._disp2 = torch.zeros((self.n_channels, nb), dtype=torch.float32, device=dev)
+        if not dual and self._w_dev is None:
+            self._w_dev = torch.from_numpy(np.ascontiguousarray(self.w, dtype=np.float32)).to(dev)
+
+    def _decay_unfilled(self, frames):
+        """Single-mode ticks of the given frame counts on a kept second state: the widget smooths an
+        all-zero second column on every tick it does not fill (spectrum.py:142,158-159), so
+        dispbuffers2 *= (1-alpha)^frames, rounded once per tick; a tick without frames smooths nothing."""
+        if self._disp2 is not None:
+            for n in frames:
+                if n:
+                    self._disp2.mul_((1. - self.alpha) ** int(n))
+
+    def _indices_to_hz(self, imax, ipitch):
         # on the call's stream, which is current: the reads wait for the kernel that writes them
         fmax = self.freq[imax.cpu().numpy()]
         fpitch = np.maximum(self.freq[ipitch.cpu().numpy()], 1e-20)     # spectrum.py:181
-        return db, fmax, fpitch
-
-    def _process_dual(self, x, stream):
-        """One STFT launch over the 2C rows, then one dual reduce over the C pairs."""
-        import torch
-        C, _, T = x.shape
-        nb = self.fft_size // 2 + 1
-        nf = frame_count(T, self.fft_size, self.hop)
-        with _lib.call_stream(x.device, stream) as sp:
-            power = self.proc.stft(x.view(2 * C, T), hop=self.hop, log=False, stream=stream)
-            if self._disp is None:
-                self._disp = torch.zeros((C, nb), dtype=torch.float32, device=x.device)
-            if self._disp2 is None:
-                self._disp2 = torch.zeros((C, nb), dtype=torch.float32, device=x.device)
-            db = torch.empty((C, nb), dtype=torch.float32, device=x.device)
-            imax = torch.empty(C, dtype=torch.int32, device=x.device)
-            ipitch = torch.empty(C, dtype=torch.int32, device=x.device)
-            # power [2C, nf, nb]: pair c's reference at row 2c, its measurement at row 2c + 1
-            p1 = power.data_ptr() if nf else 0
-            p2 = p1 + 4 * nf * nb if nf else 0
-            self.proc.handle.call("frt_spectrum_reduce_dual", _lib._ptr(p1), _lib._ptr(p2),
-                                  int(2 * nf * nb), int(nb), int(C), int(nf), int(nb),
-                                  c_float(self.alpha), _lib._ptr(self._disp), _lib._ptr(self._disp2),
-                                  _lib._ptr(db), _lib._ptr(imax), _lib._ptr(ipitch), sp)
-            return self._indices_to_hz(db, imax, ipitch)
+        return fmax, fpitch

@@ -385,7 +385,7 @@ def ticks_args(C=2, nb=513, g=2, R=3, alpha=0.5, dual=False):
 
 SINGLE_BAD = {"channels": (3, -1), "frames_per_tick 0": (4, 0), "frames_per_tick 8193": (4, 8193),
               "ticks": (5, -1), "bins": (6, 2), "alpha 0": (7, c_float(0.0)), "alpha > 1": (7, c_float(1.5)),
-              "power": (0, None), "disp": (8, None), "fmax": (11, None), "pitch": (12, None),
+              "alpha < 0": (7, c_float(-0.5)), "alpha NaN": (7, c_float(float("nan"))), "power": (0, None), "disp": (8, None), "fmax": (11, None), "pitch": (12, None),
               "bins too large": (6, 60000)}
 DUAL_BAD = {"pairs": (4, -1), "frames_per_tick 0": (5, 0), "frames_per_tick 8193": (5, 8193),
             "ticks": (6, -1), "bins": (7, 2), "alpha": (8, c_float(-0.1)), "power1": (0, None),
