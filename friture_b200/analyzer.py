@@ -19,17 +19,7 @@ import numpy as np
 from . import _lib
 from ._lib import Handle
 from .audioproc import audioproc, frame_count
-from .octavefilters import Octave_Filters
-
-
-def bank_block_ok(block, n_octaves):
-    """Whether the filterbank kernels can run blocks of ``block`` samples with ``n_octaves`` octaves
-    (csrc/bank.cu, frt_bank_check_block): a multiple of 256 samples, and the longest of the 1024, 512
-    and 256-sample tiles that divides it still even at the last of the halving stages."""
-    if block <= 0 or block % 256:
-        return False
-    tile = next(t for t in (1024, 512, 256) if block % t == 0)
-    return (tile >> (n_octaves - 1)) >= 1
+from .octavefilters import Octave_Filters, bank_block_ok, check_bank_block  # noqa: F401 (bank_block_ok: kept importable from here)
 
 
 class ChannelAnalyzer:
@@ -40,10 +30,7 @@ class ChannelAnalyzer:
         self.handle = Handle(self.device.index)
         self.n_channels = int(n_channels)
         self.fft_size, self.hop = int(fft_size), int(hop)
-        if not bank_block_ok(self.hop, n_octaves):
-            raise ValueError("hop %d is not a filterbank block for %d octaves: it must be a multiple of 256 "
-                             "samples whose longest tile of 1024, 512 or 256 that divides it holds %d samples"
-                             % (self.hop, n_octaves, 1 << (n_octaves - 1)))
+        check_bank_block(self.hop, n_octaves)   # the hop is the filterbank's block
         self.nbins = self.fft_size // 2 + 1
         self.proc = audioproc(self.handle)
         self.proc.set_fftsize(self.fft_size)

@@ -674,47 +674,111 @@ extern "C" int frt_bank_set_state(frt_handle h, const float *z_host, const float
     return FRT_OK;
 }
 
-template <int L0, bool WANT_Y>
-static int launch_bank3(frt_handle h, const BankPlan *pl, const BankArgs &a, cudaStream_t st) {
+// How blocks of `block` samples run for a plan: refused (`why`), or the kernel family and variant.
+struct BankRoute {
+    const char *why;
+    enum Kind { PIPE, SCAN, SCAN3 } kind;
+    int L0;            // samples per lane of the chunk-scan kernels' 32 * L0-sample tile
+    int logch, pack;   // PIPE: 2^logch-sample steps, channels per lane
+};
+
+// The one statement of the filterbank's block rule and kernel choice.  It depends on the plan, the
+// block and whether band outputs are wanted, not on how a stream is cut: the bits are the same.
+static BankRoute bank_route(const BankPlan *pl, int block, bool want_y) {
     const BankParams &P = pl->params;
-    const size_t smem = sizeof(float) * ((size_t)P.nsec * 8 + pl->nz + pl->ne + 32 * L0 + 64);
-    return frt_launch(h, bank_kernel3<L0, WANT_Y>, (unsigned)a.n_channels, 96, smem, st, P, a);
+    // blocks stay even-length at every stage (decimate.py:41 restarts the [::2] phase on every call),
+    // down to the chunk-scan kernels' tile: the longest of 1024, 512 and 256 samples dividing the block
+    if (block <= 0 || block % 256) return {"block must be a multiple of 256 samples"};
+    const int tile = block % 1024 == 0 ? 1024 : block % 512 == 0 ? 512 : 256;
+    if ((tile >> (P.n_oct - 1)) < 1) return {"block too short for this many octaves"};
+    const int L0 = tile / 32;
+    // The lane-pipelined kernel (bank_pipe.cu) is the fast path for the fused energies of 1- and
+    // 1/3-octave banks (pipe_ok): 64-sample steps up to 3072 channels, above that 32-sample steps with
+    // two channels per lane.  64-sample steps start at 512-sample blocks: a 256-sample block is four
+    // such steps, and its band energies would need 9 slots of the 8-slot ring at 10 octaves.
+    if (pl->pipe_ok && !want_y && (block & (block - 1)) == 0) {
+        const int pack = pl->n_channels > 3072 ? 2 : 1;
+        const int logch = (pack == 1 && block >= PIPE_MIN_BLOCK[1]) ? 6 : 5;
+        return {nullptr, BankRoute::PIPE, L0, logch, pack};
+    }
+    // Chunk-scan kernels: three warps per channel below 1536 channels (latency-bound); above, one warp
+    // per channel saturates the schedulers with less synchronisation.  The three-warp kernel, compiled
+    // for L0 <= 16, runs all log2(L0) scan-mode stages, so it needs more octaves than that.
+    const bool three = L0 <= 16 && L0 < (1 << P.n_oct) && pl->n_channels < 1536;
+    return {nullptr, three ? BankRoute::SCAN3 : BankRoute::SCAN, L0};
 }
 
-template <int L0, bool WANT_Y>
-static int launch_bank_y(frt_handle h, const BankPlan *pl, const BankArgs &a, cudaStream_t st) {
-    // few channels: three warps per channel (latency-bound regime); many channels: one warp
-    // per channel already saturates the schedulers with less synchronisation
-    // the three-warp kernel runs all log2(L0) scan-mode stages unconditionally: it needs more
-    // octaves than that (always true for the 9- and 10-octave banks of the reference)
-    if constexpr (L0 <= 16) {
-        if (pl->params.n_oct > Log2<L0>::v && a.n_channels < 1536) return launch_bank3<L0, WANT_Y>(h, pl, a, st);
-    }
+int frt_bank_check_block(frt_ctx *h, const BankPlan *pl, int block) {
+    const char *why = bank_route(pl, block, false).why;
+    return why ? frt_fail(h, FRT_EINVAL, "%s (block %d)", why, block) : FRT_OK;
+}
+
+// one warp per channel, two channels per CTA
+template <int L0>
+static int launch_scan(frt_handle h, const BankPlan *pl, const BankArgs &a, cudaStream_t st) {
     const BankParams &P = pl->params;
     const int warps = 2;
     const size_t smem = sizeof(float) * ((size_t)P.nsec * 8 + (size_t)warps * (pl->nz + pl->ne));
     const unsigned blocks = (unsigned)((a.n_channels + warps - 1) / warps);
-    return frt_launch(h, bank_kernel<L0, WANT_Y>, blocks, warps * 32, smem, st, P, a);
+    return frt_launch(h, a.y ? bank_kernel<L0, true> : bank_kernel<L0, false>, blocks, warps * 32, smem, st, P, a);
 }
 
+// one CTA of three warps per channel
 template <int L0>
-static int launch_bank(frt_handle h, const BankPlan *pl, const BankArgs &a, cudaStream_t st) {
-    return a.y ? launch_bank_y<L0, true>(h, pl, a, st) : launch_bank_y<L0, false>(h, pl, a, st);
+static int launch_scan3(frt_handle h, const BankPlan *pl, const BankArgs &a, cudaStream_t st) {
+    const BankParams &P = pl->params;
+    const size_t smem = sizeof(float) * ((size_t)P.nsec * 8 + pl->nz + pl->ne + 32 * L0 + 64);
+    const auto kernel = a.y ? bank_kernel3<L0, true> : bank_kernel3<L0, false>;
+    return frt_launch(h, kernel, (unsigned)a.n_channels, 96, smem, st, P, a);
 }
 
 static int bank_process_impl(frt_handle h, const float *x_dev, int64_t x_stride, int block,
                              int n_blocks, float *energies_dev, int64_t e_stride, float *y_dev,
-                             int64_t y_stride, int db, void *stream);
-
-// the chunk-scan kernels' tile: the longest of 1024, 512 and 256 samples that divides the block
-static int bank_tile(int block) { return (block % 1024 == 0) ? 1024 : ((block % 512 == 0) ? 512 : 256); }
-
-int frt_bank_check_block(frt_ctx *h, const BankPlan *pl, int block) {
-    // blocks must stay even-length at every stage (decimate.py:41 restarts the [::2] phase
-    // on every call), i.e. block % 2^(n_oct-1) == 0; the kernel tiles are 256/512/1024
-    FRT_CHECK_ARG(h, block > 0 && block % 256 == 0, "block must be a multiple of 256 samples");
-    FRT_CHECK_ARG(h, (bank_tile(block) >> (pl->params.n_oct - 1)) >= 1, "block too short for this many octaves");
-    return FRT_OK;
+                             int64_t y_stride, int db, void *stream) {
+    if (!h) return FRT_EINVAL;
+    if (!h->bank) return frt_fail(h, FRT_ESTATE, "frt_bank_process: call frt_bank_plan first");
+    DeviceGuard g(h->device);
+    BankPlan *pl = h->bank.get();
+    const BankParams &P = pl->params;
+    FRT_CHECK_ARG(h, n_blocks >= 0 && block >= 0, "negative shape");
+    if (n_blocks == 0 || block == 0) return FRT_OK;   // empty chunk: octavespectrum.py:94-95
+    const BankRoute r = bank_route(pl, block, y_dev != nullptr);
+    if (r.why) return frt_fail(h, FRT_EINVAL, "%s (block %d)", r.why, block);
+    FRT_CHECK_ARG(h, x_dev != nullptr, "x_dev is NULL");
+    FRT_CHECK_ARG(h, x_stride >= (int64_t)block * n_blocks, "x_stride too small");
+    const long long t_total = (long long)block * n_blocks;
+    if (y_dev) {
+        long long need = 0;
+        for (int j = 0; j < P.n_oct; j++) need += (long long)P.bpo * (t_total >> j);
+        FRT_CHECK_ARG(h, y_stride >= need, "y_stride smaller than the ragged output size");
+    }
+    BankArgs a;
+    a.x = x_dev;
+    a.x_stride = x_stride;
+    a.n_channels = pl->n_channels;
+    a.n_tiles = (int)(t_total / (32 * r.L0));
+    a.tiles_per_block = block / (32 * r.L0);
+    a.zstate = pl->zstate.get();
+    a.ema = pl->ema.get();
+    a.energies = energies_dev;
+    a.e_stride = e_stride;
+    a.y = y_dev;
+    a.y_stride = y_stride;
+    a.t_total = t_total;
+    a.db = db;
+    a.vec_ok = (((uintptr_t)x_dev & 15) == 0) && ((x_stride & 3) == 0);
+    a.weight = db ? pl->weight.get() : nullptr;
+    a.block = block;
+    a.n_blocks = n_blocks;
+    a.n_steps = 0;
+    cudaStream_t st = (cudaStream_t)stream;
+    switch (r.kind) {
+    case BankRoute::PIPE: return frt_pipe_launch(h, pl, a, r.logch, r.pack, st);
+    case BankRoute::SCAN3: return r.L0 == 16 ? launch_scan3<16>(h, pl, a, st) : launch_scan3<8>(h, pl, a, st);
+    default:
+        return r.L0 == 32 ? launch_scan<32>(h, pl, a, st)
+             : r.L0 == 16 ? launch_scan<16>(h, pl, a, st) : launch_scan<8>(h, pl, a, st);
+    }
 }
 
 extern "C" int frt_bank_process(frt_handle h, const float *x_dev, int64_t x_stride, int block,
@@ -737,65 +801,6 @@ extern "C" int frt_bank_process_strided(frt_handle h, const float *x_dev, int64_
     }
     return bank_process_impl(h, x_dev, x_stride, block, n_blocks, energies_dev, e_stride_c, nullptr, 0, db,
                              stream);
-}
-
-static int bank_process_impl(frt_handle h, const float *x_dev, int64_t x_stride, int block,
-                             int n_blocks, float *energies_dev, int64_t e_stride, float *y_dev,
-                             int64_t y_stride, int db, void *stream) {
-    if (!h) return FRT_EINVAL;
-    if (!h->bank) return frt_fail(h, FRT_ESTATE, "frt_bank_process: call frt_bank_plan first");
-    DeviceGuard g(h->device);
-    BankPlan *pl = h->bank.get();
-    const BankParams &P = pl->params;
-    FRT_CHECK_ARG(h, n_blocks >= 0 && block >= 0, "negative shape");
-    if (n_blocks == 0 || block == 0) return FRT_OK;   // empty chunk: octavespectrum.py:94-95
-    if (const int rc = frt_bank_check_block(h, pl, block)) return rc;
-    FRT_CHECK_ARG(h, x_dev != nullptr, "x_dev is NULL");
-    FRT_CHECK_ARG(h, x_stride >= (int64_t)block * n_blocks, "x_stride too small");
-    const int tile = bank_tile(block);
-    const long long t_total = (long long)block * n_blocks;
-    if (y_dev) {
-        long long need = 0;
-        for (int j = 0; j < P.n_oct; j++) need += (long long)P.bpo * (t_total >> j);
-        FRT_CHECK_ARG(h, y_stride >= need, "y_stride smaller than the ragged output size");
-    }
-    BankArgs a;
-    a.x = x_dev;
-    a.x_stride = x_stride;
-    a.n_channels = pl->n_channels;
-    a.n_tiles = (int)(t_total / tile);
-    a.tiles_per_block = block / tile;
-    a.zstate = pl->zstate.get();
-    a.ema = pl->ema.get();
-    a.energies = energies_dev;
-    a.e_stride = e_stride;
-    a.y = y_dev;
-    a.y_stride = y_stride;
-    a.t_total = t_total;
-    a.db = db;
-    a.vec_ok = (((uintptr_t)x_dev & 15) == 0) && ((x_stride & 3) == 0);
-    a.weight = db ? pl->weight.get() : nullptr;
-    a.block = block;
-    a.n_blocks = n_blocks;
-    a.n_steps = 0;
-    cudaStream_t st = (cudaStream_t)stream;
-    // Kernel choice.  The lane-pipelined kernel (bank_pipe.cu) computes every section sample once
-    // and is the fast path for the fused energies of 1- and 1/3-octave banks; the chunk-scan
-    // kernels below serve the ragged band outputs (`.filter()`), 6/12/24 bands per octave and
-    // block lengths that are not a power of two.
-    const bool pow2 = (block & (block - 1)) == 0;
-    if (pl->pipe_ok && !y_dev && pow2 && (block >> (P.n_oct - 1)) >= 1) {
-        // 64-sample steps up to 3072 channels (32-sample steps for 256-sample blocks), above that
-        // 32-sample steps with two channels per lane (two independent recurrences per lane once the
-        // schedulers are full).  The choice depends on the plan and the block length only, so a
-        // stream gives the same bits however it is cut into launches.
-        const int pack = pl->n_channels > 3072 ? 2 : 1;
-        const int logch = (block >= 512 && pack == 1) ? 6 : 5;
-        return frt_pipe_launch(h, pl, a, logch, pack, st);
-    }
-    if (tile == 1024) return launch_bank<32>(h, pl, a, st);
-    if (tile == 512) return launch_bank<16>(h, pl, a, st);
-    return launch_bank<8>(h, pl, a, st);
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -31,6 +31,7 @@ struct BankParams {
 constexpr int PIPE_MAX_SEC = 16;    // 2*bpo + 6 <= 16: bpo in {1, 3}
 constexpr int PIPE_RX = 8;          // input ring depth (chunks)
 constexpr int PIPE_PF = 4;          // prefetch distance (chunks)
+constexpr int PIPE_MIN_BLOCK[2] = {256, 512};   // [logch - 5]: shortest block bank_route runs in such steps
 
 struct PipeParams {
     float na1[PIPE_MAX_SEC], na2[PIPE_MAX_SEC];   // per section: -a1, -a2
@@ -72,7 +73,7 @@ struct BankArgs {
 struct BankPlan {
     BankParams params;
     PipeParams pipe[2];    // [logch - 5]: 32 / 64-sample steps
-    bool pipe_ok = false;  // the lane-pipelined kernel supports this bank
+    bool pipe_ok = false;  // the lane-pipelined kernel can run this bank's blocks (frt_pipe_prepare)
     int n_channels = 0;
     DeviceArray<float> zstate, ema;
     DeviceArray<float> weight;   // device copy of the dB weighting vector, or empty
@@ -80,8 +81,8 @@ struct BankPlan {
     double alphas[BANK_MAX_OCT];
 };
 
-// bank.cu: FRT_EINVAL (with the handle's error message) unless every filterbank kernel can run
-// blocks of `block` samples for this plan; the filterbank and combined entry points refuse such a
+// bank.cu: FRT_EINVAL (with the handle's error message) when the filterbank refuses blocks of
+// `block` samples for this plan (bank_route); the filterbank and combined entry points refuse such a
 // block before they queue anything
 int frt_bank_check_block(frt_ctx *h, const BankPlan *pl, int block);
 
@@ -89,5 +90,4 @@ int frt_bank_check_block(frt_ctx *h, const BankPlan *pl, int block);
 void frt_pipe_prepare(BankPlan *pl);
 void frt_pipe_schedule(int n_oct, int logch, long long t_total, int *T /*[BANK_MAX_OCT+1]*/, int *n_steps);
 int frt_pipe_flush_delta(int n_oct, int logch, const int *T);
-bool frt_pipe_supported(const BankPlan *pl, int block, int logch);
 int frt_pipe_launch(frt_ctx *h, const BankPlan *pl, BankArgs a, int logch, int pack, cudaStream_t st);

@@ -109,7 +109,7 @@ __device__ __forceinline__ void st2(float2 *p, float2 a, float2 b) {
 
 // blocks of band energies staged in shared memory before the flush: a block's vector leaves fdelta
 // steps after its last stage-0 chunk, meanwhile stage 0 keeps staging newer blocks
-// (frt_pipe_supported checks that the ring is deep enough for the block length)
+// (frt_pipe_prepare checks that the ring is deep enough for the blocks bank_route gives the kernel)
 constexpr int EN_RING = 8;
 
 // The two lane groups of a half-warp must run ONE instruction stream with per-lane predicates.
@@ -743,6 +743,9 @@ int frt_pipe_flush_delta(int n_oct, int logch, const int *T) {
     return delta;
 }
 
+// Builds the kernel's tables and sets pl->pipe_ok for bank_route: the kernel is compiled for 1 and 3
+// bands per octave, and its energy ring must hold the shortest block bank_route runs at each step size
+// (longer blocks of the same steps stage fewer); other banks run the chunk-scan kernels.
 void frt_pipe_prepare(BankPlan *pl) {
     const BankParams &B = pl->params;
     pl->pipe_ok = (B.bpo == 1 || B.bpo == 3);
@@ -763,6 +766,10 @@ void frt_pipe_prepare(BankPlan *pl) {
         for (int j = 0; j <= BANK_MAX_OCT; j++) P.alpha[j] = j < B.n_oct ? (float)pl->alphas[j] : 1.f;
         frt_pipe_schedule(B.n_oct, logch, 0, P.T, nullptr);
         P.fdelta = frt_pipe_flush_delta(B.n_oct, logch, P.T);
+        // blocks staged but not yet flushed when a block's vector leaves, plus the one being written
+        // (+1: the section loops of the next step already stage energies while a block is flushed)
+        const int nb = PIPE_MIN_BLOCK[v] >> logch;      // steps per block
+        if ((P.fdelta + nb - 1) / nb + 2 > EN_RING) pl->pipe_ok = false;
         const double q0 = 1.0 - pl->alphas[0];
         P.aq0 = (float)(1.0 - pow(q0, CH));
         for (int p = 0; p < CH; p++) {
@@ -779,21 +786,8 @@ void frt_pipe_prepare(BankPlan *pl) {
     }
 }
 
-bool frt_pipe_supported(const BankPlan *pl, int block, int logch) {
-    if (!pl->pipe_ok || (block & (block - 1)) || block < (4 << logch)) return false;
-    const PipeParams &P = pl->pipe[logch - 5];
-    if ((block >> (P.n_oct - 1)) < 1) return false;
-    const int nb = block >> logch;                      // steps per block
-    // blocks staged but not yet flushed when a block's vector leaves, plus the one being written
-    // (+1: the section loops of the next step already stage energies while a block is flushed)
-    return (P.fdelta + nb - 1) / nb + 2 <= EN_RING;
-}
-
+// Runs the variant bank_route chose; two channels per lane run 32-sample steps only.
 int frt_pipe_launch(frt_ctx *h, const BankPlan *pl, BankArgs a, int logch, int pack, cudaStream_t st) {
-    // two channels per lane run 32-sample steps only
-    if (!frt_pipe_supported(pl, a.block, logch) || (pack == 2 && logch != 5))
-        return frt_fail(h, FRT_EINVAL, "the pipelined filterbank kernel has no %d-sample steps with %d channels "
-                        "per lane for %d-sample blocks", 1 << logch, pack, a.block);
     const PipeParams &P = pl->pipe[logch - 5];
     int T[BANK_MAX_OCT + 1];
     frt_pipe_schedule(P.n_oct, logch, a.t_total, T, &a.n_steps);

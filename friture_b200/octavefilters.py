@@ -53,6 +53,25 @@ def smoothing_alphas(response_time, n_octaves=NOCTAVE, fs=SAMPLING_RATE):
                      for j in range(n_octaves)], dtype=np.float64)
 
 
+def bank_block_ok(block, n_octaves):
+    """Whether the IIR filterbank takes blocks of ``block`` samples with ``n_octaves`` octaves
+    (csrc/bank.cu, bank_route): a multiple of 256 samples, and the longest of the 1024, 512 and
+    256-sample tiles that divides it still even at the last of the halving stages."""
+    if block <= 0 or block % 256:
+        return False
+    tile = next(t for t in (1024, 512, 256) if block % t == 0)
+    return (tile >> (n_octaves - 1)) >= 1
+
+
+def check_bank_block(block, n_octaves):
+    """ValueError unless the IIR filterbank takes blocks of ``block`` samples (bank_block_ok)."""
+    if not bank_block_ok(block, n_octaves):
+        raise ValueError("the filterbank takes no %d-sample blocks at %d octaves: a block must be a multiple "
+                         "of 256 samples whose longest tile of 1024, 512 or 256 that divides it holds at least "
+                         "%d samples (every decimation stage needs an even length, friture/signal/decimate.py:41)"
+                         % (block, n_octaves, 1 << (n_octaves - 1)))
+
+
 def ragged_layout(n_samples, bpo, n_octaves=NOCTAVE):
     """(offsets, lengths) of the bands in the kernel's concatenated y layout, band k = 0..nbands-1
     (k = (n_octaves-1-j)*bpo + i, friture/filter.py:104-109)."""
@@ -249,9 +268,7 @@ class Octave_Filters():
             raise Exception("Filter input is too small")
         if block <= 0 or T % block != 0:
             raise ValueError("T must be a whole number of blocks")
-        if block % 256 != 0 or (block >> (self._n_octaves - 1)) < 1:
-            raise ValueError("block must be a multiple of 256 samples (every decimation stage "
-                             "needs an even length, friture/signal/decimate.py:41)")
+        check_bank_block(block, self._n_octaves)
         if energies and block > MAX_BLOCK:
             raise ValueError("block > %d: the reference's smoothing kernel is shorter than the "
                              "block (exp_smoothing.py:43-47)" % MAX_BLOCK)

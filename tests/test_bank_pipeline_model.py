@@ -12,6 +12,7 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 from bank_pipeline_model import PipeModel, flush_delta, n_steps_for, stage_start_steps  # noqa: E402
 
 EN_RING = 8   # staged band-energy blocks per channel slot (bank_pipe.cu)
+PIPE_MIN_BLOCK = {5: 256, 6: 512}   # logch -> shortest block bank_route runs in such steps (bank_internal.cuh)
 
 
 def _oracle_energies(bpo, n_oct, block, x, response_time=1.0):
@@ -53,19 +54,29 @@ def test_schedule_model_streaming_and_state():
     assert np.max(np.abs(got - E) / np.max(np.abs(E), axis=-1, keepdims=True)) < 1e-10
 
 
+def ring_slots(n_oct, logch, block):
+    """Energy-ring slots a block needs: a block's vector leaves flush_delta steps after its last chunk,
+    and the blocks staged meanwhile plus the one being written must fit (frt_pipe_prepare)."""
+    fdelta = flush_delta(n_oct, logch, stage_start_steps(n_oct, logch))
+    nb = block >> logch
+    return (fdelta + nb - 1) // nb + 2
+
+
 def test_energy_ring_holds_every_supported_block():
-    """frt_pipe_supported's ring condition holds for every power-of-two block the pipelined kernel
-    accepts, at both step lengths and every octave count, so the library needs no fallback to shorter
-    steps: a block's vector leaves flush_delta steps after its last chunk, and the blocks staged
-    meanwhile plus the one being written fit in the ring."""
+    """The ring holds the shortest block bank_route gives each step size at every octave count, so
+    frt_pipe_prepare never turns the pipelined kernel off for a bank the library plans; longer
+    power-of-two blocks need no more slots, which is why it checks the shortest only."""
     for n_oct in range(1, 11):
-        for logch in (5, 6):
-            fdelta = flush_delta(n_oct, logch, stage_start_steps(n_oct, logch))
-            for block in (1 << b for b in range(8, 17)):
-                if block < (4 << logch) or (block >> (n_oct - 1)) < 1:
-                    continue
-                nb = block >> logch
-                assert (fdelta + nb - 1) // nb + 2 <= EN_RING, (n_oct, logch, block, fdelta)
+        for logch, shortest in PIPE_MIN_BLOCK.items():
+            need = ring_slots(n_oct, logch, shortest)
+            assert need <= EN_RING, (n_oct, logch, shortest, need)
+            for block in (shortest << b for b in range(1, 9)):
+                assert ring_slots(n_oct, logch, block) <= need, (n_oct, logch, block)
+    assert max(ring_slots(n_oct, 6, 512) for n_oct in range(1, 11)) == 6
+    # 256-sample blocks in 64-sample steps, which bank_route does not take, would fill the ring at 9
+    # octaves and overflow it at 10 (where the block rule refuses 256-sample blocks anyway)
+    assert [ring_slots(n_oct, 6, 256) for n_oct in (8, 9, 10)] == [8, 8, 9]
+    assert all(ring_slots(n_oct, 6, 256) <= EN_RING for n_oct in range(1, 10))
 
 
 def test_library_schedule_matches_model():

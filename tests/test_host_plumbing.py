@@ -101,6 +101,23 @@ def on_cuda(t, index=0):
     return t.as_subclass(cls)
 
 
+def test_filter_batch_refuses_a_block_the_bank_refuses_before_any_call():
+    """768 samples pass the old weaker check at 10 octaves; the bank's own rule refuses them, with the
+    same message ChannelAnalyzer gives, before any plan or launch."""
+    from friture_b200.octavefilters import Octave_Filters
+
+    class NoCalls(StandInHandle):
+        def call(self, *args):
+            raise AssertionError("library called for a refused block: %s" % (args,))
+
+    for mode in ("iir", "fft"):
+        bank = Octave_Filters(3, n_octaves=10, handle=NoCalls(), mode=mode)
+        for block in (768, 384, 256):
+            with pytest.raises(ValueError, match="no %d-sample blocks at 10 octaves" % block):
+                bank.filter_batch(on_cuda(torch.zeros((2, 4 * block))), block, energies=mode == "iir",
+                                  want_y=mode == "fft")
+
+
 def test_device_rows_accepts_and_gives_the_row_stride():
     T = 1000
     for x, C, stride in [(torch.zeros((3, T)), 3, T), (torch.zeros((3, 2 * T))[:, :T], 3, 2 * T),
