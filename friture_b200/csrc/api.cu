@@ -76,9 +76,7 @@ extern "C" int frt_host_alloc(frt_handle h, size_t bytes, void **out) {
     if (!h || !out) return frt_fail(h, FRT_EINVAL, "frt_host_alloc: NULL argument");
     DeviceGuard g(h->device);
     *out = nullptr;
-    cudaError_t e = cudaHostAlloc(out, bytes ? bytes : 1, cudaHostAllocPortable);
-    if (e != cudaSuccess)
-        return frt_fail(h, FRT_ENOMEM, "cudaHostAlloc(%zu): %s", bytes, cudaGetErrorString(e));
+    FRT_CUDA(h, frt_alloc_status(cudaHostAlloc(out, bytes ? bytes : 1, cudaHostAllocPortable), bytes));
     return FRT_OK;
 }
 
@@ -99,8 +97,7 @@ extern "C" int frt_peer_alloc(frt_handle h, size_t bytes, void **out) {
     if (!h || !out) return frt_fail(h, FRT_EINVAL, "frt_peer_alloc: NULL argument");
     DeviceGuard g(h->device);
     *out = nullptr;
-    cudaError_t e = cudaMalloc(out, bytes ? bytes : 1);
-    if (e != cudaSuccess) return frt_fail(h, FRT_ENOMEM, "cudaMalloc(%zu): %s", bytes, cudaGetErrorString(e));
+    FRT_CUDA(h, frt_malloc(out, bytes ? bytes : 1));
     return FRT_OK;
 }
 

@@ -106,9 +106,7 @@ extern "C" int frt_combined_process_host(frt_handle h, const float *x_host, int6
     for (const cudaStream_t s : {p.s_out.get(), p.s_cmp.get(), p.s_in.get()}) {
         if (!s) continue;
         const cudaError_t e = cudaStreamSynchronize(s);
-        if (rc == FRT_OK && e != cudaSuccess)
-            rc = frt_fail(h, FRT_ECUDA, "cudaStreamSynchronize failed: %s (%s:%d)", cudaGetErrorString(e),
-                          __FILE__, __LINE__);
+        if (rc == FRT_OK && e != cudaSuccess) rc = frt_cuda_fail(h, e, "cudaStreamSynchronize", __FILE__, __LINE__);
     }
     return rc;
 }

@@ -44,6 +44,18 @@ inline cudaError_t frt_sync_zero(void *dst, size_t bytes) {
     return e;
 }
 
+// Every allocation's status passes through here.  The runtime may also keep a failure as its last
+// error, which would fail the next launch's check (frt_launch): clear it, and keep its size for FRT_CUDA.
+inline thread_local size_t frt_refused_bytes = 0;
+inline cudaError_t frt_alloc_status(cudaError_t e, size_t bytes) {
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        frt_refused_bytes = bytes;
+    }
+    return e;
+}
+inline cudaError_t frt_malloc(void **p, size_t bytes) { return frt_alloc_status(cudaMalloc(p, bytes), bytes); }
+
 // One cudaMalloc allocation of n elements of T, or none.  Move-only.
 template <class T>
 struct DeviceArray {
@@ -55,7 +67,7 @@ struct DeviceArray {
         p.reset();
         n = 0;
         T *d = nullptr;
-        cudaError_t e = cudaMalloc(&d, sizeof(T) * count);
+        cudaError_t e = frt_malloc((void **)&d, sizeof(T) * count);
         if (e != cudaSuccess) return e;
         p.reset(d);
         n = count;
@@ -69,6 +81,20 @@ struct DeviceArray {
     // staging: reallocates only when a call needs more than it holds, so steady-state calls do not
     cudaError_t grow(size_t count) { return count <= n ? cudaSuccess : alloc(count); }
 };
+
+// The regions of a grow-only workspace, in order, each rounded up to 256 bytes: add returns a region's
+// offset, and `bytes` is the size to grow the workspace to.
+struct WsLayout {
+    size_t bytes = 0;
+    static size_t round(size_t region) { return (region + 255) & ~size_t(255); }
+    size_t add(size_t region) { return std::exchange(bytes, bytes + round(region)); }
+};
+
+// How many items of per_item bytes a group of a call holds within `budget`: at least one, at most n.
+inline size_t frt_group_size(size_t budget, size_t per_item, size_t n) {
+    const size_t g = budget / per_item;
+    return g < 1 ? 1 : g > n ? n : g;
+}
 
 struct Stream {   // non-blocking
     std::unique_ptr<CUstream_st, StreamDestroy> s;
@@ -200,12 +226,19 @@ struct frt_ctx {
 
 int frt_fail(frt_ctx *h, int code, const char *fmt, ...);
 
+// FRT_CUDA's failure: FRT_ENOMEM when memory ran out, else FRT_ECUDA; a refused allocation's size.
+inline int frt_cuda_fail(frt_ctx *h, cudaError_t e, const char *call, const char *file, int line) {
+    const int code = e == cudaErrorMemoryAllocation ? FRT_ENOMEM : FRT_ECUDA;
+    if (const size_t bytes = std::exchange(frt_refused_bytes, 0))
+        return frt_fail(h, code, "%s failed: %s, %zu bytes asked for (%s:%d)", call, cudaGetErrorString(e), bytes,
+                        file, line);
+    return frt_fail(h, code, "%s failed: %s (%s:%d)", call, cudaGetErrorString(e), file, line);
+}
+
 #define FRT_CUDA(h, call)                                                                  \
     do {                                                                                   \
         cudaError_t e__ = (call);                                                          \
-        if (e__ != cudaSuccess)                                                            \
-            return frt_fail((h), FRT_ECUDA, "%s failed: %s (%s:%d)", #call,                \
-                            cudaGetErrorString(e__), __FILE__, __LINE__);                  \
+        if (e__ != cudaSuccess) return frt_cuda_fail((h), e__, #call, __FILE__, __LINE__); \
     } while (0)
 
 #define FRT_CHECK_ARG(h, cond, msg)                                                        \

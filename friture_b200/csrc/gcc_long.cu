@@ -577,15 +577,13 @@ static int gl_setup(frt_ctx *h, const GccLongPlan *pl, int n_pairs, int64_t stri
                     int &group) {
     const size_t M = size_t(1) << (pl->log1 + pl->log2), H = size_t(pl->Lp / 2 + 1);
     const int n_chunks = (pl->L + GL_STATS_CHUNK - 1) / GL_STATS_CHUNK;
-    auto up = [](size_t b) { return (b + 255) & ~size_t(255); };
-    const size_t per_pair = up(M * sizeof(float2)) + up(H * sizeof(float2)) + up(n_chunks * 6 * sizeof(float)) +
-                            up(sizeof(PairState));
-    size_t gr = GL_WORKSPACE_BUDGET / per_pair;
-    gr = gr < 1 ? 1 : gr > (size_t)GL_MAX_GROUP ? (size_t)GL_MAX_GROUP : gr;
-    gr = gr > (size_t)n_pairs ? (size_t)n_pairs : gr;
-    const size_t o_g = up(gr * M * sizeof(float2)), o_part = o_g + up(gr * H * sizeof(float2)),
-                 o_st = o_part + up(gr * n_chunks * 6 * sizeof(float)), bytes = o_st + gr * sizeof(PairState);
-    FRT_CUDA(h, h->gcc_long_ws.grow(bytes));
+    const size_t per_pair = WsLayout::round(M * sizeof(float2)) + WsLayout::round(H * sizeof(float2)) +
+                            WsLayout::round(n_chunks * 6 * sizeof(float)) + WsLayout::round(sizeof(PairState));
+    const size_t gr = frt_group_size(GL_WORKSPACE_BUDGET, per_pair, std::min(GL_MAX_GROUP, n_pairs));
+    WsLayout l;
+    const size_t o_buf = l.add(gr * M * sizeof(float2)), o_g = l.add(gr * H * sizeof(float2)),
+                 o_part = l.add(gr * n_chunks * 6 * sizeof(float)), o_st = l.add(gr * sizeof(PairState));
+    FRT_CUDA(h, h->gcc_long_ws.grow(l.bytes));
     unsigned char *ws = h->gcc_long_ws.get();
     group = (int)gr;
 
@@ -603,7 +601,7 @@ static int gl_setup(frt_ctx *h, const GccLongPlan *pl, int n_pairs, int64_t stri
     a.tw_sub = pl->tw_sub.get();
     a.tw_lo = pl->tw_lo.get();
     a.tw_hi = pl->tw_hi.get();
-    a.buf = (float2 *)ws;
+    a.buf = (float2 *)(ws + o_buf);
     a.g = (float2 *)(ws + o_g);
     a.part = (float *)(ws + o_part);
     a.st = (PairState *)(ws + o_st);

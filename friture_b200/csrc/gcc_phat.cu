@@ -844,19 +844,13 @@ extern "C" int frt_gcc_set_pairs(frt_handle h, int n_channels, const int *pairs_
     return FRT_OK;
 }
 
-// The spectrum workspace of frt_gcc_phat_pairs: [C][H] float2 spectra and [C] int flags.  Grow-only; a
-// failed allocation is FRT_ENOMEM and leaves the handle usable.
+// The spectrum workspace of frt_gcc_phat_pairs: [C][H] float2 spectra and [C] int flags.  Grow-only.
 static int gcc_spectra_workspace(frt_ctx *h, int H, GccSpectra &w) {
     const size_t C = (size_t)h->gcc_pairs_channels;
-    auto up = [](size_t b) { return (b + 255) & ~size_t(255); };
-    const size_t o_quiet = up(C * H * sizeof(float2)), bytes = o_quiet + up(C * sizeof(int));
-    const cudaError_t e = h->gcc_spec_ws.grow(bytes);
-    if (e == cudaErrorMemoryAllocation) {
-        cudaGetLastError();
-        return frt_fail(h, FRT_ENOMEM, "the spectra of %zu channels (%zu bytes) do not fit", C, bytes);
-    }
-    FRT_CUDA(h, e);
-    w.spec = (float2 *)h->gcc_spec_ws.get();
+    WsLayout l;
+    const size_t o_spec = l.add(C * H * sizeof(float2)), o_quiet = l.add(C * sizeof(int));
+    FRT_CUDA(h, h->gcc_spec_ws.grow(l.bytes));
+    w.spec = (float2 *)(h->gcc_spec_ws.get() + o_spec);
     w.quiet = (int *)(h->gcc_spec_ws.get() + o_quiet);
     return FRT_OK;
 }
@@ -917,32 +911,25 @@ constexpr size_t GCC_TRACK_BUDGET = size_t(2) << 30;
 
 // The workspace of a frames call, grow-only: groups of `group` frames of n_pairs rows of Lr samples,
 // plus spec_channels spectra of H bins per frame.  t gets its buffers and the call's constants; prev is
-// the two [n_pairs] halves the groups alternate between.  FRT_ENOMEM when it cannot grow (the handle
-// stays usable).
+// the two [n_pairs] halves the groups alternate between.
 static int gcc_track_workspace(frt_ctx *h, int n_pairs, int n_frames, int Lr, int spec_channels, int H,
                                GccTrack &t, int *&prev, GccSpectra &w, int &group) {
-    auto up = [](size_t b) { return (b + 255) & ~size_t(255); };
     const size_t P = (size_t)n_pairs, C = (size_t)spec_channels;
     const int nc = (Lr + GCC_TRACK_CHUNK - 1) / GCC_TRACK_CHUNK;
     const size_t per_frame = P * ((size_t)Lr * sizeof(float) + sizeof(int) +
                                   (size_t)nc * (sizeof(unsigned long long) + sizeof(double2))) +
                              C * ((size_t)H * sizeof(float2) + sizeof(int));
-    const size_t fixed = up(2 * P * sizeof(int)) + 7 * 256;
-    size_t g = GCC_TRACK_BUDGET > fixed ? (GCC_TRACK_BUDGET - fixed) / per_frame : 0;
-    g = g < 1 ? 1 : g > (size_t)n_frames ? (size_t)n_frames : g;
-    const size_t o_sil = up(g * P * Lr * sizeof(float)), o_best = o_sil + up(g * P * sizeof(int)),
-                 o_mom = o_best + up(g * P * nc * sizeof(unsigned long long)),
-                 o_prev = o_mom + up(g * P * nc * sizeof(double2)), o_spec = o_prev + up(2 * P * sizeof(int)),
-                 o_quiet = o_spec + up(g * C * H * sizeof(float2)), bytes = o_quiet + up(g * C * sizeof(int));
-    const cudaError_t e = h->gcc_track_ws.grow(bytes);
-    if (e == cudaErrorMemoryAllocation) {
-        cudaGetLastError();
-        return frt_fail(h, FRT_ENOMEM, "the workspace of one frame (%zu bytes) does not fit", per_frame);
-    }
-    FRT_CUDA(h, e);
+    const size_t fixed = WsLayout::round(2 * P * sizeof(int)) + 7 * 256;
+    const size_t g = frt_group_size(GCC_TRACK_BUDGET > fixed ? GCC_TRACK_BUDGET - fixed : 0, per_frame, n_frames);
+    WsLayout l;
+    const size_t o_xs = l.add(g * P * Lr * sizeof(float)), o_sil = l.add(g * P * sizeof(int)),
+                 o_best = l.add(g * P * nc * sizeof(unsigned long long)), o_mom = l.add(g * P * nc * sizeof(double2)),
+                 o_prev = l.add(2 * P * sizeof(int)), o_spec = l.add(g * C * H * sizeof(float2)),
+                 o_quiet = l.add(g * C * sizeof(int));
+    FRT_CUDA(h, h->gcc_track_ws.grow(l.bytes));
     unsigned char *ws = h->gcc_track_ws.get();
     t = GccTrack{};
-    t.xs = (float *)ws;
+    t.xs = (float *)(ws + o_xs);
     t.silent = (const int *)(ws + o_sil);
     t.best = (unsigned long long *)(ws + o_best);
     t.moments = (double2 *)(ws + o_mom);

@@ -278,14 +278,8 @@ static int spectrum_ticks_checks(frt_ctx *h, int n_channels, int frames_per_tick
 template <int NCH>
 static int spectrum_ticks_run(frt_ctx *h, SpecTicks t, int n_ticks, cudaStream_t st) {
     const size_t per_tick = NCH * (size_t)t.n_channels * t.nbins * sizeof(float);
-    size_t g = SPEC_TICKS_BUDGET / per_tick;
-    g = g < 1 ? 1 : g > (size_t)n_ticks ? (size_t)n_ticks : g;
-    const cudaError_t e = h->spec_ticks_ws.grow(g * per_tick);
-    if (e == cudaErrorMemoryAllocation) {
-        cudaGetLastError();
-        return frt_fail(h, FRT_ENOMEM, "the state rows of one tick (%zu bytes) do not fit", per_tick);
-    }
-    FRT_CUDA(h, e);
+    const size_t g = frt_group_size(SPEC_TICKS_BUDGET, per_tick, n_ticks);
+    FRT_CUDA(h, h->spec_ticks_ws.grow(g * per_tick));
     float *ws = (float *)h->spec_ticks_ws.get();
     for (int j = 0; j < NCH; j++) t.state[j] = ws + (size_t)j * g * t.n_channels * t.nbins;
     const long long items = (long long)t.n_channels * t.nbins;

@@ -1463,17 +1463,9 @@ extern "C" int frt_stft_process_host(frt_handle h, const float *x_host, int64_t 
     FRT_CHECK_ARG(h, x_stride >= n_samples, "x_stride smaller than n_samples");
     const int64_t frames = (n_samples - N) / hop + 1;
     // chunk = (channel group) x (frame range), sized to ~32 MiB of output per buffer
-    const size_t budget = (size_t)32 << 20;
-    int64_t fchunk = frames;
-    const size_t out_per_frame = sizeof(float) * nbins;
-    if ((size_t)fchunk * out_per_frame > budget) fchunk = (int64_t)(budget / out_per_frame);
-    if (fchunk < 1) fchunk = 1;
-    int cgroup = 1;
-    if (fchunk == frames) {
-        cgroup = (int)(budget / ((size_t)frames * out_per_frame));
-        if (cgroup < 1) cgroup = 1;
-        if (cgroup > n_channels) cgroup = n_channels;
-    }
+    const size_t budget = (size_t)32 << 20, out_per_frame = sizeof(float) * nbins;
+    const int64_t fchunk = (int64_t)frt_group_size(budget, out_per_frame, frames);
+    const int cgroup = fchunk == frames ? (int)frt_group_size(budget, frames * out_per_frame, n_channels) : 1;
     const int64_t chunk_samples = (fchunk - 1) * (int64_t)hop + N;
     StftStaging &p = h->stft_host;
     FRT_CUDA(h, p.create());

@@ -31,7 +31,10 @@ extern "C" {
 #define FRT_OK 0
 #define FRT_EINVAL (-1)   /* bad argument (shape, alignment, unsupported size)           */
 #define FRT_ECUDA (-2)    /* CUDA runtime error (message holds cudaGetErrorString)       */
-#define FRT_ENOMEM (-3)   /* host or device allocation failed                            */
+#define FRT_ENOMEM (-3)   /* host or device allocation failed: every entry point that
+                             allocates (plans, setters, grow-only workspaces, staging,
+                             frt_host_alloc, frt_peer_alloc) returns it when an
+                             allocation fails, and leaves the handle usable            */
 #define FRT_ESTATE (-4)   /* call order problem (e.g. process before plan)               */
 
 typedef struct frt_ctx *frt_handle;
@@ -263,7 +266,7 @@ int frt_gcc_set_pairs(frt_handle h, int n_channels, const int *pairs_host, int n
  * with the table (0,1), (2,3), ... the outputs are the same bits as frt_gcc_phat(x[0::2], x[1::2]).
  * The per-channel spectra take a grow-only workspace of about 8 * n_channels * (L'/2+1) bytes;
  * the Bluestein route also uses frt_gcc_phat's workspace for the transforms.  FRT_ESTATE without a
- * table or a plan; FRT_ENOMEM when the spectra do not fit on the device (the handle stays usable). */
+ * table or a plan.                                                                                 */
 int frt_gcc_phat_pairs(frt_handle h, const float *x_dev, int64_t stride, float *xcorr_dev,
                        float *smoothed_dev, int have_prev, int *idx_dev, float *val_dev, void *stream);
 /* frt_gcc_phat over n_frames frames of every pair in one call, with each frame's result kept: frame f
@@ -278,9 +281,9 @@ int frt_gcc_phat_pairs(frt_handle h, const float *x_dev, int64_t stride, float *
  * A pair silent in a frame (a constant input) gives (0, 0, 0) and keeps its smoothing row.  idx, val
  * and the final smoothed buffer are the same bits as n_frames frt_gcc_phat calls, one per frame.
  * Frames run in groups within a grow-only workspace of about 4*L' + 24*ceil(L'/2048) bytes per pair
- * and frame, kept within 2 GiB (one frame at least; FRT_ENOMEM, handle usable, when it cannot grow);
- * the Bluestein route also uses frt_gcc_phat's workspace, frame by frame.  n_frames = 0 or n_pairs = 0
- * does nothing; frame_stride >= 1 when n_frames > 1.                                              */
+ * and frame, kept within 2 GiB (one frame at least); the Bluestein route also uses frt_gcc_phat's
+ * workspace, frame by frame.  n_frames = 0 or n_pairs = 0 does nothing; frame_stride >= 1 when
+ * n_frames > 1.                                                                                    */
 int frt_gcc_phat_frames(frt_handle h, const float *d0_dev, const float *d1_dev, int64_t stride,
                         int64_t frame_stride, int n_frames, int n_pairs, float *smoothed_dev,
                         int have_prev, int *idx_dev, float *val_dev, double *std_dev, void *stream);
@@ -337,9 +340,8 @@ int frt_spectrum_reduce_dual(frt_handle h, const float *power1_dev, const float 
  * [n_ticks][C].  Every row, and disp_dev afterwards, are the same bits as n_ticks
  * frt_spectrum_reduce calls, one per tick.  Argument checks as frt_spectrum_reduce, with
  * frames_per_tick in 1..8192; n_ticks == 0 or n_channels == 0 does nothing.  The ticks run in groups
- * within a grow-only workspace of 4*C*nbins bytes per tick, kept within 256 MiB (one tick at least;
- * FRT_ENOMEM, handle usable, when it cannot grow); such a call is asynchronous on `stream` unless the
- * workspace has to grow.                                                                          */
+ * within a grow-only workspace of 4*C*nbins bytes per tick, kept within 256 MiB (one tick at least);
+ * such a call is asynchronous on `stream` unless the workspace has to grow.                       */
 int frt_spectrum_reduce_ticks(frt_handle h, const float *power_dev, int64_t stride_c,
                               int64_t stride_f, int n_channels, int frames_per_tick, int n_ticks,
                               int nbins, float alpha, float *disp_dev, const float *weight_dev,

@@ -3,7 +3,10 @@ files share.  Every kernel launch goes through frt_launch (friture_b200/csrc/frt
 sets the dynamic shared-memory limit, checks the launch and counts it; the fast log2 and the cp.async
 wrappers are defined there once.  So are frt_sync_copy and frt_sync_zero, the only synchronous copies
 and fills: they drain the device before and after, so that no kernel queued on any stream sees a plan,
-setter or reset that came after it, and no kernel launched next misses one that came before."""
+setter or reset that came after it, and no kernel launched next misses one that came before.  Every
+device allocation goes through frt_malloc, which clears a failure from the runtime's last error so
+that the next launch's check does not report it, and FRT_CUDA reports running out of memory as
+FRT_ENOMEM."""
 import os
 
 import pytest
@@ -22,6 +25,9 @@ ONLY_IN_HOME = [
     "wait_group",               # cp_async_wait<N>
     "cudaMemcpy(",              # frt_sync_copy
     "cudaMemset(",              # frt_sync_zero
+    "cudaMalloc(",              # frt_malloc
+    "cudaGetLastError",         # frt_launch's check, and frt_alloc_status clearing a failed allocation
+    "cudaErrorMemoryAllocation",   # FRT_CUDA reports it as FRT_ENOMEM
 ]
 
 
