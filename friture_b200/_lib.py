@@ -121,6 +121,17 @@ SIGNATURES = {
                                      c_float, c_void_p, c_void_p, c_int, c_void_p, c_int64, c_int64, c_void_p]),
     "frt_display_rows": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int, c_int, c_int, c_void_p, c_void_p,
                                  c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "frt_levels_plan": (c_int, [c_void_p, c_int, c_int, c_void_p, c_double, c_double, c_double]),
+    "frt_levels_reset": (c_int, [c_void_p]),
+    "frt_levels_state": (c_int, [c_void_p, c_void_p, c_void_p]),
+    "frt_levels_process": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_void_p, c_void_p, c_void_p,
+                                   c_void_p]),
+    "frt_longlevels_plan": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    "frt_longlevels_reset": (c_int, [c_void_p]),
+    "frt_longlevels_process": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_void_p, c_void_p, c_void_p,
+                                       c_int64, c_int64, c_void_p]),
+    "frt_longlevels_history": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int, c_int, c_double,
+                                       c_double, c_void_p, c_void_p]),
 }
 
 _lib = None

@@ -167,12 +167,16 @@ struct DecPlan;    // bank.cu
 struct FirPlan;    // bank_fir.cu
 struct GccPlan;    // gcc_phat.cu
 struct GccLongPlan;   // gcc_long.cu
+struct LevelsPlan;    // levels.cu
+struct LongLevelsPlan;   // levels.cu
 struct PlanDelete {
     void operator()(BankPlan *p) const;
     void operator()(DecPlan *p) const;
     void operator()(FirPlan *p) const;
     void operator()(GccPlan *p) const;
     void operator()(GccLongPlan *p) const;
+    void operator()(LevelsPlan *p) const;
+    void operator()(LongLevelsPlan *p) const;
 };
 template <class Plan>
 using PlanPtr = std::unique_ptr<Plan, PlanDelete>;
@@ -219,6 +223,8 @@ struct frt_ctx {
     int gcc_pairs_channels = 0;       // the channels of the input it indexes
     DeviceArray<unsigned char> gcc_spec_ws;   // frt_gcc_phat_pairs' per-channel spectra, grow-only
     DeviceArray<unsigned char> gcc_track_ws;  // frt_gcc_phat_frames / _pairs_frames' frame groups, grow-only
+    PlanPtr<LevelsPlan> levels;       // the meter's buffer weights and per-channel state
+    PlanPtr<LongLevelsPlan> longlevels;   // the long-term levels' filter taps and per-channel state
     DeviceArray<unsigned char> spec_ticks_ws;  // frt_spectrum_reduce_ticks / _dual_ticks' state rows, grow-only
     StftStaging stft_host;
     CombStaging comb_host;

@@ -439,6 +439,58 @@ int frt_display_rows(frt_handle h, const float *rows_dev, int64_t stride_c, int6
                      const float *out_a_dev, int n_out, float *old_data_dev, const uint32_t *lut_dev,
                      uint32_t *pixels_dev, void *stream);
 
+/* ---------------------------------------------------------------- level meter
+ * Levels_Widget.handle_new_data (friture/levels.py:84-131) for every one of C channels, with the
+ * ballistic peak of its display (BallisticPeak.peak_iec, friture/ballistic_peak.py:43-66, of
+ * dB_to_IEC(max(level_max, level_rms)), friture/iec.py).  Each buffer of `buffer` samples is one
+ * handle_new_data call.  frt_levels_plan takes the buffer length, the tail of the widget's
+ * smoothing kernel, weights_host[j] = kernel[Nk - buffer + j] (exp_smoothing.py:41-51), alpha, decay =
+ * (1 - alpha)^buffer and keep = 1 - alpha2 (levels.py:58-74), all computed by the caller as the widget
+ * does.  The per-channel state (old_rms, old_max, the ballistic peak, its decay factor and hold
+ * counter) starts from the widget's (1e-30, 1e-30, 0, 1 - 3e-6/500, 0); a plan with the planned
+ * channel count keeps it.  frt_levels_reset starts it again.                                  */
+int frt_levels_plan(frt_handle h, int n_channels, int buffer, const double *weights_host, double alpha,
+                    double decay, double keep);
+int frt_levels_reset(frt_handle h);
+/* The state after the last call: state_host [4][C] double (old_rms, old_max, peak, decay factor),
+ * hold_host [C] int.  Waits for the device.                                                     */
+int frt_levels_state(frt_handle h, double *state_host, int *hold_host);
+/* n_buffers consecutive buffers of every channel, x_dev[c*x_stride + r*buffer .. + buffer), in one
+ * launch: rms_db_dev / max_db_dev / peak_iec_dev [C][n_buffers] double get level_rms, level_max and
+ * peak_iec after each buffer.  max|x|, the peak state and the ballistic peak are the widget's
+ * double arithmetic bit for bit; the weighted sum of x^2 and log10 may differ from NumPy's by
+ * rounding.  A NaN sample acts as in the widget: max|x| is NaN, so old_max takes its decay step,
+ * and old_rms and level_rms become NaN.  x_stride >= n_buffers*buffer unless C == 1.            */
+int frt_levels_process(frt_handle h, const float *x_dev, int64_t x_stride, int n_buffers, double *rms_db_dev,
+                       double *max_db_dev, double *peak_iec_dev, void *stream);
+
+/* ---------------------------------------------------------------- long-term levels
+ * LongLevelWidget.handle_new_data and setresptime (friture/longlevels.py:150-230) for C channels:
+ * per block of 2^n_dec samples, x^2 through n_dec stages of decimate (friture/signal/decimate.py:
+ * 27-42: bdec_host, the 11 taps of gauss(11, 2), then every other output) and the 41-tap FIR
+ * bfir_host = gauss(41, 8), one linear level per block, and 10*log10(max(level, 1e-150)).  The
+ * filters are lfilter_float64_1D with a = [1, 0, ...] (friture/signal/lfilter.py:132-139) evaluated in
+ * its order, so the linear level is the same bits.  The plan and frt_longlevels_reset zero the
+ * filter state, as setresptime does (longlevels.py:207-221).  n_dec in 1..13.                   */
+int frt_longlevels_plan(frt_handle h, int n_channels, int n_dec, const double *bdec_host,
+                        const double *bfir_host);
+int frt_longlevels_reset(frt_handle h);
+/* n_blocks consecutive blocks, x_dev[c*x_stride + b*2^n_dec .. + 2^n_dec), in one launch:
+ * level_dev / db_dev [C][n_blocks] double get each block's linear level and dB, and
+ * ring_dev[c*ring_len + (ring_pos + b) % ring_len] (float32) its dB: the widget's level ring
+ * buffer (friture/ringbuffer.py:39-61) whose offset is ring_pos.  A NaN or infinite sample acts as
+ * in the widget: its transposed-form filters take y*0 into their state, so from the sample's block
+ * on the channel's levels are NaN (max(level, 1e-150) keeps NaN) until the next plan or reset.
+ * x_stride >= n_blocks*2^n_dec unless C == 1.                                                  */
+int frt_longlevels_process(frt_handle h, const float *x_dev, int64_t x_stride, int n_blocks, double *level_dev,
+                           double *db_dev, float *ring_dev, int64_t ring_len, int64_t ring_pos, void *stream);
+/* The plotted curve (longlevels.py:181-187): scaled_dev [C][length] float32 = clip(1 - (l -
+ * level_min) / (level_max - level_min), 0, 1) of the last `length` ring values before offset
+ * ring_pos (RingBuffer.data, ringbuffer.py:63-78), in double.  length <= ring_len.              */
+int frt_longlevels_history(frt_handle h, const float *ring_dev, int64_t ring_len, int64_t ring_pos,
+                           int n_channels, int length, double level_min, double level_max,
+                           float *scaled_dev, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
