@@ -132,6 +132,8 @@ SIGNATURES = {
                                        c_int64, c_int64, c_void_p]),
     "frt_longlevels_history": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int, c_int, c_double,
                                        c_double, c_void_p, c_void_p]),
+    "frt_scope_process": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int64, c_int, c_int, c_int,
+                                  c_int, c_int64, c_void_p, c_void_p, c_int64, c_double, c_void_p, c_void_p]),
 }
 
 _lib = None

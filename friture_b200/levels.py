@@ -45,6 +45,24 @@ def _check_rows(x, n_channels, name):
     return x
 
 
+def grow_ring(ring, offset, length):
+    """RingBuffer.grow_if_needed (ringbuffer.py:105-130) on ring [rows, old], a device tensor whose slot
+    p % old holds stream position p, after `offset` positions were pushed.  When length > old, the value
+    in slot s moves to slot (s + shift) % new of a zeroed ring of new = int(1.5 * length) slots, shift =
+    (offset % new - offset % old) % new.  Returns (ring, its length)."""
+    import torch
+    old = ring.shape[1]
+    if length <= old:
+        return ring, old
+    new = int(1.5 * length)
+    shift = (offset % new - offset % old) % new
+    grown = torch.zeros((ring.shape[0], new), dtype=ring.dtype, device=ring.device)
+    direct = min(old, new - shift)
+    grown[:, shift:shift + direct] = ring[:, :direct]
+    grown[:, :old - direct] = ring[:, direct:old]
+    return grown, new
+
+
 class LevelTicks(NamedTuple):
     """One column per buffer of the call, CUDA float64 [C, R]: the widget's ``level_rms`` and
     ``level_max`` (dB) and the ballistic ``peak_iec`` after that buffer."""
@@ -239,19 +257,7 @@ class LongLevelsAnalyzer:
         self._plan_ndec = self.Ndec
 
     def _grow_if_needed(self, length):
-        """RingBuffer.grow_if_needed (ringbuffer.py:101-127): the value in slot s moves to slot
-        (s + shift) % new of a zeroed ring, shift = (offset % new - offset % old) % new."""
-        import torch
-        old = self._ring_len
-        if length <= old:
-            return
-        new = int(1.5 * length)
-        shift = (self._ring_pos % new - self._ring_pos % old) % new
-        ring = torch.zeros((self.n_channels, new), dtype=torch.float32, device=self._ring.device)
-        direct = min(old, new - shift)
-        ring[:, shift:shift + direct] = self._ring[:, :direct]
-        ring[:, :old - direct] = self._ring[:, direct:old]
-        self._ring, self._ring_len = ring, new
+        self._ring, self._ring_len = grow_ring(self._ring, self._ring_pos, length)
 
     def handle_new_data(self, chunk, stream=None):
         """chunk: CUDA float32 [C, n] (or [T] for one channel), any row stride and any length.

@@ -491,6 +491,28 @@ int frt_longlevels_history(frt_handle h, const float *ring_dev, int64_t ring_len
                            int n_channels, int length, double level_min, double level_max,
                            float *scaled_dev, void *stream);
 
+/* ---------------------------------------------------------------- scope
+ * Scope_Widget.handle_new_data (friture/scope.py:78-133) for n_scopes scopes of n_ch (1 or 2)
+ * channels: row s*n_ch + k of x_dev is channel k of scope s, x_stride floats apart.  Tick r (0 <=
+ * r < n_ticks) reads the `need` samples that end at column lead + (r+1)*buffer, need = 2*width in
+ * trigger mode (trigger != 0) and width in scrolling mode; lead + buffer >= need.  The caller stages
+ * each row as the widget's ring buffer reads it, so column c is stream index origin + c.
+ *   trigger: level = max(s) * 2 / 3 of the search window s = d[width/2 .. width/2 + width) of
+ *     channel 0, a NaN anywhere making it NaN; the first i with s[i] < level <= s[i+1], compared in
+ *     double; the tick draws 2*(width/2) samples from d[i].  No such i: the tick draws nothing.
+ *   scrolling: the tick draws the last width samples.
+ * start_dev [n_scopes][n_ticks] int64 gets the stream index each tick's drawn window starts at
+ * (negative when it reaches into the zeros before the stream), or INT64_MIN when it drew nothing.
+ * For each scope whose ticks drew, the last one that drew gives curve_dev[(s*n_ch + k)*curve_stride
+ * + j] = float32(1 - (y + 1) / 2) in double (scope.py:128-133), j < its point count, and drawn_dev[s]
+ * = timerange; the other scopes' curves and drawn_dev are left alone.  Two launches; every
+ * refusal comes before the first.  x_stride >= lead + n_ticks*buffer and curve_stride >= the point
+ * count unless n_scopes*n_ch == 1.  In trigger mode width/buffer is at most 25 000.             */
+int frt_scope_process(frt_handle h, const float *x_dev, int64_t x_stride, int n_scopes, int n_ch, int64_t lead,
+                      int n_ticks, int buffer, int width, int trigger, int64_t origin, int64_t *start_dev,
+                      float *curve_dev, int64_t curve_stride, double timerange, double *drawn_dev,
+                      void *stream);
+
 #ifdef __cplusplus
 }
 #endif
